@@ -62,6 +62,9 @@ ASTC_FN void rgba_unpack(i4 in0, i4 in1, i4& out0, i4& out1) {   // :105-135
 // unpack_color_endpoints (astcenc_color_unquantize.cpp:844-1022)
 // (the _inl form lets a caller keep the results in registers: reference parameters of an out-of-line function force the
 // caller's variables into local memory)
+// LDR_ONLY: the caller decodes in an LDR profile, so the HDR unpackers are left out. An HDR format still ends as the error
+// colour below, exactly as in the general form (an LDR decode replaces any HDR endpoint pair by it).
+template <bool LDR_ONLY = false>
 ASTC_FN void unpack_color_endpoints_inl(int decode_mode, int format, const uint8_t* in, bool& rgb_hdr, bool& alpha_hdr, i4& o0, i4& o1) {
 	rgb_hdr = false;
 	alpha_hdr = false;
@@ -81,11 +84,13 @@ ASTC_FN void unpack_color_endpoints_inl(int decode_mode, int format, const uint8
 		break;
 	}
 	case FMT_HDR_LUMINANCE_SMALL_RANGE:
+		if (LDR_ONLY) { rgb_hdr = true; o0 = o1 = mki4(0, 0, 0, 0); break; }
 		rgb_hdr = true;
 		alpha_hdr_default = true;
 		hdr_luminance_small_range_unpack(in, o0, o1);
 		break;
 	case FMT_HDR_LUMINANCE_LARGE_RANGE:
+		if (LDR_ONLY) { rgb_hdr = true; o0 = o1 = mki4(0, 0, 0, 0); break; }
 		rgb_hdr = true;
 		alpha_hdr_default = true;
 		hdr_luminance_large_range_unpack(in, o0, o1);
@@ -127,6 +132,7 @@ ASTC_FN void unpack_color_endpoints_inl(int decode_mode, int format, const uint8
 		break;
 	}
 	case FMT_HDR_RGB_SCALE:
+		if (LDR_ONLY) { rgb_hdr = true; o0 = o1 = mki4(0, 0, 0, 0); break; }
 		rgb_hdr = true;
 		alpha_hdr_default = true;
 		hdr_rgbo_unpack(in, o0, o1);
@@ -142,6 +148,7 @@ ASTC_FN void unpack_color_endpoints_inl(int decode_mode, int format, const uint8
 		o1.w = 255;
 		break;
 	case FMT_HDR_RGB:
+		if (LDR_ONLY) { rgb_hdr = true; o0 = o1 = mki4(0, 0, 0, 0); break; }
 		rgb_hdr = true;
 		alpha_hdr_default = true;
 		hdr_rgb_unpack(in, o0, o1);
@@ -153,12 +160,14 @@ ASTC_FN void unpack_color_endpoints_inl(int decode_mode, int format, const uint8
 		rgba_delta_unpack(mki4(in[0], in[2], in[4], in[6]), mki4(in[1], in[3], in[5], in[7]), o0, o1);
 		break;
 	case FMT_HDR_RGB_LDR_ALPHA:
+		if (LDR_ONLY) { rgb_hdr = true; o0 = o1 = mki4(0, 0, 0, 0); break; }
 		rgb_hdr = true;
 		hdr_rgb_unpack(in, o0, o1);
 		o0.w = in[6];
 		o1.w = in[7];
 		break;
 	case FMT_HDR_RGBA: {
+		if (LDR_ONLY) { rgb_hdr = true; o0 = o1 = mki4(0, 0, 0, 0); break; }
 		rgb_hdr = true;
 		alpha_hdr = true;
 		hdr_rgb_unpack(in, o0, o1);
@@ -250,7 +259,8 @@ struct QEnds {
 	bool ok;
 };
 
-ASTC_NOINLINE QEnds quantize_rgb_v(f4 c0, f4 c1, QuantCtx q) {   // :169-193
+// (each out-of-line quantiser below is also instantiated inline, _inl, by the one-partition LDR refinement step)
+ASTC_FN QEnds quantize_rgb_inl(f4 c0, f4 c1, QuantCtx q) {   // :169-193
 	i4 c0i, c1i;
 	do {
 		i4 a = f4_to_i4_rtn(c0);
@@ -268,6 +278,7 @@ ASTC_NOINLINE QEnds quantize_rgb_v(f4 c0, f4 c1, QuantCtx q) {   // :169-193
 	r.ok = true;
 	return r;
 }
+ASTC_NOINLINE QEnds quantize_rgb_v(f4 c0, f4 c1, QuantCtx q) { return quantize_rgb_inl(c0, c1, q); }
 ASTC_FN void quantize_rgb(f4 c0, f4 c1, i4& o0, i4& o1, QuantCtx q) {
 	QEnds r = quantize_rgb_v(c0, c1, q);
 	o0 = r.a;
@@ -290,7 +301,7 @@ ASTC_FN f4 blue_contract_fwd(f4 c) {   // c += c - c.bbba
 	return mk4(c.x + (c.x - c.z), c.y + (c.y - c.z), c.z + (c.z - c.z), c.w + (c.w - c.w));
 }
 
-ASTC_NOINLINE QEnds try_quantize_rgb_blue_contract_v(f4 c0, f4 c1, QuantCtx q) {   // :237-267
+ASTC_FN QEnds try_quantize_rgb_blue_contract_inl(f4 c0, f4 c1, QuantCtx q) {   // :237-267
 	QEnds r;
 	r.a = r.b = mki4(0, 0, 0, 0);
 	r.ok = false;
@@ -309,6 +320,7 @@ ASTC_NOINLINE QEnds try_quantize_rgb_blue_contract_v(f4 c0, f4 c1, QuantCtx q) {
 	r.ok = true;
 	return r;
 }
+ASTC_NOINLINE QEnds try_quantize_rgb_blue_contract_v(f4 c0, f4 c1, QuantCtx q) { return try_quantize_rgb_blue_contract_inl(c0, c1, q); }
 // (a failed attempt leaves o0 / o1 untouched, like the reference)
 ASTC_FN bool try_quantize_rgb_blue_contract(f4 c0, f4 c1, i4& o0, i4& o1, QuantCtx q) {
 	QEnds r = try_quantize_rgb_blue_contract_v(c0, c1, q);
@@ -329,7 +341,7 @@ ASTC_FN bool try_quantize_rgba_blue_contract(f4 c0, f4 c1, i4& o0, i4& o1, Quant
 }
 
 // common body of try_quantize_rgb_delta (:321-400) and ..._delta_blue_contract (:403-488)
-ASTC_NOINLINE QEnds rgb_delta_core_v(f4 c0, f4 c1, QuantCtx q, bool want_negative_sum) {
+ASTC_FN QEnds rgb_delta_core_inl(f4 c0, f4 c1, QuantCtx q, bool want_negative_sum) {
 	QEnds res;
 	res.a = res.b = mki4(0, 0, 0, 0);
 	res.ok = false;
@@ -365,6 +377,7 @@ ASTC_NOINLINE QEnds rgb_delta_core_v(f4 c0, f4 c1, QuantCtx q, bool want_negativ
 	res.ok = true;
 	return res;
 }
+ASTC_NOINLINE QEnds rgb_delta_core_v(f4 c0, f4 c1, QuantCtx q, bool want_negative_sum) { return rgb_delta_core_inl(c0, c1, q, want_negative_sum); }
 ASTC_FN bool rgb_delta_core(f4 c0, f4 c1, i4& o0, i4& o1, QuantCtx q, bool want_negative_sum) {
 	QEnds r = rgb_delta_core_v(c0, c1, q, want_negative_sum);
 	if (r.ok) {
@@ -392,7 +405,7 @@ struct QAlpha {
 	int a0, a1;
 	bool ok;
 };
-ASTC_NOINLINE QAlpha try_quantize_alpha_delta_v(f4 c0, f4 c1, QuantCtx q) {   // :504-570
+ASTC_FN QAlpha try_quantize_alpha_delta_inl(f4 c0, f4 c1, QuantCtx q) {   // :504-570
 	QAlpha res;
 	res.a0 = res.a1 = 0;
 	res.ok = false;
@@ -429,6 +442,7 @@ ASTC_NOINLINE QAlpha try_quantize_alpha_delta_v(f4 c0, f4 c1, QuantCtx q) {   //
 	res.ok = true;
 	return res;
 }
+ASTC_NOINLINE QAlpha try_quantize_alpha_delta_v(f4 c0, f4 c1, QuantCtx q) { return try_quantize_alpha_delta_inl(c0, c1, q); }
 ASTC_FN bool try_quantize_alpha_delta(f4 c0, f4 c1, i4& o0, i4& o1, QuantCtx q) {
 	QAlpha r = try_quantize_alpha_delta_v(c0, c1, q);
 	if (r.ok) {
@@ -673,7 +687,8 @@ ASTC_NOINLINE uint8_t pack_hdr_endpoints(int lane, f4 color0, f4 color1, f4 rgbo
 // smallest round-trip error wins, the earlier one on a tie. For a single-partition candidate the four run on four lanes
 // (the two offset forms share their instruction stream, as do the four round-trip error evaluations); the winner stores
 // the bytes. `output` is shared memory, every lane passes the same arguments, the caller synchronises.
-ASTC_NOINLINE uint8_t pack_rgb_endpoints_coop(int lane, f4 color0, f4 color1, int format, uint8_t* output, int quant_level) {
+// INL: the quantisers are inlined (the one-partition LDR refinement step) instead of called
+template <bool INL> ASTC_FN uint8_t pack_rgb_endpoints_coop_t(int lane, f4 color0, f4 color1, int format, uint8_t* output, int quant_level) {
 	QuantCtx q;
 	q.tab = STAGED.cq_smem_off != 0 ? astc_smem + STAGED.cq_smem_off + 512 * (quant_level - QUANT_6)
 	                                : ASTC_CT->color_unquant_to_uquant[quant_level - QUANT_6];
@@ -705,19 +720,19 @@ ASTC_NOINLINE uint8_t pack_rgb_endpoints_coop(int lane, f4 color0, f4 color1, in
 				ok = in_0_255(a) && in_0_255(b);
 			}
 			if (ok) {
-				QEnds r = rgb_delta_core_v(a, b, q, bc);
+				QEnds r = INL ? rgb_delta_core_inl(a, b, q, bc) : rgb_delta_core_v(a, b, q, bc);
 				ok = r.ok;
 				o0 = r.a;
 				o1 = r.b;
 			}
 			if (ok && has_a) {
-				QAlpha ra = try_quantize_alpha_delta_v(bc ? c1l : c0l, bc ? c0l : c1l, q);
+				QAlpha ra = INL ? try_quantize_alpha_delta_inl(bc ? c1l : c0l, bc ? c0l : c1l, q) : try_quantize_alpha_delta_v(bc ? c1l : c0l, bc ? c0l : c1l, q);
 				ok = ra.ok;
 				o0.w = ra.a0;
 				o1.w = ra.a1;
 			}
 		} else if (k == 2) {
-			QEnds r = try_quantize_rgb_blue_contract_v(c0l, c1l, q);
+			QEnds r = INL ? try_quantize_rgb_blue_contract_inl(c0l, c1l, q) : try_quantize_rgb_blue_contract_v(c0l, c1l, q);
 			ok = r.ok;
 			o0 = r.a;
 			o1 = r.b;
@@ -726,7 +741,7 @@ ASTC_NOINLINE uint8_t pack_rgb_endpoints_coop(int lane, f4 color0, f4 color1, in
 				o1.w = quant_color_f(q, f2i_rtn(c0l.w), c0l.w);
 			}
 		} else {
-			QEnds r = quantize_rgb_v(c0l, c1l, q);
+			QEnds r = INL ? quantize_rgb_inl(c0l, c1l, q) : quantize_rgb_v(c0l, c1l, q);
 			ok = true;
 			o0 = r.a;
 			o1 = r.b;
@@ -783,4 +798,7 @@ ASTC_NOINLINE uint8_t pack_rgb_endpoints_coop(int lane, f4 color0, f4 color1, in
 		}
 	}
 	return (uint8_t)(best_k < 2 ? (has_a ? FMT_RGBA_DELTA : FMT_RGB_DELTA) : (has_a ? FMT_RGBA : FMT_RGB));
+}
+ASTC_NOINLINE uint8_t pack_rgb_endpoints_coop(int lane, f4 color0, f4 color1, int format, uint8_t* output, int quant_level) {
+	return pack_rgb_endpoints_coop_t<false>(lane, color0, color1, format, output, quant_level);
 }

@@ -25,12 +25,15 @@ ASTC_FN void quantize_candidate_weights_to(const WCtx& w, SPtr<uint8_t> dst, int
 		dst[pl * 32 + k] = (uint8_t)quantize_weight(z, dwi[id]);
 	}
 }
-ASTC_COOP void quantize_candidate_weights(WCtx w, int decimation_mode, int quant_mode, int nplanes, float cutoff1, float cutoff2) {
+ASTC_FN void quantize_candidate_weights_t(const WCtx& w, int decimation_mode, int quant_mode, int nplanes, float cutoff1, float cutoff2) {
 	quantize_candidate_weights_to(w, work_weights_of(w), decimation_mode, quant_mode, nplanes, cutoff1, cutoff2);
 	wsync();
 }
+ASTC_COOP void quantize_candidate_weights(WCtx w, int decimation_mode, int quant_mode, int nplanes, float cutoff1, float cutoff2) {
+	quantize_candidate_weights_t(w, decimation_mode, quant_mode, nplanes, cutoff1, cutoff2);
+}
 
-ASTC_COOP void copy_work_to_best(WCtx w) {
+ASTC_FN void copy_work_to_best_t(const WCtx& w) {
 	// best_weights[64] best_colors[32] | work_weights[64] work_colors[32]: one word per lane
 	SPtr<uint32_t> dst = sptr<uint32_t>(w.base + A_SCB);
 	SPtr<uint32_t> src = sptr<uint32_t>(w.base + A_SCB + 96);
@@ -40,11 +43,16 @@ ASTC_COOP void copy_work_to_best(WCtx w) {
 	}
 	wsync();
 }
+ASTC_COOP void copy_work_to_best(WCtx w) {
+	copy_work_to_best_t(w);
+}
 
 // Pack the endpoints of partitions 0..pc-1 of the work candidate at quant_level into colors (work_colors or
 // mod_colors). LDR formats: lanes over partitions; HDR formats: one partition after the other, the warp running the
 // format's sub-mode ladder lane-parallel. The resulting formats come back packed 8 bits each (exchanged via tmpf).
-ASTC_COOP uint32_t pack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats_in, int quant_level, uint32_t colors_off) {
+// L1: one partition and LDR formats are compile-time facts; the RGB / RGBA contest is inlined, the HDR packers are left out.
+template <bool L1> ASTC_FN uint32_t pack_work_endpoints_t(const WCtx& w, unsigned int pc_in, uint32_t formats_in, int quant_level, uint32_t colors_off) {
+	const unsigned int pc = L1 ? 1u : pc_in;
 	SPtr<f4> ep = ep_of(w);
 	SPtr<uint8_t> colors = sptr<uint8_t>(colors_off);
 	SPtr<uint32_t> colors32 = sptr<uint32_t>(colors_off);
@@ -62,7 +70,8 @@ ASTC_COOP uint32_t pack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats
 	const bool rgb_coop = pc == 1 && (fmt0 == FMT_RGB || fmt0 == FMT_RGBA);
 #endif
 	if (rgb_coop) {
-		uint8_t fmt = pack_rgb_endpoints_coop(w.lane, ep[EP_WORK_0], ep[EP_WORK_1], fmt0, &colors[0], quant_level);
+		uint8_t fmt = L1 ? pack_rgb_endpoints_coop_t<true>(w.lane, ep[EP_WORK_0], ep[EP_WORK_1], fmt0, &colors[0], quant_level)
+		                 : pack_rgb_endpoints_coop(w.lane, ep[EP_WORK_0], ep[EP_WORK_1], fmt0, &colors[0], quant_level);
 		if (w.lane == 0) {
 			xch[0] = fmt;
 		}
@@ -70,7 +79,7 @@ ASTC_COOP uint32_t pack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats
 	ASTC_NOUNROLL
 	for (unsigned int j = (unsigned int)w.lane; j < pc && !rgb_coop; j += ASTC_WARP) {
 		int fmt_in = (int)((formats_in >> (8 * j)) & 0xFF);
-		if (!is_hdr_format(fmt_in)) {
+		if (L1 || !is_hdr_format(fmt_in)) {
 			// (packed straight into the shared arena: a local byte array behind a pointer would live in local memory)
 			xch[(int)j] = pack_color_endpoints(ep[EP_WORK_0 + (int)j], ep[EP_WORK_1 + (int)j], ep[EP_RGBS + (int)j], ep[EP_RGBO + (int)j], fmt_in, &colors[(int)j * 8], quant_level);
 		}
@@ -78,7 +87,7 @@ ASTC_COOP uint32_t pack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats
 	ASTC_NOUNROLL
 	for (unsigned int j = 0; j < pc; j++) {
 		int fmt_in = (int)((formats_in >> (8 * j)) & 0xFF);
-		if (is_hdr_format(fmt_in)) {
+		if (!L1 && is_hdr_format(fmt_in)) {
 			uint8_t fmt = pack_hdr_endpoints(w.lane, ep[EP_WORK_0 + (int)j], ep[EP_WORK_1 + (int)j], ep[EP_RGBO + (int)j], fmt_in, &colors[(int)j * 8], quant_level);
 			if (w.lane == 0) {
 				xch[(int)j] = fmt;
@@ -94,6 +103,9 @@ ASTC_COOP uint32_t pack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats
 	}
 	wsync();
 	return r;
+}
+ASTC_COOP uint32_t pack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats_in, int quant_level, uint32_t colors_off) {
+	return pack_work_endpoints_t<false>(w, pc, formats_in, quant_level, colors_off);
 }
 
 ASTC_FN void set_formats(ScbHdr& h, uint32_t f) {

@@ -486,8 +486,13 @@ ASTC_FN void refine_begin_trial(const WCtx& w, const Trial& t, Refine& r, const 
 	ST_WRITE_END(w)
 }
 
+// The refinement step exists in two instantiations of the same source. L1 = false: the general step, every part an
+// out-of-line function that reads the trial's shape (partitions, planes, HDR formats) at run time. L1 = true: the trial has
+// one partition, one plane and an LDR profile (so LDR endpoint formats) - compile-time facts, and every part of the step is
+// inlined into its caller with the two-plane, n-partition and HDR branches folded away.
+
 // start candidate r.i (quantise its weights, reset the work endpoints): the part of the candidate loop before `for l`
-ASTC_COOP void refine_begin_candidate(WCtx w, const Trial& t, Refine& r) {
+template <bool L1> ASTC_FN void refine_begin_candidate_t(const WCtx& w, const Trial& t, Refine& r) {
 	unsigned int ci = r.i;
 	bool from_candw = r.from_candw;
 	Candidate cd = cand_of(w)[(int)ci];
@@ -502,6 +507,8 @@ ASTC_COOP void refine_begin_candidate(WCtx w, const Trial& t, Refine& r) {
 		for (int k = w.lane; k < 16; k += ASTC_WARP) {
 			ww[k] = cw[k];
 		}
+	} else if (L1) {
+		quantize_candidate_weights_t(w, dmode, qmode, 1, t.cutoff1, t.cutoff2);
 	} else {
 		quantize_candidate_weights(w, dmode, qmode, t.dual ? 2 : 1, t.cutoff1, t.cutoff2);
 	}
@@ -530,40 +537,58 @@ ASTC_COOP void refine_begin_candidate(WCtx w, const Trial& t, Refine& r) {
 		r.work.constant_color[0] = r.work.constant_color[1] = r.work.constant_color[2] = r.work.constant_color[3] = 0;
 	ST_WRITE_END(w)
 }
+ASTC_COOP void refine_begin_candidate(WCtx w, const Trial& t, Refine& r) {
+	refine_begin_candidate_t<false>(w, t, r);
+}
+
+// the trial's partitioning (L1: the single partition)
+template <bool L1> ASTC_FN PartView refine_part_view(const Trial& t) {
+	return L1 ? part_view_packed(1, 0) : part_view_packed(t.partition_count, t.packed);
+}
 
 // step part 1: refit the endpoint colours
-ASTC_COOP void refine_recompute(WCtx w, const Trial& t, Refine& r) {
+template <bool L1> ASTC_FN void refine_recompute_t(const WCtx& w, const Trial& t, Refine& r) {
 	bool first = r.l == 0;
 	ST_WRITE_BEGIN(w)
 		r.in_step = true;
 	ST_WRITE_END(w)
 	if (first) {
-		refine_begin_candidate(w, t, r);
+		if (L1) {
+			refine_begin_candidate_t<true>(w, t, r);
+		} else {
+			refine_begin_candidate(w, t, r);
+		}
 	}
-	if (t.dual) {
+	if (!L1 && t.dual) {
 		recompute_ideal_colors_2planes(w, (unsigned int)r.dmode, t.plane2_component);
+	} else if (L1) {
+		recompute_ideal_colors_1plane_t<true>(w, refine_part_view<true>(t), (unsigned int)r.dmode);
 	} else {
 		PartView pi = part_view_packed(t.partition_count, t.packed);
 		recompute_ideal_colors_1plane(w, pi, (unsigned int)r.dmode);
 	}
 }
+ASTC_COOP void refine_recompute(WCtx w, const Trial& t, Refine& r) {
+	refine_recompute_t<false>(w, t, r);
+}
 
 // step part 2: quantise the endpoints (with the matched-format retry of :560-601)
-ASTC_COOP void refine_pack(WCtx w, const Trial& t, Refine& r) {
+template <bool L1> ASTC_FN void refine_pack_t(const WCtx& w, const Trial& t, Refine& r) {
 	uint32_t cd_formats = r.cd_formats;
 	int quant_level = r.quant_level, quant_level_mod = r.quant_level_mod;
 	uint16_t mode_index = r.mode_index;
-	int dual = t.dual;
-	unsigned int partition_count = dual ? 1u : t.partition_count;
-	unsigned int partition_index = dual ? 0u : t.partition_index;
-	int plane2_component = dual ? t.plane2_component : -1;
+	int dual = L1 ? 0 : t.dual;
+	unsigned int partition_count = L1 ? 1u : (dual ? 1u : t.partition_count);
+	unsigned int partition_index = L1 ? 0u : (dual ? 0u : t.partition_index);
+	int plane2_component = dual ? t.plane2_component : -1;      // (L1: folds to -1)
 	uint32_t formats;
 	int matched = 0;
 	if (dual) {
 		formats = pack_work_endpoints(w, 1, cd_formats, quant_level, work_colors_of(w).off);
 		formats &= 0xFF;
 	} else {
-		formats = pack_work_endpoints(w, partition_count, cd_formats, quant_level, work_colors_of(w).off);
+		formats = L1 ? pack_work_endpoints_t<true>(w, 1, cd_formats, quant_level, work_colors_of(w).off)
+		             : pack_work_endpoints(w, partition_count, cd_formats, quant_level, work_colors_of(w).off);
 		bool all_same = quant_level != quant_level_mod;
 		for (unsigned int j = 1; j < 4; j++) {
 			if (j < partition_count) {
@@ -610,11 +635,21 @@ ASTC_COOP void refine_pack(WCtx w, const Trial& t, Refine& r) {
 		r.formats = formats;
 	ST_WRITE_END(w)
 	// integer endpoints of the packed candidate, once per step: both scores and the realignment read them
-	unpack_work_endpoints(w, partition_count, formats, ends_off_of(w));
+	if (L1) {
+		unpack_work_endpoints_t<true>(w, 1, formats, ends_off_of(w));
+	} else {
+		unpack_work_endpoints(w, partition_count, formats, ends_off_of(w));
+	}
+}
+ASTC_COOP void refine_pack(WCtx w, const Trial& t, Refine& r) {
+	refine_pack_t<false>(w, t, r);
 }
 
-ASTC_FN float refine_score(WCtx w, const Trial& t, const Refine& r) {
-	PartView pi = part_view_packed(t.partition_count, t.packed);
+template <bool L1> ASTC_FN float refine_score(const WCtx& w, const Trial& t, const Refine& r) {
+	PartView pi = refine_part_view<L1>(t);
+	if (L1) {
+		return compute_symbolic_block_difference_t<true>(w, 1, r.formats, -1, pi, (unsigned int)r.dmode, false);
+	}
 	return compute_symbolic_block_difference(w, t.partition_count, r.formats, t.plane2_component, pi, (unsigned int)r.dmode, t.dual != 0);
 }
 
@@ -623,7 +658,7 @@ ASTC_FN float refine_score(WCtx w, const Trial& t, const Refine& r) {
 enum { RF_KEEP = 0, RF_NEXT_CANDIDATE = 1, RF_STOP_ALL = 2, RF_NEXT_ITERATION = 3 };
 
 // advance to the next candidate / the next refinement iteration / finish the trial
-ASTC_FN void refine_apply(const WCtx& w, const Trial& t, Refine& r, BlockSearch& s, int action, bool error_block, float best_in_mode, bool new_best, float errorval) {
+template <bool L1> ASTC_FN void refine_apply(const WCtx& w, const Trial& t, Refine& r, BlockSearch& s, int action, bool error_block, float best_in_mode, bool new_best, float errorval) {
 	unsigned int i = r.i, l = r.l;
 	unsigned int candidate_count = t.candidate_count;
 	ST_WRITE_BEGIN(w)
@@ -650,13 +685,17 @@ ASTC_FN void refine_apply(const WCtx& w, const Trial& t, Refine& r, BlockSearch&
 		}
 	ST_WRITE_END(w)
 	if (new_best) {
-		copy_work_to_best(w);
+		if (L1) {
+			copy_work_to_best_t(w);
+		} else {
+			copy_work_to_best(w);
+		}
 	}
 }
 
 // step part 3 (first iteration of a candidate only): score before realignment (:606-640)
-ASTC_FN void refine_first_score(WCtx w, const Trial& t, Refine& r, BlockSearch& s) {
-	float errorval = refine_score(w, t, r);
+template <bool L1> ASTC_FN void refine_first_score_t(const WCtx& w, const Trial& t, Refine& r, BlockSearch& s) {
+	float errorval = refine_score<L1>(w, t, r);
 	float best_in_mode = r.best_errorval_in_mode, best_in_scb = r.best_errorval_in_scb;
 	unsigned int l = r.l;
 	bool error_block = false;
@@ -677,14 +716,17 @@ ASTC_FN void refine_first_score(WCtx w, const Trial& t, Refine& r, BlockSearch& 
 			action = RF_STOP_ALL;
 		}
 	}
-	refine_apply(w, t, r, s, action, error_block, best_in_mode, new_best, errorval);
+	refine_apply<L1>(w, t, r, s, action, error_block, best_in_mode, new_best, errorval);
+}
+ASTC_FN void refine_first_score(const WCtx& w, const Trial& t, Refine& r, BlockSearch& s) {
+	refine_first_score_t<false>(w, t, r, s);
 }
 
 // step part 5: score after realignment and decide how to go on (:642-698)
-ASTC_FN void refine_second_score(WCtx w, const Trial& t, Refine& r, BlockSearch& s) {
+template <bool L1> ASTC_FN void refine_second_score_t(const WCtx& w, const Trial& t, Refine& r, BlockSearch& s) {
 	float errorval = ERROR_CALC_DEFAULT;
 	if (r.work.block_type != SYM_BTYPE_ERROR) {
-		errorval = refine_score(w, t, r);
+		errorval = refine_score<L1>(w, t, r);
 	}
 	float best_in_mode = r.best_errorval_in_mode, best_in_scb = r.best_errorval_in_scb;
 	unsigned int l = r.l;
@@ -712,16 +754,23 @@ ASTC_FN void refine_second_score(WCtx w, const Trial& t, Refine& r, BlockSearch&
 			action = RF_NEXT_ITERATION;
 		}
 	}
-	refine_apply(w, t, r, s, action, error_block, best_in_mode, new_best, errorval);
+	refine_apply<L1>(w, t, r, s, action, error_block, best_in_mode, new_best, errorval);
+}
+ASTC_FN void refine_second_score(const WCtx& w, const Trial& t, Refine& r, BlockSearch& s) {
+	refine_second_score_t<false>(w, t, r, s);
 }
 
 // step part 4: realign the weights of the work candidate
-ASTC_FN void refine_realign(WCtx w, const Trial& t, Refine& r) {
-	PartView pi = part_view_packed(t.partition_count, t.packed);
-	bool adjustments = realign_weights(w, t.partition_count, r.formats, t.plane2_component, pi, r.qmode, t.dual != 0, (unsigned int)r.dmode);
+template <bool L1> ASTC_FN void refine_realign_t(const WCtx& w, const Trial& t, Refine& r) {
+	PartView pi = refine_part_view<L1>(t);
+	bool adjustments = L1 ? realign_weights_t<true>(w, 1, r.formats, -1, pi, r.qmode, false, (unsigned int)r.dmode)
+	                      : realign_weights(w, t.partition_count, r.formats, t.plane2_component, pi, r.qmode, t.dual != 0, (unsigned int)r.dmode);
 	ST_WRITE_BEGIN(w)
 		r.adjustments = adjustments;
 	ST_WRITE_END(w)
+}
+ASTC_FN void refine_realign(const WCtx& w, const Trial& t, Refine& r) {
+	refine_realign_t<false>(w, t, r);
 }
 
 #if defined(ASTC_HOSTSIM) && defined(ASTC_TRIAL_STATS)

@@ -675,7 +675,7 @@ ASTC_FN RefineScratch make_refine_scratch(const WCtx& w) {
 }
 
 // undecimate the quantised weights of `planes` planes: lanes over texels
-ASTC_COOP void undecimate_weights(WCtx w, unsigned int d, int planes) {
+ASTC_FN void undecimate_weights_t(const WCtx& w, unsigned int d, int planes) {
 	RefineScratch rs = make_refine_scratch(w);
 	DecView di = dec_view(d);
 	int T = w.T;
@@ -698,14 +698,23 @@ ASTC_COOP void undecimate_weights(WCtx w, unsigned int d, int planes) {
 	}
 	wsync();
 }
+ASTC_COOP void undecimate_weights(WCtx w, unsigned int d, int planes) {
+	undecimate_weights_t(w, d, planes);
+}
 
 // recompute_ideal_colors_1plane :1146-1366. Per-texel terms (in partition-texel order):
 //   0 left, 1 middle, 2 right, 3 weight_weight, 4-7 color_vec_x, 8-11 color_vec_y, 12-13 scale_vec;
 // one chain per (partition, term).
-ASTC_COOP void recompute_ideal_colors_1plane(WCtx w, const PartView& pi, unsigned int d) {
+// L1: one partition and LDR endpoints are compile-time facts (the refinement step of the one-partition, one-plane LDR trial inlines
+// this instantiation; the out-of-line function is the general one).
+template <bool L1> ASTC_FN void recompute_ideal_colors_1plane_t(const WCtx& w, const PartView& pi, unsigned int d) {
 	RefineScratch rs = make_refine_scratch(w);
-	unsigned int pc = pi.partition_count;
-	undecimate_weights(w, d, 1);
+	const unsigned int pc = L1 ? 1u : pi.partition_count;
+	if (L1) {
+		undecimate_weights_t(w, d, 1);
+	} else {
+		undecimate_weights(w, d, 1);
+	}
 	SPtr<float> undec = sptr<float>(rs.undec[0]);
 	SPtr<float> tmpf = tmpf_of(w);
 	SPtr<float> sdv = tmpf + 64;            // scale_dir per partition, 4 floats each
@@ -876,7 +885,7 @@ ASTC_COOP void recompute_ideal_colors_1plane(WCtx w, const PartView& pi, unsigne
 		epf[(EP_RGBS + (int)i) * 4 + c] = rgbs_c;
 	}
 	wsync();
-	if (bi.rgb_lns0 || bi.alpha_lns0) {
+	if (!L1 && (bi.rgb_lns0 || bi.alpha_lns0)) {
 		// HDR: the RGBO fit mixes the channels - one lane per partition
 		SPtr<f4> ep = ep_of(w);
 		ASTC_NOUNROLL
@@ -896,6 +905,9 @@ ASTC_COOP void recompute_ideal_colors_1plane(WCtx w, const PartView& pi, unsigne
 		}
 		wsync();
 	}
+}
+ASTC_COOP void recompute_ideal_colors_1plane(WCtx w, const PartView& pi, unsigned int d) {
+	recompute_ideal_colors_1plane_t<false>(w, pi, d);
 }
 
 // recompute_ideal_colors_2planes :1369-1650. Per-texel terms (texel order):
@@ -1073,7 +1085,8 @@ ASTC_FN int lerp1(bool u8, int c0, int c1, int w1) {   // lerp_color_int :37-61
 }
 
 // Unpack the integer endpoints of the work candidate into the arena: ends[p * 8 + 0..3] = endpoint 0 (rgba), + 4..7 = endpoint 1.
-ASTC_COOP void unpack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats, uint32_t ends_off) {
+template <bool L1> ASTC_FN void unpack_work_endpoints_t(const WCtx& w, unsigned int pc_in, uint32_t formats, uint32_t ends_off) {
+	const unsigned int pc = L1 ? 1u : pc_in;
 	SPtr<int> ends = sptr<int>(ends_off);
 	SPtr<uint8_t> wc = work_colors_of(w);
 	ASTC_NOUNROLL
@@ -1081,12 +1094,15 @@ ASTC_COOP void unpack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats, 
 		const uint8_t* in = &wc[(int)p * 8];      // (straight from the shared arena: no local copy)
 		bool rgb_lns, a_lns;
 		i4 e0, e1;
-		unpack_color_endpoints_inl(CFG.profile, (int)((formats >> (8 * p)) & 0xFF), in, rgb_lns, a_lns, e0, e1);
+		unpack_color_endpoints_inl<L1>(CFG.profile, (int)((formats >> (8 * p)) & 0xFF), in, rgb_lns, a_lns, e0, e1);
 		SPtr<int> o = ends + (int)p * 8;
 		o[0] = e0.x; o[1] = e0.y; o[2] = e0.z; o[3] = e0.w;
 		o[4] = e1.x; o[5] = e1.y; o[6] = e1.z; o[7] = e1.w;
 	}
 	wsync();
+}
+ASTC_COOP void unpack_work_endpoints(WCtx w, unsigned int pc, uint32_t formats, uint32_t ends_off) {
+	unpack_work_endpoints_t<false>(w, pc, formats, ends_off);
 }
 ASTC_FN uint32_t pack_formats(const ScbHdr& h) {
 	return (uint32_t)h.color_formats[0] | ((uint32_t)h.color_formats[1] << 8) | ((uint32_t)h.color_formats[2] << 16) | ((uint32_t)h.color_formats[3] << 24);
@@ -1098,7 +1114,10 @@ ASTC_FN uint32_t ends_off_of(const WCtx& w) { return w.base + A_TMPF + 96 * 4; }
 // compute_symbolic_block_difference_{2plane,1plane,1plane_1partition} (:313-618) on the work candidate.
 // Per-texel terms by lanes over texels (integer infill :89-167 inlined), then the reference's summation order:
 // 4-lane accumulator (1 partition, 1 plane, no RGBM) or one scalar chain.
-ASTC_COOP float compute_symbolic_block_difference(WCtx w, unsigned int pc, uint32_t formats, int plane2_component, const PartView& pi, unsigned int d, bool dual) {
+template <bool L1> ASTC_FN float compute_symbolic_block_difference_t(const WCtx& w, unsigned int pc_in, uint32_t formats, int plane2_in, const PartView& pi, unsigned int d, bool dual_in) {
+	const unsigned int pc = L1 ? 1u : pc_in;
+	const int plane2_component = L1 ? -1 : plane2_in;
+	const bool dual = L1 ? false : dual_in;
 	RefineScratch rs = make_refine_scratch(w);
 	DecView di = dec_view(d);
 	int T = w.T;
@@ -1204,6 +1223,9 @@ ASTC_COOP float compute_symbolic_block_difference(WCtx w, unsigned int pc, uint3
 	wsync();
 	return r;
 }
+ASTC_COOP float compute_symbolic_block_difference(WCtx w, unsigned int pc, uint32_t formats, int plane2_component, const PartView& pi, unsigned int d, bool dual) {
+	return compute_symbolic_block_difference_t<false>(w, pc, formats, plane2_component, pi, d, dual);
+}
 
 // =============================================================================================
 // Weight realignment (astcenc_compress_symbolic.cpp:69-350)
@@ -1214,7 +1236,10 @@ ASTC_COOP float compute_symbolic_block_difference(WCtx w, unsigned int pc, uint3
 // [12][8] tile; twelve chain lanes (3 candidates x 4 channels) then add them in texel order, and a few shuffles fold
 // the channel sums the way the reference's dot product does. The bilinear infill of every texel (wb) is kept
 // current instead of being rebuilt for every weight: it only changes for the texels of a weight that moved.
-ASTC_COOP bool realign_weights(WCtx w, unsigned int pc, uint32_t formats, int plane2_component, const PartView& pi, int quant_mode, bool is_dual, unsigned int d) {
+template <bool L1> ASTC_FN bool realign_weights_t(const WCtx& w, unsigned int pc_in, uint32_t formats, int plane2_in, const PartView& pi, int quant_mode, bool dual_in, unsigned int d) {
+	const unsigned int pc = L1 ? 1u : pc_in;
+	const int plane2_component = L1 ? -1 : plane2_in;
+	const bool is_dual = L1 ? false : dual_in;
 	const DevConstTables* ct = ASTC_CT;
 	RefineScratch rs = make_refine_scratch(w);
 	DecView di = dec_view(d);
@@ -1599,6 +1624,9 @@ ASTC_COOP bool realign_weights(WCtx w, unsigned int pc, uint32_t formats, int pl
 #endif
 	}
 	return wany(adjustments);
+}
+ASTC_COOP bool realign_weights(WCtx w, unsigned int pc, uint32_t formats, int plane2_component, const PartView& pi, int quant_mode, bool is_dual, unsigned int d) {
+	return realign_weights_t<false>(w, pc, formats, plane2_component, pi, quant_mode, is_dual, d);
 }
 
 // =============================================================================================

@@ -26,6 +26,10 @@
 // length, and warps of a CTA wait for each other every round. Each warp drains class 0, then 1, ... so that the warps
 // voting together are (almost always) doing the same kind of step.
 #define ASTC_Q_CLASSES 4
+// Refinement items have one class more: the one-partition trials are split by planes (class 0: one partition, one plane - the
+// mode-0 trial and the full one-plane trial of every block, most of the refinement work; class 1: two planes; class p: p
+// partitions). Class 0 of an LDR profile runs the specialised refinement step (astc_dev_lockstep.cuh, L1).
+#define ASTC_Q_RCLASSES (ASTC_Q_CLASSES + 1)
 // Set-up items are queued by the trial's weight quantisation limit as well (Trial::max_weight_quant, 12 values): a later trial of
 // a block searches only the modes up to the limit its best result so far allows, and the cost of a set-up follows it (a
 // two-plane set-up at QUANT_32 costs several times one at QUANT_2). Mixed in one queue, every round of a CTA lasts as long as
@@ -46,7 +50,7 @@
 #else
 	#define ASTC_Q_RSUB 4
 #endif
-enum { Q_SETUP = 0, Q_REFINE = ASTC_Q_CLASSES * ASTC_Q_SUB, Q_PREPARE = Q_REFINE + ASTC_Q_CLASSES * ASTC_Q_RSUB, Q_EMIT = Q_PREPARE + ASTC_Q_PREP, ASTC_Q_KINDS = Q_EMIT + 1 };
+enum { Q_SETUP = 0, Q_REFINE = ASTC_Q_CLASSES * ASTC_Q_SUB, Q_PREPARE = Q_REFINE + ASTC_Q_RCLASSES * ASTC_Q_RSUB, Q_EMIT = Q_PREPARE + ASTC_Q_PREP, ASTC_Q_KINDS = Q_EMIT + 1 };
 
 struct WaveArgs {
 	uint8_t* records;            // [blocks] x record_bytes
@@ -276,6 +280,10 @@ ASTC_FN int trial_class(const Trial& t) {
 	int c = t.dual ? 0 : (int)t.partition_count - 1;
 	return c < 0 ? 0 : (c >= ASTC_Q_CLASSES ? ASTC_Q_CLASSES - 1 : c);
 }
+// the class of a trial's refinement queue (ASTC_Q_RCLASSES)
+ASTC_FN int refine_class(const Trial& t) {
+	return (!t.dual && t.partition_count == 1) ? 0 : trial_class(t) + 1;
+}
 
 #if defined(ASTC_STEP_STATS)
 // dev instrumentation (make -C astc-encoder_b200 variant NAME=stats DEFS=-DASTC_STEP_STATS=1): cycles per part, printed by the emit kernel.
@@ -431,10 +439,9 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 				}
 			}
 			wsync();
-			int klass = trial_class(t);
 			STAT_T(s5);
 			record_save(w, a, b, a.wave == 0);
-			q_push(w, a, refine_queue_of(w, t, klass), a.wave, b);
+			q_push(w, a, refine_queue_of(w, t, refine_class(t)), a.wave, b);
 #if defined(ASTC_STEP_STATS)
 			if (w.lane == 0) {
 				long long s6 = clock64();
@@ -480,7 +487,6 @@ ASTC_COOP void wave_finish_trial(WCtx w, const WaveArgs& a, unsigned int b, Bloc
 			t.candidate_count = ready;
 		}
 	ST_WRITE_END(w)
-	int klass = trial_class(t);
 	if (straight) {
 		// the set-up of the trial just finished already selected this trial's candidates: go straight to refinement
 		SPtr<uint32_t> dst = sptr<uint32_t>(w.base + A_CAND);
@@ -490,12 +496,12 @@ ASTC_COOP void wave_finish_trial(WCtx w, const WaveArgs& a, unsigned int b, Bloc
 			dst[k] = src[k];
 		}
 		record_save(w, a, b);
-		q_push(w, a, refine_queue_of(w, t, klass), a.wave + 1, b);
+		q_push(w, a, refine_queue_of(w, t, refine_class(t)), a.wave + 1, b);
 		return;
 	}
 	record_save(w, a, b);
 	if (next == NEXT_TRIAL) {
-		q_push(w, a, setup_queue_of(t, klass), a.wave + 1, b);
+		q_push(w, a, setup_queue_of(t, trial_class(t)), a.wave + 1, b);
 	} else if (next == NEXT_PREPARE) {
 		int pk = s.phase == 1 ? 0 : (s.pc < 2 ? 1 : (s.pc > ASTC_Q_PREP ? ASTC_Q_PREP - 1 : s.pc - 1));
 		q_push(w, a, Q_PREPARE + pk, a.wave, b);
@@ -512,6 +518,8 @@ ASTC_COOP void wave_finish_trial(WCtx w, const WaveArgs& a, unsigned int b, Bloc
 #define ASTC_REFINE_STATE_BYTES 128
 static_assert(sizeof(Refine) <= ASTC_REFINE_STATE_BYTES, "Refine must fit its shared-memory slot");
 
+// L1_STEP = false compiles the specialised step out (the kernel of the HDR profiles, which never take it)
+template <bool L1_STEP = true>
 ASTC_COOP void wave_refine(WCtx w, WaveArgs a, uint32_t warp_index) {
 	BlockSearch& s = search_of(w);
 	Trial& t = trial_of(w);
@@ -524,6 +532,10 @@ ASTC_COOP void wave_refine(WCtx w, WaveArgs a, uint32_t warp_index) {
 	uint32_t rec_phase = 0;
 	record_mbar_init(w);
 	const unsigned int vote_mask = (1u << ((a.sync_mask >> 8) & 7)) - 1u;
+	// class 0 of an LDR profile: the step with every part inlined (one partition, one plane, LDR endpoint formats). The warp's
+	// queue cursor says which class the item came from; the classes are drained in order, so the specialised items come first.
+	const bool ldr = L1_STEP && (CFG.profile == PRF_LDR || CFG.profile == PRF_LDR_SRGB);
+	bool l1 = false;
 #if defined(ASTC_STEP_STATS)
 	int st_prev_class = -1;
 	long long st_prev_end = 0;
@@ -531,14 +543,16 @@ ASTC_COOP void wave_refine(WCtx w, WaveArgs a, uint32_t warp_index) {
 	while (true) {
 		while (!has_item && !drained) {
 #if ASTC_Q_RSUB == 1
-			if (!q_pop_classes(w, a, Q_REFINE, a.wave, cls, b)) {
+			if (!q_pop_classes(w, a, Q_REFINE, a.wave, cls, b, ASTC_Q_RCLASSES)) {
 #else
-			if (!q_pop_sorted(w, a, Q_REFINE, ASTC_Q_RSUB, a.wave, cls, b, ASTC_Q_CLASSES)) {
+			if (!q_pop_sorted(w, a, Q_REFINE, ASTC_Q_RSUB, a.wave, cls, b, ASTC_Q_RCLASSES)) {
 #endif
 				drained = true;
 				break;
 			}
 			record_restore(w, a, b, rec_phase);
+			// (the restored trial's own shape is checked too: only a one-partition, one-plane trial may run the folded step)
+			l1 = ldr && cls < ASTC_Q_RSUB && !t.dual && t.partition_count == 1;
 			refine_begin_trial(w, t, r, s, true);
 			if (!r.running) {
 				wave_finish_trial(w, a, b, s, t, r.best_errorval_in_mode);
@@ -564,19 +578,34 @@ ASTC_COOP void wave_refine(WCtx w, WaveArgs a, uint32_t warp_index) {
 			stat_hist(7, t0 - tv);
 		}
 #endif
-		if (has_item) refine_recompute(w, t, r);
+		if (has_item) {
+			if (l1) refine_recompute_t<true>(w, t, r);
+			else refine_recompute(w, t, r);
+		}
 		STAT_T(t1);
 		if (a.sync_mask & 16) cta_sync();
-		if (has_item) refine_pack(w, t, r);
+		if (has_item) {
+			if (l1) refine_pack_t<true>(w, t, r);
+			else refine_pack(w, t, r);
+		}
 		STAT_T(t2);
 		if (a.sync_mask & 32) cta_sync();
-		if (has_item && r.l == 0) refine_first_score(w, t, r, s);
+		if (has_item && r.l == 0) {
+			if (l1) refine_first_score_t<true>(w, t, r, s);
+			else refine_first_score(w, t, r, s);
+		}
 		STAT_T(t3);
 		if (a.sync_mask & 64) cta_sync();
-		if (has_item && r.running && r.in_step) refine_realign(w, t, r);
+		if (has_item && r.running && r.in_step) {
+			if (l1) refine_realign_t<true>(w, t, r);
+			else refine_realign(w, t, r);
+		}
 		STAT_T(t4);
 		if (a.sync_mask & 128) cta_sync();
-		if (has_item && r.running && r.in_step) refine_second_score(w, t, r, s);
+		if (has_item && r.running && r.in_step) {
+			if (l1) refine_second_score_t<true>(w, t, r, s);
+			else refine_second_score(w, t, r, s);
+		}
 		STAT_T(t5);
 #if defined(ASTC_STEP_STATS)
 		if (st_on) {

@@ -139,9 +139,13 @@ astc_wave_setup_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant
 #ifndef ASTC_REFINE_MIN_CTAS
 #define ASTC_REFINE_MIN_CTAS 1
 #endif
+// Two instantiations: L1_STEP = true for the LDR profiles (the specialised one-partition, one-plane step inlined beside the
+// general one), false for the HDR profiles, which never take it - their kernel carries the general step alone, laid out as
+// it was before the specialised step existed.
+template <bool L1_STEP>
 __global__ void __launch_bounds__(ASTC_REFINE_THREADS_MAX, ASTC_REFINE_MIN_CTAS)
 astc_wave_refine_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img, const __grid_constant__ WaveArgs a) {
-	if (wave_queue_empty(a, Q_REFINE, 0, ASTC_Q_CLASSES * ASTC_Q_RSUB)) {
+	if (wave_queue_empty(a, Q_REFINE, 0, ASTC_Q_RCLASSES * ASTC_Q_RSUB)) {
 		return;
 	}
 	stage_launch_constants(bsd, cfg, img);
@@ -150,8 +154,11 @@ astc_wave_refine_kernel(const __grid_constant__ DevBsd bsd, const __grid_constan
 	w.lane = threadIdx.x & 31;
 	w.base = ASTC_SMEM_HDR + a.stage_bytes + (uint32_t)(threadIdx.x >> 5) * bsd.arena_bytes_small;
 	w.T = bsd.texel_count;
-	wave_refine(w, a, threadIdx.x >> 5);
+	wave_refine<L1_STEP>(w, a, threadIdx.x >> 5);
 }
+
+// which refinement kernel a context launches
+static inline bool refine_l1_step(const DevConfig& cfg) { return cfg.profile == PRF_LDR || cfg.profile == PRF_LDR_SRGB; }
 
 __global__ void __launch_bounds__(ASTC_REFINE_THREADS_MAX, 1)
 astc_wave_prepare_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img, const __grid_constant__ WaveArgs a) {
@@ -659,7 +666,8 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 			ctx->smem_small = ASTC_SMEM_HDR + arena_small * wr;
 			ctx->smem_refine = ASTC_SMEM_HDR + ctx->refine_stage_bytes + arena_small * wr + (size_t)ASTC_REFINE_STATE_BYTES * wr;
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 			// a block runs at most this many trials (compress_block: mode-0 + full 1-plane, 4 two-plane, then the partition candidates)
 			int waves = 2 + 4;
@@ -920,7 +928,11 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d
 			} else {
 				astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
 			}
-			astc_wave_refine_kernel<<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
+			if (refine_l1_step(ctx->dcfg)) {
+				astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
+			} else {
+				astc_wave_refine_kernel<false><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
+			}
 			astc_wave_prepare_kernel<<<grid * 2, wp * 32, ASTC_SMEM_HDR + (size_t)bsd.arena_bytes_small * wp, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
 			ctx->launches += 3;
 		}
@@ -1155,7 +1167,11 @@ static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, in
 				astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
 				mark(0);
 			}
-			astc_wave_refine_kernel<<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+			if (refine_l1_step(ctx->dcfg)) {
+				astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+			} else {
+				astc_wave_refine_kernel<false><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+			}
 			mark(1);
 			// (statistics / partition search gain nothing from phase alignment: two half-size CTAs per SM wait less)
 			int wp = ctx->warps_small >= 2 ? ctx->warps_small / 2 : 1;

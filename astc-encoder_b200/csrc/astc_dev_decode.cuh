@@ -279,6 +279,11 @@ ASTC_FN void store_texel(const DevImage& img, unsigned int x, unsigned int y, un
 				zN = 0.0f;
 			}
 			vz = (sqrtf(zN) * 0.5f) + 0.5f;
+			// A NaN input gives a NaN Z. The reference's x86 arithmetic passes on the first NaN operand's payload (quieted),
+			// which through 1 - xN * xN - yN * yN is R's, else A's; the GPU's arithmetic would give its canonical NaN instead.
+			if (d.x != d.x || d.w != d.w) {
+				vz = ASTC_U2F(ASTC_F2U(d.x != d.x ? d.x : d.w) | 0x00400000u);
+			}
 		}
 		float sel[4];
 		for (int k = 0; k < 4; k++) {

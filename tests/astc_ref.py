@@ -236,6 +236,10 @@ class AstcencLib:
         finally:
             self.lib.astcenc_context_free(ctx)
 
+    def block_info_fields(self, blocks, profile, bx, by, flags=0, quality=PRE_MEDIUM, bz=1):
+        """The header fields of astcenc_get_block_info for every block: a uint32 array with one row of BLOCK_INFO_FIELDS per block."""
+        return block_info_fields(self.block_infos(blocks, profile, bx, by, flags=flags, quality=quality, bz=bz))
+
     def decompress(self, blocks, w, h, profile, bx, by, out_type=TYPE_U8, flags=0, swz=(0, 1, 2, 3), quality=PRE_MEDIUM):
         """blocks: uint8 array of 16-byte blocks. Returns a numpy (h, w, 4) image of out_type; raises on API errors."""
         cfg = self.config(profile, bx, by, quality, flags)
@@ -255,6 +259,24 @@ class AstcencLib:
             return out
         finally:
             self.lib.astcenc_context_free(ctx)
+
+
+# the fields a block's header determines (is_hdr_block also depends on the profile and the endpoint values)
+BLOCK_INFO_FIELDS = ("is_error_block", "is_constant_block", "is_dual_plane_block", "partition_count", "partition_index",
+                     "dual_plane_component", "color_endpoint_modes", "color_level_count", "weight_level_count", "weight_x", "weight_y", "weight_z")
+
+
+def block_info_fields(infos):
+    """Raw astcenc_block_info structs -> uint32 array (blocks, 15): BLOCK_INFO_FIELDS in order, the four endpoint modes expanded."""
+    rows = []
+    for raw in infos:
+        info = BlockInfo.from_buffer_copy(raw)
+        row = []
+        for name in BLOCK_INFO_FIELDS:
+            v = getattr(info, name)
+            row += list(v) if name == "color_endpoint_modes" else [int(v)]
+        rows.append(row)
+    return np.array(rows, dtype=np.uint32).reshape(-1, 15)
 
 
 def have_ref():
@@ -366,7 +388,7 @@ class RecordedReference:
     output does not depend on it (test_reference_thread_invariance). With `live` (the reference build itself) every call
     is forwarded to it and its answer recorded; save() merges the recording into a golden file."""
 
-    METHODS = ("compress", "compress_volume", "decompress_volume", "block_infos", "config")
+    METHODS = ("compress", "compress_volume", "decompress_volume", "block_infos", "block_info_fields", "config")
 
     def __init__(self, live=None, path=GOLDEN_REFERENCE):
         self.live = live

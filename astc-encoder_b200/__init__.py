@@ -171,18 +171,50 @@ def config_init(profile, block_x, block_y, quality, flags=0, block_z=1, **overri
 
 _DTYPES = {np.dtype(np.uint8): TYPE_U8, np.dtype(np.float16): TYPE_F16, np.dtype(np.float32): TYPE_F32}
 
+PROGRESS_CALLBACK = C.CFUNCTYPE(None, C.c_float)      # astcenc_progress_callback
+
 
 class Context:
-    """astcenc_context (astcenc_context_alloc / astcenc_compress_image / astcenc_context_free)."""
+    """astcenc_context (astcenc_context_alloc / astcenc_compress_image / astcenc_context_free).
 
-    def __init__(self, config, thread_count=1):
-        self.config = config
+    progress: optional callable(float), the config's progress_callback. compress_image calls it from the thread that runs
+    the pass while blocks complete, and exactly once with 100.0 when the payload is in place (not after cancel()); it may
+    call cancel(). parent: another Context whose tables this one shares (astcenc_context_alloc's parent argument); the
+    config then comes from the parent."""
+
+    def __init__(self, config=None, thread_count=1, progress=None, parent=None):
+        self.handle = None
+        self._progress = None
+        if parent is not None:
+            config = parent.config
+        cfg = Config.from_buffer_copy(config)
+        if progress is not None:
+            # the trampoline must outlive every call that can reach it: it is kept with the context
+            self._progress = PROGRESS_CALLBACK(lambda value: progress(float(value)))
+            cfg.progress_callback = C.cast(self._progress, C.c_void_p)
+        self.config = cfg
         self.thread_count = thread_count
-        self.handle = C.c_void_p()
-        err = lib().astcenc_context_alloc(C.byref(config), thread_count, C.byref(self.handle), None)
+        handle = C.c_void_p()
+        if parent is not None:
+            err = lib().astcenc_context_alloc(None, thread_count, C.byref(handle), parent.handle)
+        else:
+            err = lib().astcenc_context_alloc(C.byref(cfg), thread_count, C.byref(handle), None)
         if err:
-            self.handle = None
             raise AstcencError(err, "astcenc_context_alloc")
+        self.handle = handle
+
+    def cancel(self):
+        """astcenc_compress_cancel: a running compress_image stops handing out blocks and returns without writing its output;
+        safe from any thread and from inside the progress callback."""
+        err = lib().astcenc_compress_cancel(self.handle)
+        if err:
+            raise AstcencError(err, "astcenc_compress_cancel")
+
+    def reset(self):
+        """astcenc_compress_reset: ready for the next image (clears a cancel)."""
+        err = lib().astcenc_compress_reset(self.handle)
+        if err:
+            raise AstcencError(err, "astcenc_compress_reset")
 
     def close(self):
         if self.handle:

@@ -24,21 +24,50 @@ ASTC_FN void cta_sync() { __syncthreads(); }
 ASTC_FN bool cta_any(bool p) { return __syncthreads_or(p ? 1 : 0) != 0; }
 #endif
 
+// Progress and cancellation of an astcenc_compress_image pass: two device words per context, null when the pass has none.
+// The cancel flag is written by a DMA from the host while the kernels run; one lane reads it (from L2) wherever a warp takes
+// new work, and a raised flag looks exactly like an empty queue / exhausted ticket feed, so the warps leave through their usual
+// exits. The done counter gets one add per block whose search has ended (its result is final).
+#if defined(ASTC_HOSTSIM)
+// (a harness may watch every look at the flag: tests/hostsim/hostsim_progress.cpp raises it after a number of pops)
+static void (*g_hostsim_cancel_look)() = nullptr;
+ASTC_FN bool pass_cancelled(const uint32_t* flag) {
+	if (flag == nullptr) {
+		return false;
+	}
+	if (g_hostsim_cancel_look != nullptr) {
+		g_hostsim_cancel_look();
+	}
+	return *flag != 0;
+}
+ASTC_FN void pass_done_add(uint32_t* done) { if (done != nullptr) *done += 1u; }
+#else
+ASTC_FN bool pass_cancelled(const uint32_t* flag) { return flag != nullptr && __ldcg(flag) != 0u; }
+ASTC_FN void pass_done_add(uint32_t* done) { if (done != nullptr) atomicAdd(done, 1u); }
+#endif
+// a block's search has ended (called by the whole warp)
+ASTC_FN void pass_block_done(const WCtx& w, uint32_t* done) {
+	if (w.lane == 0) {
+		pass_done_add(done);
+	}
+}
+
 // where the next block index comes from (device: a global ticket counter; host simulation: a plain counter)
 struct BlockFeed {
 	unsigned int* ticket;
 	unsigned int total;
 	unsigned int blocks_x;
+	const uint32_t* cancel = ASTC_PASS_CANCEL_DEFAULT;      // raised: the feed is exhausted (may be null)
 };
 
 ASTC_FN bool feed_next(const WCtx& w, const BlockFeed& f, unsigned int& b) {
 #if defined(ASTC_HOSTSIM) && defined(ASTC_ONE_LANE)
-	b = (*f.ticket)++;
+	b = pass_cancelled(f.cancel) ? 0xFFFFFFFFu : (*f.ticket)++;
 #elif defined(ASTC_DEBUG_SINGLE_LANE)
-	b = atomicAdd(f.ticket, 1u);
+	b = pass_cancelled(f.cancel) ? 0xFFFFFFFFu : atomicAdd(f.ticket, 1u);
 #else
-	unsigned int v = 0;
-	if (w.lane == 0) {
+	unsigned int v = 0xFFFFFFFFu;
+	if (w.lane == 0 && !pass_cancelled(f.cancel)) {
 		v = atomicAdd(f.ticket, 1u);
 	}
 	b = __shfl_sync(0xffffffffu, v, 0);
@@ -815,10 +844,12 @@ ASTC_COOP void compress_blocks_lockstep(WCtx w, BlockFeed feed, uint32_t refine_
 					}
 					wsync();
 					emit_if_constant(w, b);
+					pass_block_done(w, IMG.done);
 					continue;
 				}
 				load_block(w, bx, by + IMG.block_row0);
 				if (emit_if_constant(w, b)) {
+					pass_block_done(w, IMG.done);
 					continue;
 				}
 				block_search_begin(w, s, b);
@@ -829,6 +860,7 @@ ASTC_COOP void compress_blocks_lockstep(WCtx w, BlockFeed feed, uint32_t refine_
 				break;
 			}
 			emit_block(w, s);
+			pass_block_done(w, IMG.done);
 			has_block = false;
 		}
 		if (!cta_any(active)) {

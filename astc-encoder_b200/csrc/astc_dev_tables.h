@@ -132,6 +132,15 @@ struct DevConfig {
 	float tune_search_mode0_enable;
 };
 
+// Where a DevImage's progress words point unless they are set: nowhere (progress and cancellation off). A host-simulation
+// harness may define these to its own words before it includes the device source (tests/hostsim/hostsim_progress.cpp).
+#ifndef ASTC_PASS_CANCEL_DEFAULT
+#define ASTC_PASS_CANCEL_DEFAULT nullptr
+#endif
+#ifndef ASTC_PASS_DONE_DEFAULT
+#define ASTC_PASS_DONE_DEFAULT nullptr
+#endif
+
 // One image (or slab) to compress.
 struct DevImage {
 	const void* data;          // RGBA texels, row-major, tightly packed
@@ -146,4 +155,8 @@ struct DevImage {
 	uint8_t* out;              // 16 bytes per block, slab-relative
 	const float* alpha_avg;    // per-texel alpha averages of the alpha-scale pre-pass, or NULL
 	float alpha_threshold;     // blocks with no average above this are emitted as constant zero
+	// progress and cancellation (astc_dev_lockstep.cuh, pass_cancelled) for the kernels that take no WaveArgs: the alpha-scale
+	// pre-pass and the single-kernel drivers; null = off
+	const uint32_t* cancel = ASTC_PASS_CANCEL_DEFAULT;
+	uint32_t* done = ASTC_PASS_DONE_DEFAULT;
 };

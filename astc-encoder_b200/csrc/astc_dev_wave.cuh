@@ -72,6 +72,8 @@ struct WaveArgs {
 	uint32_t stage_bytes_setup;  // set-up kernel: the same (decimation tables only)
 	uint32_t refine_state_off;   // refine kernel: offset of the per-warp Refine slots (ASTC_REFINE_STATE_BYTES each) in the shared window
 	uint32_t stage_bytes;        // refine kernel: bytes of tables staged between the header and the arenas (0 = none)
+	// (the progress and cancellation words of the pass are in the launch constants, IMG.cancel / IMG.done: kept out of this
+	// struct, which the item loops take by value)
 };
 
 #if defined(ASTC_HOSTSIM)
@@ -82,7 +84,9 @@ ASTC_FN uint32_t q_atomic_add(uint32_t* p, uint32_t v) { return atomicAdd(p, v);
 ASTC_FN uint32_t q_load(const uint32_t* p) { return __ldcg(p); }
 #endif
 
-ASTC_FN bool q_pop(const WCtx& w, const WaveArgs& a, int kind, int wave, unsigned int& b) {
+// q_pop without the look at the cancel flag: the refinement kernel looks once per item in its drain loop instead (wave_refine).
+// (The look inside each pop of q_pop_classes costs the refinement kernels more spill code, -Xptxas -v.)
+ASTC_FN bool q_pop_plain(const WCtx& w, const WaveArgs& a, int kind, int wave, unsigned int& b) {
 	uint32_t i = 0;
 	if (w.lane == 0) {
 		i = q_atomic_add(a.head + kind * ASTC_MAX_WAVES + wave, 1u);
@@ -94,11 +98,24 @@ ASTC_FN bool q_pop(const WCtx& w, const WaveArgs& a, int kind, int wave, unsigne
 	b = q_load(a.queues + (size_t)kind * a.queue_stride + i);
 	return true;
 }
+// one item of a queue; false once the queue is empty or the pass is cancelled (the flag is looked at before the item is taken)
+ASTC_FN bool q_pop(const WCtx& w, const WaveArgs& a, int kind, int wave, unsigned int& b) {
+	uint32_t i = 0xFFFFFFFFu;      // (past the end of every queue: what a warp sees once the pass is cancelled)
+	if (w.lane == 0 && !pass_cancelled(IMG.cancel)) {
+		i = q_atomic_add(a.head + kind * ASTC_MAX_WAVES + wave, 1u);
+	}
+	i = wbroadcast0(w, i);
+	if (i >= q_load(a.count + kind * ASTC_MAX_WAVES + wave)) {
+		return false;
+	}
+	b = q_load(a.queues + (size_t)kind * a.queue_stride + i);
+	return true;
+}
 
-// pop from the classes of a kind in order; cls is the warp's cursor
+// pop from the classes of a kind in order; cls is the warp's cursor (the caller looks at the cancel flag)
 ASTC_FN bool q_pop_classes(const WCtx& w, const WaveArgs& a, int kind, int wave, int& cls, unsigned int& b, int cls_end = ASTC_Q_CLASSES) {
 	while (cls < cls_end) {
-		if (q_pop(w, a, kind + cls, wave, b)) {
+		if (q_pop_plain(w, a, kind + cls, wave, b)) {
 			return true;
 		}
 		cls++;
@@ -322,6 +339,7 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 	feed.ticket = a.ticket;      // wave 0 has no queue: a ticket counter hands out the band's blocks
 	feed.total = a.band_blocks;
 	feed.blocks_x = a.blocks_x;
+	feed.cancel = IMG.cancel;
 	int cls = a.cls_lo * ASTC_Q_SUB;
 	uint32_t rec_phase = 0;
 	record_mbar_init(w);
@@ -343,10 +361,12 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 					}
 					wsync();
 					emit_if_constant(w, b);
+					pass_block_done(w, IMG.done);
 					continue;
 				}
 				load_block(w, bx, by + IMG.block_row0);
 				if (emit_if_constant(w, b)) {
+					pass_block_done(w, IMG.done);
 					continue;
 				}
 				block_search_begin(w, s, b);
@@ -507,6 +527,7 @@ ASTC_COOP void wave_finish_trial(WCtx w, const WaveArgs& a, unsigned int b, Bloc
 		q_push(w, a, Q_PREPARE + pk, a.wave, b);
 	} else {
 		q_push(w, a, Q_EMIT, 0, b);
+		pass_block_done(w, IMG.done);
 	}
 }
 
@@ -543,7 +564,14 @@ ASTC_COOP void wave_refine(WCtx w, WaveArgs a, uint32_t warp_index) {
 	while (true) {
 		while (!has_item && !drained) {
 #if ASTC_Q_RSUB == 1
-			if (!q_pop_classes(w, a, Q_REFINE, a.wave, cls, b, ASTC_Q_RCLASSES)) {
+			// (a raised cancel flag drains the queues; a pass without one skips the look)
+			bool stop = false;
+			if (IMG.cancel != nullptr) {
+				uint32_t c = 0;
+				if (w.lane == 0) c = pass_cancelled(IMG.cancel) ? 1u : 0u;
+				stop = wbroadcast0(w, c) != 0u;
+			}
+			if (stop || !q_pop_classes(w, a, Q_REFINE, a.wave, cls, b, ASTC_Q_RCLASSES)) {
 #else
 			if (!q_pop_sorted(w, a, Q_REFINE, ASTC_Q_RSUB, a.wave, cls, b, ASTC_Q_RCLASSES)) {
 #endif
@@ -665,6 +693,7 @@ ASTC_COOP void wave_prepare(WCtx w, WaveArgs a) {
 				q_push(w, a, setup_queue_of(t, klass), a.wave + 1, b);
 			} else {
 				q_push(w, a, Q_EMIT, 0, b);
+				pass_block_done(w, IMG.done);
 			}
 		}
 	}

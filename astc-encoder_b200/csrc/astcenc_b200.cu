@@ -17,6 +17,8 @@
 #include <cstring>
 #include <cstddef>
 #include <new>
+#include <thread>
+#include <chrono>
 
 #include "astc_dev_search.cuh"
 #include "astc_dev_metrics.cuh"
@@ -175,6 +177,10 @@ astc_wave_prepare_kernel(const __grid_constant__ DevBsd bsd, const __grid_consta
 
 __global__ void __launch_bounds__(ASTC_EMIT_THREADS, 1)
 astc_wave_emit_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img, const __grid_constant__ WaveArgs a) {
+	// a cancelled pass packs nothing (one look per CTA, so that the whole CTA leaves together; no barrier when the pass has no flag)
+	if (img.cancel != nullptr && __syncthreads_or(threadIdx.x == 0 && pass_cancelled(img.cancel) ? 1 : 0)) {
+		return;
+	}
 	stage_launch_constants(bsd, cfg, img);
 	wave_emit(threadIdx.x & 31, ASTC_SMEM_HDR + (uint32_t)(threadIdx.x >> 5) * (32 * EMIT_SLICE), a);
 }
@@ -183,6 +189,10 @@ astc_wave_emit_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant_
 #define ASTC_ALPHA_THREADS 128
 __global__ void __launch_bounds__(ASTC_ALPHA_THREADS, 1)
 astc_alpha_average_kernel(const __grid_constant__ DevImage img, unsigned int radius, unsigned int tiles_x, float* __restrict__ averages) {
+	// (a cancelled pass reads no averages: wave 0 finds the same raised flag)
+	if (img.cancel != nullptr && __syncthreads_or(threadIdx.x == 0 && pass_cancelled(img.cancel) ? 1 : 0)) {
+		return;
+	}
 	unsigned int ty = blockIdx.x / tiles_x;
 	unsigned int tx = blockIdx.x - ty * tiles_x;
 	alpha_average_tile(img, radius, tx * ALPHA_TILE, ty * ALPHA_TILE, 0, averages, (int)threadIdx.x, (int)blockDim.x);
@@ -235,6 +245,7 @@ astc_compress_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__
 		feed.ticket = ticket;
 		feed.total = total;
 		feed.blocks_x = blocks_x;
+		feed.cancel = img.cancel;
 		// (the Refine slots sit behind the arenas: the host sizes the window for them)
 		compress_blocks_lockstep(w, feed, ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + (uint32_t)(blockDim.x >> 5) * bsd.arena_bytes + (uint32_t)warp * ASTC_REFINE_STATE_BYTES);
 		return;
@@ -248,7 +259,7 @@ astc_compress_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__
 			unsigned int* cta_ticket = reinterpret_cast<unsigned int*>(astc_smem + ASTC_SMEM_HDR - 4);
 			__syncthreads();
 			if (threadIdx.x == 0) {
-				*cta_ticket = atomicAdd(ticket, 1u);
+				*cta_ticket = pass_cancelled(img.cancel) ? 0xFFFFFFFFu : atomicAdd(ticket, 1u);
 			}
 			__syncthreads();
 			b = *cta_ticket;
@@ -256,7 +267,7 @@ astc_compress_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__
 #endif
 		{
 			if (lane == 0) {
-				b = atomicAdd(ticket, 1u);
+				b = pass_cancelled(img.cancel) ? 0xFFFFFFFFu : atomicAdd(ticket, 1u);
 			}
 #if !defined(ASTC_DEBUG_SINGLE_LANE)
 			b = __shfl_sync(0xffffffffu, b, 0);
@@ -269,6 +280,7 @@ astc_compress_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__
 		unsigned int bx = b - by * blocks_x;
 		load_block(w, bx, by + IMG.block_row0);
 		compress_block(w, IMG.out + (size_t)b * 16);
+		pass_block_done(w, img.done);
 	}
 }
 
@@ -341,6 +353,8 @@ struct astcenc_context {
 	uint32_t refine_stage_bytes;   // tables staged behind the header of the refine kernel's shared window (0 = none)
 	int max_waves;
 	unsigned int volume_dim_z;      // slices of the volume the current pass reads (3D block sizes; 1 otherwise), set under launch_mtx
+	uint32_t* pass_cancel;          // the progress words the current pass's kernels see (null for the device-resident paths), set under launch_mtx
+	uint32_t* pass_done;
 	// wave pipeline buffers, grown on demand
 	uint8_t* d_records;
 	size_t d_records_bytes;
@@ -388,6 +402,16 @@ struct astcenc_context {
 	int dstate;                  // the same for decompression
 	astcenc_error dresult;
 	std::atomic<bool> cancel;
+	// Progress and cancellation of astcenc_compress_image (astc_dev_lockstep.cuh, pass_cancelled): d_words = {cancel flag, done
+	// counter}; h_words (pinned) = {0, 1, counter read-back}: the flag is written by 4-byte DMAs from h_words[0] / [1] and the
+	// counter read by one into h_words[2], all on ctl_stream, which never waits for the pass. flag_mtx makes "set ctx->cancel,
+	// enqueue the matching flag write" one step, so that the device flag always ends on the value ctx->cancel holds.
+	uint32_t* d_words;
+	uint32_t* h_words;
+	cudaStream_t ctl_stream;
+	cudaEvent_t ctl_ready;          // after the last flag clear: a pass starts behind it
+	std::mutex flag_mtx;
+	bool flag_raised;               // a raise was enqueued since the last clear (under flag_mtx)
 	// stats
 	unsigned long long launches;
 	float last_kernel_ms;
@@ -497,6 +521,12 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	ctx->dstate = 0;
 	ctx->dresult = ASTCENC_SUCCESS;
 	ctx->cancel = false;
+	ctx->d_words = nullptr;
+	ctx->h_words = nullptr;
+	ctx->ctl_stream = nullptr;
+	ctx->ctl_ready = nullptr;
+	ctx->flag_raised = false;
+	ctx->pass_cancel = ctx->pass_done = nullptr;
 	ctx->launches = 0;
 	ctx->last_kernel_ms = 0.0f;
 	ctx->last_h2d = ctx->last_d2h = 0;
@@ -676,6 +706,15 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 			CUDA_TRY(cudaMalloc(&ctx->d_counters, sizeof(uint32_t) * ASTC_COUNTER_WORDS * ASTC_MAX_PIPES), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
 		}
 		CUDA_TRY(cudaMalloc(&ctx->d_ticket, sizeof(unsigned int)), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
+		// progress and cancellation: the device words start cleared
+		CUDA_TRY(cudaMalloc(&ctx->d_words, 2 * sizeof(uint32_t)), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
+		CUDA_TRY(cudaMemset(ctx->d_words, 0, 2 * sizeof(uint32_t)), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaHostAlloc(&ctx->h_words, 3 * sizeof(uint32_t), cudaHostAllocDefault), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
+		ctx->h_words[0] = 0;
+		ctx->h_words[1] = 1;
+		ctx->h_words[2] = 0;
+		CUDA_TRY(cudaStreamCreateWithFlags(&ctx->ctl_stream, cudaStreamNonBlocking), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaEventCreateWithFlags(&ctx->ctl_ready, cudaEventDisableTiming), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 	}
 	CUDA_TRY(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 	CUDA_TRY(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
@@ -741,6 +780,13 @@ void astcenc_context_free(astcenc_context* ctx) {
 		if (ctx->pipe_done[i]) cudaEventDestroy(ctx->pipe_done[i]);
 	}
 	if (ctx->pipe_start) cudaEventDestroy(ctx->pipe_start);
+	if (ctx->ctl_stream) {
+		cudaStreamSynchronize(ctx->ctl_stream);
+		cudaStreamDestroy(ctx->ctl_stream);
+	}
+	if (ctx->ctl_ready) cudaEventDestroy(ctx->ctl_ready);
+	cudaFree(ctx->d_words);
+	if (ctx->h_words) cudaFreeHost(ctx->h_words);
 	if (ctx->stream) cudaStreamDestroy(ctx->stream);
 	if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
 	release_tables(ctx->tables);
@@ -792,11 +838,14 @@ static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, in
 static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
                                         unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up);
 
+// d_cancel / d_done: the progress words of an astcenc_compress_image pass (null: no progress, no cancellation).
 static astcenc_error launch_slab(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
                                  unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up = nullptr,
-                                 unsigned int volume_dim_z = 1) {
+                                 unsigned int volume_dim_z = 1, uint32_t* d_cancel = nullptr, uint32_t* d_done = nullptr) {
 	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
 	ctx->volume_dim_z = volume_dim_z;
+	ctx->pass_cancel = d_cancel;
+	ctx->pass_done = d_done;
 	if (ctx->scratch_used) {
 		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
@@ -867,6 +916,8 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d
 		im.out = d_out + first * 16;
 		im.alpha_avg = ctx->config.a_scale_radius != 0 && bsd.dim_z == 1 ? ctx->d_alpha : nullptr;
 		im.alpha_threshold = ctx->alpha_threshold;
+		im.cancel = ctx->pass_cancel;
+		im.done = ctx->pass_done;
 		uint32_t* counters = ctx->d_counters + (size_t)p * ASTC_COUNTER_WORDS;
 		CUDA_TRY(cudaMemsetAsync(counters, 0, sizeof(uint32_t) * ASTC_COUNTER_WORDS, ps), return ASTCENC_ERR_BAD_CONTEXT);
 		WaveArgs& w = a[p];
@@ -990,8 +1041,7 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 		if (smem > 48 * 1024) {
 			CUDA_TRY(cudaFuncSetAttribute(astc_alpha_average_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), return ASTCENC_ERR_BAD_CONTEXT);
 		}
-		DevImage aimg;
-		memset(&aimg, 0, sizeof(aimg));
+		DevImage aimg{};
 		aimg.data = d_pixels;
 		aimg.data_type = data_type;
 		aimg.dim_x = dim_x;
@@ -999,6 +1049,7 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 		for (int i = 0; i < 4; i++) {
 			aimg.swz[i] = swz[i];
 		}
+		aimg.cancel = ctx->pass_cancel;
 		unsigned int tiles_x = (dim_x + ALPHA_TILE - 1) / ALPHA_TILE, tiles_y = (dim_y + ALPHA_TILE - 1) / ALPHA_TILE;
 		astc_alpha_average_kernel<<<tiles_x * tiles_y, ASTC_ALPHA_THREADS, smem, stream>>>(aimg, radius, tiles_x, ctx->d_alpha);
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
@@ -1044,6 +1095,8 @@ static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, in
 	img.out = d_out;
 	img.alpha_avg = ctx->config.a_scale_radius != 0 && bsd.dim_z == 1 ? ctx->d_alpha : nullptr;
 	img.alpha_threshold = ctx->alpha_threshold;
+	img.cancel = ctx->pass_cancel;
+	img.done = ctx->pass_done;
 	size_t total = (size_t)img.blocks_x * block_rows;
 	if (ctx->driver == 0) {
 		// ---- wave pipeline ----
@@ -1207,11 +1260,53 @@ static astcenc_error ensure_buffer(uint8_t*& buf, size_t& have, size_t need) {
 	return ASTCENC_SUCCESS;
 }
 
+// Progress of one astcenc_compress_image call, reported like the reference's task pool (astcenc_internal_entry.h:199-295):
+// value = done / total * 100 over the blocks of the whole image, a call whenever it has moved by more than
+// max(1 %, 4096 blocks) since the last call, and exactly one call with 100 once the payload is in the caller's buffer.
+// The counter is read every ASTC_POLL_US: 1 ms is a tenth of the 1 % step of a 100 ms pass (a pass that short needs no
+// finer bar), a read costs the host thread one 4-byte copy (~10 us), and a finished or cancelled pass is noticed within 1 ms.
+#define ASTC_POLL_US 1000
+struct PassProgress {
+	astcenc_progress_callback callback;     // null: no polling, the pass is waited for with a plain synchronise
+	float total;                            // blocks of the whole image
+	float min_diff;
+	float last;
+};
+
+// Waits until `end` (recorded on the pass stream after the pass's kernels) has completed; with a callback, polls the done
+// counter meanwhile and reports progress. The callback may call astcenc_compress_cancel.
+static astcenc_error wait_pass(astcenc_context* ctx, cudaEvent_t end, PassProgress& pp) {
+	if (!pp.callback) {
+		CUDA_TRY(cudaEventSynchronize(end), return ASTCENC_ERR_BAD_CONTEXT);
+		return ASTCENC_SUCCESS;
+	}
+	while (true) {
+		cudaError_t q = cudaEventQuery(end);
+		if (q == cudaSuccess) {
+			return ASTCENC_SUCCESS;
+		}
+		if (q != cudaErrorNotReady) {
+			CUDA_TRY(q, return ASTCENC_ERR_BAD_CONTEXT);
+		}
+		std::this_thread::sleep_for(std::chrono::microseconds(ASTC_POLL_US));
+		CUDA_TRY(cudaMemcpyAsync(ctx->h_words + 2, ctx->d_words + 1, sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->ctl_stream), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaStreamSynchronize(ctx->ctl_stream), return ASTCENC_ERR_BAD_CONTEXT);
+		float value = (static_cast<float>(ctx->h_words[2]) / pp.total) * 100.0f;
+		// (100 is reported once, after the payload copy; nothing is reported once the pass is cancelled)
+		if (value < 100.0f && value - pp.last > pp.min_diff && !ctx->cancel.load()) {
+			pp.callback(value);
+			pp.last = value;
+		}
+	}
+}
+
 // The host-pointer path (what the reference's callers use: astcenccli_toplevel.cpp:2195-2215 passes plain heap memory).
 // The image goes up in bands on the copy stream while wave 0 already works on the bands that arrived; the payload comes
 // back with one copy when the emit kernel is done. Works with pageable and with pinned host memory alike (with pageable
 // memory the driver stages each band through its own pinned buffers and the call blocks for the band's duration -
 // the kernels of the earlier bands are running meanwhile).
+// A cancelled call (astcenc_compress_cancel) skips the remaining slices and copies no payload back: the caller's buffer keeps
+// its bytes, and the call still returns ASTCENC_SUCCESS (astcenc.h: the data is then undefined).
 static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_image& image, const astcenc_swizzle& swizzle, uint8_t* data_out) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	DeviceGuard guard(ctx->device);
@@ -1234,6 +1329,17 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 	ctx->last_h2d = ctx->last_d2h = 0;
 	ctx->last_kernel_ms = 0.0f;
 	float total_ms = 0.0f;
+	// the pass starts behind the last flag clear (astcenc_compress_reset), with its done counter at zero
+	uint32_t* d_cancel = ctx->d_words;
+	uint32_t* d_done = ctx->d_words + 1;
+	CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ctl_ready, 0), return ASTCENC_ERR_BAD_CONTEXT);
+	CUDA_TRY(cudaMemsetAsync(d_done, 0, sizeof(uint32_t), ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+	PassProgress pp;
+	pp.callback = ctx->config.progress_callback;
+	pp.total = static_cast<float>(blocks_x * blocks_y * (bsd.dim_z > 1 ? block_count_axis(image.dim_z, bsd.dim_z) : (size_t)image.dim_z));
+	pp.min_diff = (4096.0f / pp.total) * 100.0f;
+	pp.min_diff = pp.min_diff > 1.0f ? pp.min_diff : 1.0f;
+	pp.last = 0.0f;
 	if (bsd.dim_z > 1) {
 		// 3D block sizes (astcenc_entry.cpp:906-1043): the slices go up into one contiguous volume, the blocks come out in (z, y, x)
 		// order; "block rows" of the pass count layer * blocks_y + row
@@ -1246,30 +1352,41 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
+		if (ctx->cancel.load()) {
+			return ASTCENC_SUCCESS;
+		}
 		for (unsigned int z = 0; z < image.dim_z; z++) {
 			CUDA_TRY(cudaMemcpyAsync(ctx->d_image + (size_t)z * slice_bytes, image.data[z], slice_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		}
 		CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		st = launch_slab(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, swz, 0, (unsigned int)(blocks_y * blocks_z), ctx->d_out, ctx->stream, nullptr, image.dim_z);
+		st = launch_slab(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, swz, 0, (unsigned int)(blocks_y * blocks_z), ctx->d_out, ctx->stream, nullptr, image.dim_z,
+		                 d_cancel, d_done);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
 		CUDA_TRY(cudaEventRecord(ctx->ev1, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		st = wait_pass(ctx, ctx->ev1, pp);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
+		if (ctx->cancel.load()) {
+			return ASTCENC_SUCCESS;
+		}
 		CUDA_TRY(cudaMemcpyAsync(data_out, ctx->d_out, vol_out, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		cudaEventElapsedTime(&total_ms, ctx->ev0, ctx->ev1);
 		ctx->last_kernel_ms = total_ms;
 		ctx->last_h2d = slice_bytes * image.dim_z;
 		ctx->last_d2h = vol_out;
-		if (ctx->config.progress_callback) {
-			ctx->config.progress_callback(100.0f);
+		if (pp.callback) {
+			pp.callback(100.0f);
 		}
 		return ASTCENC_SUCCESS;
 	}
-	// 3D images with 2D blocks are an array of independent 2D slices (astcenc.h:94-100)
+	// 3D images with 2D blocks are an array of independent 2D slices (astcenc.h:94-100); progress runs over all of them
 	for (unsigned int z = 0; z < image.dim_z; z++) {
 		if (ctx->cancel.load()) {
-			break;
+			return ASTCENC_SUCCESS;
 		}
 		UploadPlan up;
 		up.host = static_cast<const uint8_t*>(image.data[z]);
@@ -1277,11 +1394,18 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 		up.row_bytes = (size_t)image.dim_x * bpt;
 		up.bands = ctx->knobs.upload_bands;
 		CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		st = launch_slab(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, swz, 0, (unsigned int)blocks_y, ctx->d_out, ctx->stream, &up);
+		st = launch_slab(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, swz, 0, (unsigned int)blocks_y, ctx->d_out, ctx->stream, &up, 1, d_cancel, d_done);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
 		CUDA_TRY(cudaEventRecord(ctx->ev1, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		st = wait_pass(ctx, ctx->ev1, pp);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
+		if (ctx->cancel.load()) {
+			return ASTCENC_SUCCESS;
+		}
 		CUDA_TRY(cudaMemcpyAsync(data_out + (size_t)z * out_bytes, ctx->d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		float ms = 0.0f;
@@ -1289,11 +1413,11 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 		total_ms += ms;
 		ctx->last_h2d += slice_bytes;
 		ctx->last_d2h += out_bytes;
-		if (ctx->config.progress_callback) {
-			ctx->config.progress_callback(100.0f * static_cast<float>(z + 1) / static_cast<float>(image.dim_z));
-		}
 	}
 	ctx->last_kernel_ms = total_ms;
+	if (pp.callback) {
+		pp.callback(100.0f);
+	}
 	return ASTCENC_SUCCESS;
 }
 
@@ -1359,15 +1483,31 @@ astcenc_error astcenc_compress_reset(astcenc_context* ctx) {
 	if (ctx->state != 1) {
 		ctx->state = 0;
 	}
+	std::lock_guard<std::mutex> fl(ctx->flag_mtx);
 	ctx->cancel = false;
+	if (ctx->flag_raised) {
+		// clear the device flag on the control stream (behind any raise enqueued before) and start the next pass behind it
+		DeviceGuard guard(ctx->device);
+		CUDA_TRY(cudaMemcpyAsync(ctx->d_words, ctx->h_words, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->ctl_stream), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaEventRecord(ctx->ctl_ready, ctx->ctl_stream), return ASTCENC_ERR_BAD_CONTEXT);
+		ctx->flag_raised = false;
+	}
 	return ASTCENC_SUCCESS;
 }
 
+// Takes neither ctx->mtx nor launch_mtx: it is called from other threads while a pass runs, and from inside the progress
+// callback on the thread that runs the pass.
 astcenc_error astcenc_compress_cancel(astcenc_context* ctx) {
 	if (ctx->config.flags & ASTCENC_FLG_DECOMPRESS_ONLY) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
+	std::lock_guard<std::mutex> fl(ctx->flag_mtx);
 	ctx->cancel = true;
+	// a 4-byte DMA from pinned memory on the control stream: it lands while the pass's kernels run, and their next look at the
+	// flag finds every queue empty
+	DeviceGuard guard(ctx->device);
+	CUDA_TRY(cudaMemcpyAsync(ctx->d_words, ctx->h_words + 1, sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->ctl_stream), return ASTCENC_ERR_BAD_CONTEXT);
+	ctx->flag_raised = true;
 	return ASTCENC_SUCCESS;
 }
 
@@ -1431,6 +1571,8 @@ static astcenc_error decompress_image_gpu(astcenc_context* ctx, const uint8_t* d
 	img.out = nullptr;
 	img.alpha_avg = nullptr;
 	img.alpha_threshold = 0.0f;
+	img.cancel = nullptr;
+	img.done = nullptr;
 	cudaDeviceProp prop;
 	CUDA_TRY(cudaGetDeviceProperties(&prop, ctx->device), return ASTCENC_ERR_BAD_CONTEXT);
 	unsigned int nblocks = (unsigned int)(blocks_x * blocks_y * blocks_z);
@@ -1535,8 +1677,7 @@ astcenc_error astcenc_get_block_info(astcenc_context* ctx, const uint8_t data[16
 	unsigned long long lo, hi;
 	memcpy(&lo, data, 8);
 	memcpy(&hi, data + 8, 8);
-	DevImage img;
-	memset(&img, 0, sizeof(img));
+	DevImage img{};
 	astc_block_info_kernel<<<1, 32, ASTC_SMEM_HDR + D_SLICE, ctx->stream>>>(ctx->tables->bsd, ctx->dcfg, img, lo, hi, d_info);
 	ctx->launches++;
 	DevBlockInfo h;

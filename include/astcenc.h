@@ -183,9 +183,14 @@ ASTCENC_PUBLIC const char* astcenc_get_error_string(enum astcenc_error status);
 
 /* Behaviour notes for the ten reference entry points above, where the GPU implementation differs in timing (never in
  * results) from the reference's thread pool:
- *  - progress_callback is called once per 2D slice (at 100 % for a 2D image); the reference calls it per 16-block ticket
- *    (astcenc_entry.cpp:937). astcenc_compress_cancel() takes effect between slices: a pipeline pass that is already
- *    enqueued runs to its end (the reference stops handing out tickets, astcenc_internal_entry.h:219).
+ *  - progress_callback is called as blocks complete, like the reference's task pool (astcenc_internal_entry.h:199-295): with
+ *    done / total * 100 over the blocks of the whole image (all slices of a volume), whenever the value has moved by more
+ *    than max(1 %, 4096 blocks) since the last call, and exactly once with 100 after the payload is in data_out. Only the
+ *    calling thread that runs the pass calls it; the library polls a device counter about every millisecond.
+ *  - astcenc_compress_cancel() stops a running pass at once: the kernels stop taking blocks (the flag is written into device
+ *    memory while they run), remaining slices are skipped, and the call returns ASTCENC_SUCCESS without writing data_out and
+ *    without the 100 % call. It takes no lock a pass holds, so it may be called from the progress callback. The
+ *    astcenc_b200_* device-resident and multi-GPU entry points have neither progress nor cancellation.
  *  - Every entry point runs on the CUDA device that was current in astcenc_context_alloc() and restores the caller's
  *    current device before it returns.
  *  - Block sizes: the fourteen 2D and the ten 3D footprints (block_z > 1: 3x3x3 .. 6x6x6, astcenc_block_sizes.cpp:1025). With a

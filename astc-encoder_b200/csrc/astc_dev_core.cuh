@@ -643,8 +643,10 @@ struct PartitionMetrics {
 // Partition means. For >= 2 partitions the reference accumulates with masked haccumulate: texel i adds
 // to lane (i mod 4) of its partition's accumulator -> one chain per (partition, channel, i mod 4).
 // ncomp = 4 (rgba) or 3 (rgb, lane 3 zero).
-ASTC_COOP void compute_partition_averages(WCtx w, const PartView& pi, int ncomp, f4 averages[4]) {
-	unsigned int pc = pi.partition_count;
+// (S1 in this section and the next: the trial has one partition and one plane, a compile-time fact - the wave-0 set-up of an
+// LDR profile inlines that instantiation, astc_dev_wave.cuh; the out-of-line function is the general one)
+template <bool S1> ASTC_FN void compute_partition_averages_t(const WCtx& w, const PartView& pi, int ncomp, f4 averages[4]) {
+	const unsigned int pc = S1 ? 1u : pi.partition_count;
 	f4 dm = bi_of(w).data_mean;
 	f4 mean = ncomp == 4 ? dm : mk4(dm.x, dm.y, dm.z, 0.0f);
 	if (pc == 1) {
@@ -684,11 +686,14 @@ ASTC_COOP void compute_partition_averages(WCtx w, const PartView& pi, int ncomp,
 	averages[pc - 1] = rest / static_cast<float>(pv_count(pi, pc - 1));
 	wsync();
 }
+ASTC_COOP void compute_partition_averages(WCtx w, const PartView& pi, int ncomp, f4 averages[4]) {
+	compute_partition_averages_t<false>(w, pi, ncomp, averages);
+}
 
 // Sign-split direction sums: one chain per (partition, split axis K, component c), in partition-texel order.
 // chan = the ncomp block channels taking part, 4 bits each (channel c of the fit is block channel (chan >> 4c) & 15).
-ASTC_COOP void compute_dirs(WCtx w, const PartView& pi, uint32_t chan, int ncomp, const f4 averages[4], PartitionMetrics pm[4]) {
-	unsigned int pc = pi.partition_count;
+template <bool S1> ASTC_FN void compute_dirs_t(const WCtx& w, const PartView& pi, uint32_t chan, int ncomp, const f4 averages[4], PartitionMetrics pm[4]) {
+	const unsigned int pc = S1 ? 1u : pi.partition_count;
 	SPtr<float> tmpf = tmpf_of(w);
 	int per_part = ncomp * ncomp;
 	int nchains = (int)pc * per_part;
@@ -741,13 +746,24 @@ ASTC_COOP void compute_dirs(WCtx w, const PartView& pi, uint32_t chan, int ncomp
 	}
 	wsync();
 }
+ASTC_COOP void compute_dirs(WCtx w, const PartView& pi, uint32_t chan, int ncomp, const f4 averages[4], PartitionMetrics pm[4]) {
+	compute_dirs_t<false>(w, pi, chan, ncomp, averages, pm);
+}
 
 ASTC_FN uint32_t chan_list(int a, int b, int c, int d) { return (uint32_t)a | ((uint32_t)b << 4) | ((uint32_t)c << 8) | ((uint32_t)d << 12); }
 
-ASTC_COOP void compute_avgs_and_dirs_4_comp(WCtx w, const PartView& pi, PartitionMetrics pm[4]) {
+template <bool S1> ASTC_FN void compute_avgs_and_dirs_4_comp_t(const WCtx& w, const PartView& pi, PartitionMetrics pm[4]) {
 	f4 averages[4];
-	compute_partition_averages(w, pi, 4, averages);
-	compute_dirs(w, pi, chan_list(0, 1, 2, 3), 4, averages, pm);
+	if (S1) {
+		compute_partition_averages_t<true>(w, pi, 4, averages);
+		compute_dirs_t<true>(w, pi, chan_list(0, 1, 2, 3), 4, averages, pm);
+	} else {
+		compute_partition_averages(w, pi, 4, averages);
+		compute_dirs(w, pi, chan_list(0, 1, 2, 3), 4, averages, pm);
+	}
+}
+ASTC_COOP void compute_avgs_and_dirs_4_comp(WCtx w, const PartView& pi, PartitionMetrics pm[4]) {
+	compute_avgs_and_dirs_4_comp_t<false>(w, pi, pm);
 }
 
 ASTC_COOP void compute_avgs_and_dirs_3_comp(WCtx w, const PartView& pi, unsigned int omitted, PartitionMetrics pm[4]) {
@@ -764,10 +780,18 @@ ASTC_COOP void compute_avgs_and_dirs_3_comp(WCtx w, const PartView& pi, unsigned
 	compute_dirs(w, pi, chan, 3, averages, pm);
 }
 
-ASTC_COOP void compute_avgs_and_dirs_3_comp_rgb(WCtx w, const PartView& pi, PartitionMetrics pm[4]) {
+template <bool S1> ASTC_FN void compute_avgs_and_dirs_3_comp_rgb_t(const WCtx& w, const PartView& pi, PartitionMetrics pm[4]) {
 	f4 averages[4];
-	compute_partition_averages(w, pi, 3, averages);
-	compute_dirs(w, pi, chan_list(0, 1, 2, 2), 3, averages, pm);
+	if (S1) {
+		compute_partition_averages_t<true>(w, pi, 3, averages);
+		compute_dirs_t<true>(w, pi, chan_list(0, 1, 2, 2), 3, averages, pm);
+	} else {
+		compute_partition_averages(w, pi, 3, averages);
+		compute_dirs(w, pi, chan_list(0, 1, 2, 2), 3, averages, pm);
+	}
+}
+ASTC_COOP void compute_avgs_and_dirs_3_comp_rgb(WCtx w, const PartView& pi, PartitionMetrics pm[4]) {
+	compute_avgs_and_dirs_3_comp_rgb_t<false>(w, pi, pm);
 }
 
 ASTC_COOP void compute_avgs_and_dirs_2_comp(WCtx w, const PartView& pt, unsigned int comp1, unsigned int comp2, PartitionMetrics pm[4]) {
@@ -854,9 +878,9 @@ ASTC_COOP void compute_ideal_colors_and_weights_1_comp(WCtx w, const PartView& p
 }
 
 // Projection on the partition lines (shared tail of the 2/3/4 component fits).
-ASTC_COOP void ideal_project(WCtx w, const PartView& pi, int which, const PartitionMetrics pms[4], int ncomp, uint32_t chan, float error_weight,
-                             f4 lowv[4], f4 highv[4]) {
-	unsigned int pc = pi.partition_count;
+template <bool S1> ASTC_FN void ideal_project_t(const WCtx& w, const PartView& pi, int which, const PartitionMetrics pms[4], int ncomp, uint32_t chan,
+                                               float error_weight, f4 lowv[4], f4 highv[4]) {
+	const unsigned int pc = S1 ? 1u : pi.partition_count;
 	SPtr<float> weights = eiw_of(w, which);
 	SPtr<float> wes = eis_of(w, which);
 	SPtr<float> c0 = blk_of(w, (int)(chan & 15)), c1 = blk_of(w, (int)((chan >> 4) & 15)), c2 = blk_of(w, (int)((chan >> 8) & 15)),
@@ -916,6 +940,10 @@ ASTC_COOP void ideal_project(WCtx w, const PartView& pi, int which, const Partit
 	}
 	wsync();
 }
+ASTC_COOP void ideal_project(WCtx w, const PartView& pi, int which, const PartitionMetrics pms[4], int ncomp, uint32_t chan, float error_weight,
+                             f4 lowv[4], f4 highv[4]) {
+	ideal_project_t<false>(w, pi, which, pms, ncomp, chan, error_weight, lowv, highv);
+}
 
 ASTC_COOP void compute_ideal_colors_and_weights_2_comp(WCtx w, const PartView& pi, int which, int ep0slot, int ep1slot, int comp1, int comp2) {   // :217-351
 	f4 cw = bi_of(w).channel_weight;
@@ -939,7 +967,9 @@ ASTC_COOP void compute_ideal_colors_and_weights_2_comp(WCtx w, const PartView& p
 	wsync();
 }
 
-ASTC_COOP void compute_ideal_colors_and_weights_3_comp(WCtx w, const PartView& pi, int which, int ep0slot, int ep1slot, unsigned int omitted) {   // :354-517
+// (S1: only the one-plane fit without alpha, omitted = 3, reaches this instantiation)
+template <bool S1> ASTC_FN void compute_ideal_colors_and_weights_3_comp_t(const WCtx& w, const PartView& pi, int which, int ep0slot, int ep1slot, unsigned int omitted_in) {
+	const unsigned int omitted = S1 ? 3u : omitted_in;
 	f4 cw = bi_of(w).channel_weight;
 	uint32_t chan;
 	float error_weight;
@@ -958,16 +988,22 @@ ASTC_COOP void compute_ideal_colors_and_weights_3_comp(WCtx w, const PartView& p
 	}
 	error_weight = error_weight * (1.0f / 3.0f);
 	PartitionMetrics pms[4];
-	if (omitted == 3) {
+	if (S1) {
+		compute_avgs_and_dirs_3_comp_rgb_t<true>(w, pi, pms);
+	} else if (omitted == 3) {
 		compute_avgs_and_dirs_3_comp_rgb(w, pi, pms);
 	} else {
 		compute_avgs_and_dirs_3_comp(w, pi, omitted, pms);
 	}
 	f4 lowv[4], highv[4];
-	ideal_project(w, pi, which, pms, 3, chan, error_weight, lowv, highv);
+	if (S1) {
+		ideal_project_t<true>(w, pi, which, pms, 3, chan, error_weight, lowv, highv);
+	} else {
+		ideal_project(w, pi, which, pms, 3, chan, error_weight, lowv, highv);
+	}
 	SPtr<f4> ep = ep_of(w);
 	f4 bmin = bi_of(w).data_min, bmax = bi_of(w).data_max;
-	for (unsigned int i = 0; i < pi.partition_count; i++) {
+	for (unsigned int i = 0; i < (S1 ? 1u : pi.partition_count); i++) {
 		f4 e0 = lowv[i], e1 = highv[i];
 		f4 r0, r1;
 		switch (omitted) {
@@ -983,15 +1019,23 @@ ASTC_COOP void compute_ideal_colors_and_weights_3_comp(WCtx w, const PartView& p
 	}
 	wsync();
 }
+ASTC_COOP void compute_ideal_colors_and_weights_3_comp(WCtx w, const PartView& pi, int which, int ep0slot, int ep1slot, unsigned int omitted) {   // :354-517
+	compute_ideal_colors_and_weights_3_comp_t<false>(w, pi, which, ep0slot, ep1slot, omitted);
+}
 
-ASTC_COOP void compute_ideal_colors_and_weights_4_comp(WCtx w, const PartView& pi, int which, int ep0slot, int ep1slot) {   // :520-609
+template <bool S1> ASTC_FN void compute_ideal_colors_and_weights_4_comp_t(const WCtx& w, const PartView& pi, int which, int ep0slot, int ep1slot) {
 	float error_weight = hadd_s(bi_of(w).channel_weight) / 4.0f;
 	PartitionMetrics pms[4];
-	compute_avgs_and_dirs_4_comp(w, pi, pms);
 	f4 lowv[4], highv[4];
-	ideal_project(w, pi, which, pms, 4, chan_list(0, 1, 2, 3), error_weight, lowv, highv);
+	if (S1) {
+		compute_avgs_and_dirs_4_comp_t<true>(w, pi, pms);
+		ideal_project_t<true>(w, pi, which, pms, 4, chan_list(0, 1, 2, 3), error_weight, lowv, highv);
+	} else {
+		compute_avgs_and_dirs_4_comp(w, pi, pms);
+		ideal_project(w, pi, which, pms, 4, chan_list(0, 1, 2, 3), error_weight, lowv, highv);
+	}
 	SPtr<f4> ep = ep_of(w);
-	for (unsigned int i = 0; i < pi.partition_count; i++) {
+	for (unsigned int i = 0; i < (S1 ? 1u : pi.partition_count); i++) {
 		if (w.lane == 0) {
 			ep[ep0slot + (int)i] = lowv[i];
 			ep[ep1slot + (int)i] = highv[i];
@@ -999,14 +1043,27 @@ ASTC_COOP void compute_ideal_colors_and_weights_4_comp(WCtx w, const PartView& p
 	}
 	wsync();
 }
+ASTC_COOP void compute_ideal_colors_and_weights_4_comp(WCtx w, const PartView& pi, int which, int ep0slot, int ep1slot) {   // :520-609
+	compute_ideal_colors_and_weights_4_comp_t<false>(w, pi, which, ep0slot, ep1slot);
+}
 
-ASTC_COOP void compute_ideal_colors_and_weights_1plane(WCtx w, const PartView& pi) {   // :612-627
+// S1: pi is the one-partition view
+template <bool S1> ASTC_FN void compute_ideal_colors_and_weights_1plane_t(const WCtx& w, const PartView& pi) {   // :612-627
 	bool uses_alpha = !is_constant_channel(w, 3);
-	if (uses_alpha) {
+	if (S1) {
+		if (uses_alpha) {
+			compute_ideal_colors_and_weights_4_comp_t<true>(w, pi, 0, EP_EI1_0, EP_EI1_1);
+		} else {
+			compute_ideal_colors_and_weights_3_comp_t<true>(w, pi, 0, EP_EI1_0, EP_EI1_1, 3);
+		}
+	} else if (uses_alpha) {
 		compute_ideal_colors_and_weights_4_comp(w, pi, 0, EP_EI1_0, EP_EI1_1);
 	} else {
 		compute_ideal_colors_and_weights_3_comp(w, pi, 0, EP_EI1_0, EP_EI1_1, 3);
 	}
+}
+ASTC_COOP void compute_ideal_colors_and_weights_1plane(WCtx w, const PartView& pi) {
+	compute_ideal_colors_and_weights_1plane_t<false>(w, pi);
 }
 
 ASTC_COOP void compute_ideal_colors_and_weights_2planes(WCtx w, unsigned int plane2_component) {   // :630-683
@@ -1034,7 +1091,8 @@ ASTC_FN float bilinear_infill(const DecView& di, SPtr<float> weights, int t) {
 
 // compute_ideal_weights_for_decimation (:845-971) for one grid; nplanes = 1 or 2 (second plane: ei slot 1,
 // output W floats further on). Lanes over grid weights / texels; the per-weight sums are chains.
-ASTC_COOP void compute_ideal_weights_for_decimation(WCtx w, unsigned int d, int nplanes) {
+template <bool S1> ASTC_FN void compute_ideal_weights_for_decimation_t(const WCtx& w, unsigned int d, int nplanes_in) {
+	const int nplanes = S1 ? 1 : nplanes_in;
 	DecView di = dec_view(d);
 	int T = di.T;
 	int W = di.W;
@@ -1120,6 +1178,9 @@ ASTC_COOP void compute_ideal_weights_for_decimation(WCtx w, unsigned int d, int 
 	}
 	wsync();
 }
+ASTC_COOP void compute_ideal_weights_for_decimation(WCtx w, unsigned int d, int nplanes) {
+	compute_ideal_weights_for_decimation_t<false>(w, d, nplanes);
+}
 
 // =============================================================================================
 // Angular weight-range search (astcenc_weight_align.cpp:94-355).
@@ -1155,7 +1216,8 @@ ASTC_FN int angular_steps_of(unsigned int d, int nplanes, uint16_t mask, unsigne
 }
 
 // compute_angular_endpoints_1plane / _2planes (:358-500)
-ASTC_COOP void compute_angular_endpoints(WCtx w, bool only_always, int nplanes, unsigned int max_weight_quant) {
+template <bool S1> ASTC_FN void compute_angular_endpoints_t(const WCtx& w, bool only_always, int nplanes_in, unsigned int max_weight_quant) {
+	const int nplanes = S1 ? 1 : nplanes_in;
 	unsigned int max_dm = (nplanes == 1 && only_always) ? BSD.decimation_mode_count_always : BSD.decimation_mode_count_selected;
 	uint16_t mask = (uint16_t)((1u << (max_weight_quant + 1)) - 1);
 	int pairs = (int)max_dm * nplanes;
@@ -1373,6 +1435,9 @@ ASTC_COOP void compute_angular_endpoints(WCtx w, bool only_always, int nplanes, 
 		wsync();
 		pair0 += npair;
 	}
+}
+ASTC_COOP void compute_angular_endpoints(WCtx w, bool only_always, int nplanes, unsigned int max_weight_quant) {
+	compute_angular_endpoints_t<false>(w, only_always, nplanes, max_weight_quant);
 }
 
 // The (low, high) weight range of a packed block mode, including the "snap high to 1.0" rule of

@@ -386,28 +386,44 @@ ASTC_FN bool emit_if_constant(const WCtx& w, unsigned int out_index) {
 }
 
 // ---- trial stages (compress_symbolic_block_for_partition_1plane :353-712 / _2planes :715-1044) ----
-ASTC_COOP void stage_ideal(WCtx w, const Trial& t) {
-	if (t.dual) {
+// Each stage exists in two instantiations of the same source. S1 = false: the general stage, an out-of-line function that reads
+// the trial's shape (partitions, planes, HDR endpoints) at run time. S1 = true: the trial has one partition and one plane in an
+// LDR profile - compile-time facts; the wave-0 set-up inlines this instantiation with the two-plane, n-partition and HDR
+// branches folded away.
+template <bool S1> ASTC_FN void stage_ideal_t(const WCtx& w, const Trial& t) {
+	if (S1) {
+		compute_ideal_colors_and_weights_1plane_t<true>(w, part_view_packed(1, 0));
+	} else if (t.dual) {
 		compute_ideal_colors_and_weights_2planes(w, (unsigned int)t.plane2_component);
 	} else {
 		PartView pi = part_view_packed(t.partition_count, t.packed);
 		compute_ideal_colors_and_weights_1plane(w, pi);
 	}
 }
+ASTC_COOP void stage_ideal(WCtx w, const Trial& t) {
+	stage_ideal_t<false>(w, t);
+}
 
-ASTC_COOP void stage_decimate(WCtx w, const Trial& t) {
-	unsigned int ndm = (!t.dual && t.only_always) ? BSD.decimation_mode_count_always : BSD.decimation_mode_count_selected;
+template <bool S1> ASTC_FN void stage_decimate_t(const WCtx& w, const Trial& t) {
+	unsigned int ndm = ((S1 || !t.dual) && t.only_always) ? BSD.decimation_mode_count_always : BSD.decimation_mode_count_selected;
 	uint16_t refmask = (uint16_t)((1u << (t.max_weight_quant + 1)) - 1);
 	// (one grid after the other: a single pass over the weights of all grids through a slot map was measured slower - the
 	//  per-slot table look-ups cost more than the fuller warps gain)
 	ASTC_NOUNROLL
 	for (unsigned int i = 0; i < ndm; i++) {
-		uint16_t ref = t.dual ? ASTC_LDG(&BSD.dec_modes[i].refprec_2planes) : ASTC_LDG(&BSD.dec_modes[i].refprec_1plane);
+		uint16_t ref = (!S1 && t.dual) ? ASTC_LDG(&BSD.dec_modes[i].refprec_2planes) : ASTC_LDG(&BSD.dec_modes[i].refprec_1plane);
 		if ((ref & refmask) == 0) {
 			continue;
 		}
-		compute_ideal_weights_for_decimation(w, i, t.dual ? 2 : 1);
+		if (S1) {
+			compute_ideal_weights_for_decimation_t<true>(w, i, 1);
+		} else {
+			compute_ideal_weights_for_decimation(w, i, t.dual ? 2 : 1);
+		}
 	}
+}
+ASTC_COOP void stage_decimate(WCtx w, const Trial& t) {
+	stage_decimate_t<false>(w, t);
 }
 
 // weight cut-offs (:430-432 / :791-798) and the block-mode range of the trial
@@ -453,10 +469,19 @@ ASTC_FN void trial_cutoffs(const WCtx& w, Trial& t) {
 	ST_WRITE_END(w)
 }
 
-ASTC_COOP void stage_formats(WCtx w, Trial& t) {
+template <bool S1> ASTC_FN void stage_formats_t(const WCtx& w, Trial& t) {
 	SPtr<f4> ep = ep_of(w);
 	unsigned int count;
-	if (!t.dual) {
+	if (S1) {
+		PartView pi = part_view_packed(1, 0);
+		endpoint_formats_prepare_t<true>(w, pi, EP_EI1_0, EP_EI1_1, 1, t.start_mode, t.end_mode);
+		count = endpoint_formats_select_t<true>(w, 1, 1, t.start_mode, t.end_mode, w.base + A_CAND, false);
+		ASTC_NOUNROLL
+		for (int k = w.lane; k < 4; k += ASTC_WARP) {
+			ep[EP_BASE_0 + k] = ep[EP_EI1_0 + k];
+			ep[EP_BASE_1 + k] = ep[EP_EI1_1 + k];
+		}
+	} else if (!t.dual) {
 		PartView pi = part_view_packed(t.partition_count, t.packed);
 		count = compute_ideal_endpoint_formats(w, pi, EP_EI1_0, EP_EI1_1, 1, t.start_mode, t.end_mode);
 		ASTC_NOUNROLL
@@ -483,6 +508,9 @@ ASTC_COOP void stage_formats(WCtx w, Trial& t) {
 	ST_WRITE_BEGIN(w)
 		t.candidate_count = count;
 	ST_WRITE_END(w)
+}
+ASTC_COOP void stage_formats(WCtx w, Trial& t) {
+	stage_formats_t<false>(w, t);
 }
 
 // Refinement state of the candidate a warp is working on (the loop nest of :504-699 / :886-1044 flattened into steps).

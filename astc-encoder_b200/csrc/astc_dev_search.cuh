@@ -18,8 +18,11 @@
 // (astcenc_compress_symbolic.cpp:434-485 / :803-868 + ideal_endpoints.cpp:688-842, :974-1080).
 // Lanes over block modes; the texel error sum keeps the reference's 4-lane accumulator order per mode.
 // =============================================================================================
-ASTC_COOP void quantize_and_score_modes(WCtx w, unsigned int start_mode, unsigned int end_mode, int nplanes, unsigned int partition_count,
-                                        int max_weight_quant, float min_wt_cutoff1, float min_wt_cutoff2) {
+// S1: one plane and one partition are compile-time facts (the wave-0 set-up of an LDR profile inlines that instantiation)
+template <bool S1> ASTC_FN void quantize_and_score_modes_t(const WCtx& w, unsigned int start_mode, unsigned int end_mode, int nplanes_in,
+                                                          unsigned int partition_count_in, int max_weight_quant, float min_wt_cutoff1, float min_wt_cutoff2) {
+	const int nplanes = S1 ? 1 : nplanes_in;
+	const unsigned int partition_count = S1 ? 1u : partition_count_in;
 	int free_bits = partition_count == 1 ? 115 - 4 : partition_count == 2 ? 111 - 4 - 10 : partition_count == 3 ? 108 - 4 - 10 : 105 - 4 - 10;
 	SPtr<uint8_t> uqrow = sptr<uint8_t>(su_of(w) + (uint32_t)w.lane * UQ_ROW_STRIDE);
 	SPtr<float> mode_err = mode_err_of(w);
@@ -106,6 +109,10 @@ ASTC_COOP void quantize_and_score_modes(WCtx w, unsigned int start_mode, unsigne
 	}
 	wsync();
 }
+ASTC_COOP void quantize_and_score_modes(WCtx w, unsigned int start_mode, unsigned int end_mode, int nplanes, unsigned int partition_count,
+                                        int max_weight_quant, float min_wt_cutoff1, float min_wt_cutoff2) {
+	quantize_and_score_modes_t<false>(w, start_mode, end_mode, nplanes, partition_count, max_weight_quant, min_wt_cutoff1, min_wt_cutoff2);
+}
 
 // =============================================================================================
 // Endpoint format choice (astcenc_pick_best_endpoint_format.cpp)
@@ -134,10 +141,15 @@ struct EfTables {
 // compute_encoding_choice_errors :222-312 with compute_error_squared_rgb_single_partition :72-219.
 // Terms per texel: 0 alpha drop, 1 uncorrelated line, 2 same-chroma line, 3 rgb-luma line, 4 luminance line;
 // one chain per (partition, term, texel index mod 4).
-ASTC_COOP void compute_encoding_choice_errors(WCtx w, const PartView& pi, int ep0slot, int ep1slot, EncodingChoiceErrors eci[4]) {
-	int pc = (int)pi.partition_count;
+// (S1 here and below: one partition, one plane, LDR endpoint formats - see quantize_and_score_modes_t)
+template <bool S1> ASTC_FN void compute_encoding_choice_errors_t(const WCtx& w, const PartView& pi, int ep0slot, int ep1slot, EncodingChoiceErrors eci[4]) {
+	const int pc = S1 ? 1 : (int)pi.partition_count;
 	PartitionMetrics pms[4];
-	compute_avgs_and_dirs_3_comp_rgb(w, pi, pms);
+	if (S1) {
+		compute_avgs_and_dirs_3_comp_rgb_t<true>(w, pi, pms);
+	} else {
+		compute_avgs_and_dirs_3_comp_rgb(w, pi, pms);
+	}
 	SPtr<float> tmpf = tmpf_of(w);
 	SPtr<float> lines = tmpf + 80;          // per partition: uncor.amod[3] uncor.bs[3] samec.bs[3] rgbl.amod[3]
 	if (w.lane == 0) {
@@ -168,7 +180,7 @@ ASTC_COOP void compute_encoding_choice_errors(WCtx w, const PartView& pi, int ep
 	const float u3 = 0.577350258827209473f;
 	chain_sums<5>(w, w.T, su_of(w), tmpf, nchains,
 		[&](int pos, float* term) {
-			int t = pv_texel(pi, pos);
+			int t = S1 ? pos : pv_texel(pi, pos);
 			int p = pc > 1 ? (int)ASTC_LDG(&pi.partition_of_texel[t]) : 0;
 			SPtr<float> l = lines + p * 12;
 			float dr = br[t], dg = bg[t], db = bb[t];
@@ -230,6 +242,9 @@ ASTC_COOP void compute_encoding_choice_errors(WCtx w, const PartView& pi, int ep
 	}
 	wsync();
 }
+ASTC_COOP void compute_encoding_choice_errors(WCtx w, const PartView& pi, int ep0slot, int ep1slot, EncodingChoiceErrors eci[4]) {
+	compute_encoding_choice_errors_t<false>(w, pi, ep0slot, ep1slot, eci);
+}
 
 // 5^2 7^2 9^2 11^2 15^2 19^2 23^2 31^2 39^2 47^2 63^2 79^2 95^2 127^2 159^2 191^2 255^2: (levels - 1)^2 from QUANT_6 up
 ASTC_FN float quant_den(int q) {
@@ -238,6 +253,8 @@ ASTC_FN float quant_den(int q) {
 }
 
 // compute_color_error_for_every_integer_count_and_quant_level :315-675. Lanes over quant levels.
+// (the one-partition, one-plane set-up calls this out-of-line function too: as an inlined template instantiation the general
+// function compiled to different code)
 ASTC_COOP void compute_color_error_tables(WCtx w, int partition_size, int partition_index, const EncodingChoiceErrors& eci, int ep0slot, int ep1slot) {
 	const BlkInfo& bi = bi_of(w);
 	EfTables& ef = EF_OF(w);
@@ -443,10 +460,11 @@ ASTC_COOP void multi_partition_find_best_combination(WCtx w, int pc) {
 }
 
 // one_partition_/N-partition _find_best_combination_for_bitcount (:678-725, :768-1093)
-ASTC_NOINLINE float find_best_combination_for_bitcount(int pc, uint32_t ef_off, int bits_available, uint8_t& best_quant_level, uint8_t& best_quant_level_mod, uint8_t* best_formats) {
+template <bool S1> ASTC_FN float find_best_combination_for_bitcount_t(int pc, uint32_t ef_off, int bits_available, uint8_t& best_quant_level, uint8_t& best_quant_level_mod,
+                                                                 uint8_t* best_formats) {
 	const DevConstTables* ct = ASTC_CT;
 	const EfTables& ef = *reinterpret_cast<const EfTables*>(astc_smem + ef_off);
-	if (pc == 1) {
+	if (S1 || pc == 1) {
 		int best_integer_count = 0;
 		float best_integer_count_error = ERROR_CALC_DEFAULT;
 		ASTC_NOUNROLL
@@ -502,6 +520,9 @@ ASTC_NOINLINE float find_best_combination_for_bitcount(int pc, uint32_t ef_off, 
 	}
 	return best_integer_count_error;
 }
+ASTC_NOINLINE float find_best_combination_for_bitcount(int pc, uint32_t ef_off, int bits_available, uint8_t& best_quant_level, uint8_t& best_quant_level_mod, uint8_t* best_formats) {
+	return find_best_combination_for_bitcount_t<false>(pc, ef_off, bits_available, best_quant_level, best_quant_level_mod, best_formats);
+}
 
 // candidate record kept in the arena (8 bytes each)
 struct Candidate {
@@ -518,13 +539,19 @@ ASTC_FN int mode_bitcount(int weight_bits, int nplanes, int pc) {
 
 // compute_ideal_endpoint_formats :1096-1357, in two parts.
 // Part 1: error tables + the total error of every block mode in [start, end) (overwrites the weight error in place).
-ASTC_COOP void endpoint_formats_prepare(WCtx w, const PartView& pi, int ep0slot, int ep1slot, int nplanes,
-                                        unsigned int start_block_mode, unsigned int end_block_mode) {
-	int pc = (int)pi.partition_count;
+template <bool S1> ASTC_FN void endpoint_formats_prepare_t(const WCtx& w, const PartView& pi, int ep0slot, int ep1slot, int nplanes_in,
+                                                          unsigned int start_block_mode, unsigned int end_block_mode) {
+	const int pc = S1 ? 1 : (int)pi.partition_count;
+	const int nplanes = S1 ? 1 : nplanes_in;
 	EncodingChoiceErrors eci[4];
-	compute_encoding_choice_errors(w, pi, ep0slot, ep1slot, eci);
-	for (int i = 0; i < pc; i++) {
-		compute_color_error_tables(w, pv_count(pi, (unsigned int)i), i, eci[i], ep0slot, ep1slot);
+	if (S1) {
+		compute_encoding_choice_errors_t<true>(w, pi, ep0slot, ep1slot, eci);
+		compute_color_error_tables(w, pv_count(pi, 0), 0, eci[0], ep0slot, ep1slot);
+	} else {
+		compute_encoding_choice_errors(w, pi, ep0slot, ep1slot, eci);
+		for (int i = 0; i < pc; i++) {
+			compute_color_error_tables(w, pv_count(pi, (unsigned int)i), i, eci[i], ep0slot, ep1slot);
+		}
 	}
 	if (pc >= 2) {
 		multi_partition_find_best_combination(w, pc);
@@ -539,16 +566,24 @@ ASTC_COOP void endpoint_formats_prepare(WCtx w, const PartView& pi, int ep0slot,
 			continue;
 		}
 		uint8_t ql, qlm, fmts[4];
-		float error_of_best = find_best_combination_for_bitcount(pc, ef_off, mode_bitcount(ASTC_LDG(&BSD.block_modes[i].weight_bits), nplanes, pc), ql, qlm, fmts);
+		int bits = mode_bitcount(ASTC_LDG(&BSD.block_modes[i].weight_bits), nplanes, pc);
+		float error_of_best = S1 ? find_best_combination_for_bitcount_t<true>(1, ef_off, bits, ql, qlm, fmts)
+		                         : find_best_combination_for_bitcount(pc, ef_off, bits, ql, qlm, fmts);
 		mode_err[(int)i] = error_of_best + qwt;
 	}
 	wsync();
 }
+ASTC_COOP void endpoint_formats_prepare(WCtx w, const PartView& pi, int ep0slot, int ep1slot, int nplanes,
+                                        unsigned int start_block_mode, unsigned int end_block_mode) {
+	endpoint_formats_prepare_t<false>(w, pi, ep0slot, ep1slot, nplanes, start_block_mode, end_block_mode);
+}
 
 // Part 2: the tune_candidate_limit lowest totals of [start, end), lowest index first among equals (:1286-1333), written
 // to the Candidate array at cand_off. With keep_errors the totals survive (a second selection over another range follows).
-ASTC_COOP unsigned int endpoint_formats_select(WCtx w, int pc, int nplanes, unsigned int start_block_mode, unsigned int end_block_mode,
-                                               uint32_t cand_off, bool keep_errors) {
+template <bool S1> ASTC_FN unsigned int endpoint_formats_select_t(const WCtx& w, int pc_in, int nplanes_in, unsigned int start_block_mode, unsigned int end_block_mode,
+                                                                 uint32_t cand_off, bool keep_errors) {
+	const int pc = S1 ? 1 : pc_in;
+	const int nplanes = S1 ? 1 : nplanes_in;
 	uint32_t ef_off = su_of(w);
 	SPtr<float> mode_err = mode_err_of(w);
 	unsigned int limit = CFG.tune_candidate_limit;
@@ -586,7 +621,12 @@ ASTC_COOP unsigned int endpoint_formats_select(WCtx w, int pc, int nplanes, unsi
 		Candidate c;
 		c.block_mode = (uint16_t)best_idx;
 		c.formats[0] = c.formats[1] = c.formats[2] = c.formats[3] = 0;
-		find_best_combination_for_bitcount(pc, ef_off, mode_bitcount(ASTC_LDG(&BSD.block_modes[best_idx].weight_bits), nplanes, pc), c.quant_level, c.quant_level_mod, c.formats);
+		int bits = mode_bitcount(ASTC_LDG(&BSD.block_modes[best_idx].weight_bits), nplanes, pc);
+		if (S1) {
+			find_best_combination_for_bitcount_t<true>(1, ef_off, bits, c.quant_level, c.quant_level_mod, c.formats);
+		} else {
+			find_best_combination_for_bitcount(pc, ef_off, bits, c.quant_level, c.quant_level_mod, c.formats);
+		}
 		cands[(int)k] = c;
 	}
 	wsync();
@@ -597,6 +637,10 @@ ASTC_COOP unsigned int endpoint_formats_select(WCtx w, int pc, int nplanes, unsi
 	}
 	wsync();
 	return count;
+}
+ASTC_COOP unsigned int endpoint_formats_select(WCtx w, int pc, int nplanes, unsigned int start_block_mode, unsigned int end_block_mode,
+                                               uint32_t cand_off, bool keep_errors) {
+	return endpoint_formats_select_t<false>(w, pc, nplanes, start_block_mode, end_block_mode, cand_off, keep_errors);
 }
 
 ASTC_COOP unsigned int compute_ideal_endpoint_formats(WCtx w, const PartView& pi, int ep0slot, int ep1slot, int nplanes,

@@ -327,8 +327,12 @@ __device__ __forceinline__ void stat_hist(int part, long long cycles) {
 
 // ---------------------------------------------------------------------------------------------
 // S: trial setup. Wave 0 reads the image (load_block, constant-colour blocks are emitted on the spot).
+// S1 = true: the wave-0 launches of an LDR profile. The first trial of every block has one partition and one plane, so its
+// stages run the S1 instantiation (astc_dev_lockstep.cuh, "trial stages"), inlined here; a trial of another shape would take
+// the general stages.
 // ---------------------------------------------------------------------------------------------
-ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
+template <bool S1>
+ASTC_COOP void wave_setup_t(WCtx w, WaveArgs a) {
 	// one copy of the search state per warp, in the arena slots the record keeps it in (discipline: astc_dev_lockstep.cuh,
 	// "THE SEARCH STATE ..."); the widened copy of the trial used by the shared set-up sits in the work / mod colour slots,
 	// which only refinement uses
@@ -390,6 +394,8 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 		// errors of the shared modes are identical (compress_symbolic.cpp:1243-1270 runs the same code twice).
 		// One set-up over the full range therefore serves both; the second candidate list waits in A_CAND2.
 		bool shared = active && !t.dual && t.only_always && t.partition_count == 1;
+		// (the restored trial's own shape is checked too: only a one-partition, one-plane trial may run the folded stages)
+		const bool s1 = S1 && active && !t.dual && t.partition_count == 1;
 		if (active) {
 			ST_WRITE_BEGIN(w)
 				tf = t;
@@ -398,19 +404,29 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 				}
 			ST_WRITE_END(w)
 		}
-		if (active) stage_ideal(w, tf);
-		STAT_T(s1);
+		if (active) {
+			if (s1) stage_ideal_t<true>(w, tf);
+			else stage_ideal(w, tf);
+		}
+		STAT_T(st1);
 		if (a.sync_mask & 1) cta_sync();
-		if (active) stage_decimate(w, tf);
+		if (active) {
+			if (s1) stage_decimate_t<true>(w, tf);
+			else stage_decimate(w, tf);
+		}
 		STAT_T(s2);
 		if (a.sync_mask & 2) cta_sync();
 		if (active) {
 			trial_cutoffs(w, tf);
-			compute_angular_endpoints(w, tf.only_always != 0, tf.dual ? 2 : 1, (unsigned int)tf.max_weight_quant);
+			if (s1) compute_angular_endpoints_t<true>(w, tf.only_always != 0, 1, (unsigned int)tf.max_weight_quant);
+			else compute_angular_endpoints(w, tf.only_always != 0, tf.dual ? 2 : 1, (unsigned int)tf.max_weight_quant);
 		}
 		STAT_T(s3);
 		if (a.sync_mask & 4) cta_sync();
-		if (active) quantize_and_score_modes(w, tf.start_mode, tf.end_mode, tf.dual ? 2 : 1, tf.partition_count, tf.max_weight_quant, tf.cutoff1, tf.cutoff2);
+		if (active) {
+			if (s1) quantize_and_score_modes_t<true>(w, tf.start_mode, tf.end_mode, 1, 1, tf.max_weight_quant, tf.cutoff1, tf.cutoff2);
+			else quantize_and_score_modes(w, tf.start_mode, tf.end_mode, tf.dual ? 2 : 1, tf.partition_count, tf.max_weight_quant, tf.cutoff1, tf.cutoff2);
+		}
 		STAT_T(s4);
 		if (a.sync_mask & 8) cta_sync();
 		STAT_T(s4b);
@@ -420,9 +436,15 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 				PartView pi = part_view_packed(1, 0);
 				SPtr<f4> ep = ep_of(w);
 				unsigned int end_full = tf.end_mode;
-				endpoint_formats_prepare(w, pi, EP_EI1_0, EP_EI1_1, 1, 0, end_full);
-				count = endpoint_formats_select(w, 1, 1, 0, BSD.block_mode_count_1plane_always, w.base + A_CAND, true);
-				count_next = endpoint_formats_select(w, 1, 1, 0, end_full, w.base + A_CAND2, false);
+				if (s1) {
+					endpoint_formats_prepare_t<true>(w, pi, EP_EI1_0, EP_EI1_1, 1, 0, end_full);
+					count = endpoint_formats_select_t<true>(w, 1, 1, 0, BSD.block_mode_count_1plane_always, w.base + A_CAND, true);
+					count_next = endpoint_formats_select_t<true>(w, 1, 1, 0, end_full, w.base + A_CAND2, false);
+				} else {
+					endpoint_formats_prepare(w, pi, EP_EI1_0, EP_EI1_1, 1, 0, end_full);
+					count = endpoint_formats_select(w, 1, 1, 0, BSD.block_mode_count_1plane_always, w.base + A_CAND, true);
+					count_next = endpoint_formats_select(w, 1, 1, 0, end_full, w.base + A_CAND2, false);
+				}
 				ASTC_NOUNROLL
 				for (int k = w.lane; k < 4; k += ASTC_WARP) {
 					ep[EP_BASE_0 + k] = ep[EP_EI1_0 + k];
@@ -440,11 +462,12 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 				}
 			ST_WRITE_END(w)
 			if (!shared) {
-				stage_formats(w, t);
+				if (s1) stage_formats_t<true>(w, t);
+				else stage_formats(w, t);
 			}
 			// the refinement kernel has no decimated ideal weights: quantise every candidate's weights now, straight into the
 			// candidates' slots (unused bytes of a slot are never read), one barrier at the end
-			int nplanes = t.dual ? 2 : 1;
+			int nplanes = s1 ? 1 : (t.dual ? 2 : 1);
 			float cutoff1 = t.cutoff1, cutoff2 = t.cutoff2;
 			ASTC_NOUNROLL
 			for (int list = 0; list < 2; list++) {
@@ -466,8 +489,8 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 			if (w.lane == 0) {
 				long long s6 = clock64();
 				int kind = t.dual ? 1 : (t.partition_count > 1 ? 2 : 0);
-				atomicAdd(&g_setup_stats[kind][0], (unsigned long long)(s1 - s0));
-				atomicAdd(&g_setup_stats[kind][1], (unsigned long long)(s2 - s1));
+				atomicAdd(&g_setup_stats[kind][0], (unsigned long long)(st1 - s0));
+				atomicAdd(&g_setup_stats[kind][1], (unsigned long long)(s2 - st1));
 				atomicAdd(&g_setup_stats[kind][2], (unsigned long long)(s3 - s2));
 				atomicAdd(&g_setup_stats[kind][3], (unsigned long long)(s4 - s3));
 				atomicAdd(&g_setup_stats[kind][4], (unsigned long long)(s5 - s4b));
@@ -490,6 +513,16 @@ ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
 			}
 #endif
 		}
+	}
+}
+
+// which instantiation a set-up launch of wave a.wave runs: S1 for wave 0 of an LDR or sRGB profile, the general one otherwise
+// (the rule the host code applies when it picks the set-up kernel, astcenc_b200.cu setup_kernel; the host simulation calls this)
+ASTC_COOP void wave_setup(WCtx w, WaveArgs a) {
+	if (a.wave == 0 && (CFG.profile == PRF_LDR || CFG.profile == PRF_LDR_SRGB)) {
+		wave_setup_t<true>(w, a);
+	} else {
+		wave_setup_t<false>(w, a);
 	}
 }
 

@@ -123,6 +123,10 @@ static __device__ __forceinline__ bool wave_setup_queues_empty(const WaveArgs& a
 #endif
 #define ASTC_EMIT_THREADS 256
 
+// Two instantiations: S1 = true for the wave-0 launches of the LDR profiles (the first trial of every block, one partition and
+// one plane, runs the specialised set-up stages inlined beside the general ones), false for every later wave and for the HDR
+// profiles - their kernel carries the general stages alone, laid out as it was before the specialised stages existed.
+template <bool S1>
 __global__ void __launch_bounds__(ASTC_SETUP_THREADS_MAX, 1)
 astc_wave_setup_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img, const __grid_constant__ WaveArgs a) {
 	if (a.wave != 0 && wave_setup_queues_empty(a)) {
@@ -135,7 +139,7 @@ astc_wave_setup_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant
 	w.lane = threadIdx.x & 31;
 	w.base = ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + a.stage_bytes_setup + (uint32_t)(threadIdx.x >> 5) * bsd.arena_bytes;
 	w.T = bsd.texel_count;
-	wave_setup(w, a);
+	wave_setup_t<S1>(w, a);
 }
 
 #ifndef ASTC_REFINE_MIN_CTAS
@@ -161,6 +165,11 @@ astc_wave_refine_kernel(const __grid_constant__ DevBsd bsd, const __grid_constan
 
 // which refinement kernel a context launches
 static inline bool refine_l1_step(const DevConfig& cfg) { return cfg.profile == PRF_LDR || cfg.profile == PRF_LDR_SRGB; }
+// which set-up kernel a launch of wave `wave` takes (the same profiles as the refinement kernel, wave 0 only)
+typedef void (*SetupKernel)(const DevBsd, const DevConfig, const DevImage, const WaveArgs);
+static inline SetupKernel setup_kernel(const DevConfig& cfg, int wave) {
+	return (wave == 0 && refine_l1_step(cfg)) ? astc_wave_setup_kernel<true> : astc_wave_setup_kernel<false>;
+}
 
 __global__ void __launch_bounds__(ASTC_REFINE_THREADS_MAX, 1)
 astc_wave_prepare_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img, const __grid_constant__ WaveArgs a) {
@@ -690,7 +699,8 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 			}
 			ctx->smem_small = ASTC_SMEM_HDR + arena_small * wr;
 			ctx->smem_refine = ASTC_SMEM_HDR + ctx->refine_stage_bytes + arena_small * wr + (size_t)ASTC_REFINE_STATE_BYTES * wr;
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
@@ -963,16 +973,16 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d
 				if (wave != 0) {
 					a[p].cls_lo = 0;
 					a[p].cls_hi = 1;
-					astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
+					astc_wave_setup_kernel<false><<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
 					ctx->launches++;
 					a[p].cls_lo = 1;
 					a[p].cls_hi = ASTC_Q_CLASSES;
 				}
-				astc_wave_setup_kernel<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, ps>>>(ctx->tables->bsd_1p, ctx->dcfg, img[p], a[p]);
+				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, ps>>>(ctx->tables->bsd_1p, ctx->dcfg, img[p], a[p]);
 				a[p].cls_lo = 0;
 				a[p].cls_hi = ASTC_Q_CLASSES;
 			} else {
-				astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
+				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
 			}
 			if (refine_l1_step(ctx->dcfg)) {
 				astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
@@ -1187,9 +1197,9 @@ static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, in
 					a.first_block = row * img.blocks_x;
 					a.band_blocks = (row_end - row) * img.blocks_x;
 					if (ctx->warps_setup_1p) {
-						astc_wave_setup_kernel<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
+						setup_kernel(ctx->dcfg, 0)<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
 					} else {
-						astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
+						setup_kernel(ctx->dcfg, 0)<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
 					}
 					ctx->launches++;
 					row = row_end;
@@ -1202,17 +1212,17 @@ static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, in
 				if (wave != 0) {
 					a.cls_lo = 0;
 					a.cls_hi = 1;
-					astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
+					astc_wave_setup_kernel<false><<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
 					ctx->launches++;
 					a.cls_lo = 1;
 					a.cls_hi = ASTC_Q_CLASSES;
 				}
-				astc_wave_setup_kernel<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
+				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
 				a.cls_lo = 0;
 				a.cls_hi = ASTC_Q_CLASSES;
 				mark(0);
 			} else {
-				astc_wave_setup_kernel<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
+				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
 				mark(0);
 			}
 			if (refine_l1_step(ctx->dcfg)) {

@@ -229,17 +229,10 @@ class Context:
 
     def compress_image(self, img, swizzle=(0, 1, 2, 3), out=None, thread_index=0):
         """Host-pointer path: img is a (H, W, 4) or (D, H, W, 4) numpy array of uint8 / float16 / float32."""
-        img = np.ascontiguousarray(img)
-        if img.ndim == 3:
-            img = img[None]
-        d, h, w = img.shape[:3]
-        slices = (C.c_void_p * d)(*[img[z].ctypes.data for z in range(d)])
-        image = Image(w, h, d, _DTYPES[img.dtype], slices)
+        img, slices, image, nbytes = self._image(img)
         sw = Swizzle(*swizzle)
-        nbx, nby = self.blocks(w, h)
-        bz = max(1, self.config.block_z)      # 3D block sizes: blocks come out in (z, y, x) order
         if out is None:
-            out = np.empty(nbx * nby * ((d + bz - 1) // bz) * 16, dtype=np.uint8)
+            out = np.empty(nbytes, dtype=np.uint8)
         err = lib().astcenc_compress_image(self.handle, C.byref(image), C.byref(sw), out.ctypes.data, out.nbytes, thread_index)
         if err:
             raise AstcencError(err, "astcenc_compress_image")
@@ -290,17 +283,25 @@ class Context:
             raise AstcencError(err, "astcenc_b200_slab_rows")
         return a.value, n.value
 
-    def compress_image_sharded(self, img, out=None, root=0, swizzle=(0, 1, 2, 3)):
-        """Slab mode (collective): every rank passes the same (H, W, 4) image; the root gets the whole payload in `out`."""
+    def _image(self, img):
+        """(H, W, 4) or (D, H, W, 4) numpy array -> (contiguous array, slice pointers, Image, payload bytes)."""
         img = np.ascontiguousarray(img)
-        h, w = img.shape[:2]
-        slices = (C.c_void_p * 1)(img.ctypes.data)
-        image = Image(w, h, 1, _DTYPES[img.dtype], slices)
-        sw = Swizzle(*swizzle)
+        if img.ndim == 3:
+            img = img[None]
+        d, h, w = img.shape[:3]
+        slices = (C.c_void_p * d)(*[img[z].ctypes.data for z in range(d)])
         nbx, nby = self.blocks(w, h)
+        bz = max(1, self.config.block_z)      # 3D block sizes: blocks come out in (z, y, x) order
+        return img, slices, Image(w, h, d, _DTYPES[img.dtype], slices), nbx * nby * ((d + bz - 1) // bz) * 16
+
+    def compress_image_sharded(self, img, out=None, root=0, swizzle=(0, 1, 2, 3)):
+        """Slab mode (collective): every rank passes the same (H, W, 4) image or (D, H, W, 4) volume / texture array; the root
+        gets the whole payload in `out`."""
+        img, slices, image, nbytes = self._image(img)
+        sw = Swizzle(*swizzle)
         is_root = getattr(self, "rank", 0) == root
         if out is None and is_root:
-            out = np.empty(nbx * nby * 16, dtype=np.uint8)
+            out = np.empty(nbytes, dtype=np.uint8)
         err = lib().astcenc_b200_compress_image_sharded(self.handle, C.byref(image), C.byref(sw), out.ctypes.data if out is not None else None,
                                                         out.nbytes if out is not None else 0, root)
         if err:
@@ -308,16 +309,14 @@ class Context:
         return out
 
     def compress_batch(self, images, outs=None, root=0, swizzle=(0, 1, 2, 3)):
-        """Batch mode (collective): images[i] (None for images of other ranks) -> outs[i] on the root."""
+        """Batch mode (collective): images[i] ((H, W, 4) or (D, H, W, 4); None for images of other ranks) -> outs[i] on the root."""
         n = len(images)
         keep = []
         ptrs = (C.POINTER(Image) * n)()
         for i, im in enumerate(images):
             if im is None:
                 continue
-            im = np.ascontiguousarray(im)
-            slices = (C.c_void_p * 1)(im.ctypes.data)
-            st = Image(im.shape[1], im.shape[0], 1, _DTYPES[im.dtype], slices)
+            im, slices, st, _ = self._image(im)
             keep.append((im, slices, st))
             ptrs[i] = C.pointer(st)
         sw = Swizzle(*swizzle)

@@ -119,6 +119,28 @@ ASTC_FN void alpha_average_tile(const DevImage& img, unsigned int radius, unsign
 	cta_sync();
 }
 
+// The pre-pass window of image rows [y0, y1) (a slab's rows, y0 < y1 <= dim_y): tile rows [tile_row0, tile_row0 + tile_rows) of
+// the 32 x 32 grid cover them, and those tiles read image rows [read_row0, read_row1). The grid stays anchored at (0, 0) for
+// every slab: a texel's average depends on its whole padded tile (the prefix sums' association order follows padsize), so a
+// shifted grid would change the bytes. A pass over the slab needs the averages of its own texels only, which the window's
+// tiles write; outside the read rows the image may hold anything.
+struct AlphaWindow {
+	unsigned int tile_row0, tile_rows;
+	unsigned int read_row0, read_row1;
+};
+
+static inline AlphaWindow alpha_window(unsigned int dim_y, unsigned int radius, unsigned int y0, unsigned int y1) {
+	AlphaWindow w;
+	unsigned int t1 = (y1 + ALPHA_TILE - 1) / ALPHA_TILE;
+	w.tile_row0 = y0 / ALPHA_TILE;
+	w.tile_rows = t1 - w.tile_row0;
+	// alpha_average_tile clamps its source rows to [0, dim_y - 1]: the first tile reads from oy - r, the last up to oy + size_y + r - 1
+	size_t lo = (size_t)w.tile_row0 * ALPHA_TILE, hi = (size_t)t1 * ALPHA_TILE + radius;
+	w.read_row0 = lo > radius ? (unsigned int)(lo - radius) : 0u;
+	w.read_row1 = hi < dim_y ? (unsigned int)hi : dim_y;
+	return w;
+}
+
 // Alpha-scale RDO test of one block (astcenc_entry.cpp:973-1003): false = no texel of the block has an alpha average above
 // the threshold, the block is emitted as constant zero without looking at it.
 ASTC_FN bool block_has_alpha(const WCtx& w, const float* averages, float threshold, unsigned int pos_x, unsigned int pos_y) {

@@ -195,15 +195,17 @@ astc_wave_emit_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant_
 }
 
 // ---- alpha-scale pre-pass (SURVEY.md section 8f): one CTA per 32 x 32 tile ----
+// The grid covers tile rows [tile_row0, tile_row0 + gridDim.x / tiles_x): the window of one slab (alpha_window).
 #define ASTC_ALPHA_THREADS 128
 __global__ void __launch_bounds__(ASTC_ALPHA_THREADS, 1)
-astc_alpha_average_kernel(const __grid_constant__ DevImage img, unsigned int radius, unsigned int tiles_x, float* __restrict__ averages) {
+astc_alpha_average_kernel(const __grid_constant__ DevImage img, unsigned int radius, unsigned int tiles_x, unsigned int tile_row0, float* __restrict__ averages) {
 	// (a cancelled pass reads no averages: wave 0 finds the same raised flag)
 	if (img.cancel != nullptr && __syncthreads_or(threadIdx.x == 0 && pass_cancelled(img.cancel) ? 1 : 0)) {
 		return;
 	}
 	unsigned int ty = blockIdx.x / tiles_x;
 	unsigned int tx = blockIdx.x - ty * tiles_x;
+	ty += tile_row0;
 	alpha_average_tile(img, radius, tx * ALPHA_TILE, ty * ALPHA_TILE, 0, averages, (int)threadIdx.x, (int)blockDim.x);
 }
 
@@ -865,8 +867,24 @@ static astcenc_error launch_slab(astcenc_context* ctx, const void* d_pixels, int
 	return st;
 }
 
-static astcenc_error upload_whole(astcenc_context* ctx, const UploadPlan& up, unsigned int dim_y, cudaStream_t stream) {
-	CUDA_TRY(cudaMemcpyAsync(up.device, up.host, up.row_bytes * dim_y, cudaMemcpyHostToDevice, ctx->copy_stream), return ASTCENC_ERR_BAD_CONTEXT);
+// Image rows [y0, y1) that a pass over block rows [block_row0, block_row0 + block_rows) of a 2D image reads: the slab's own
+// rows, or with alpha-scale the rows its pre-pass window reads (a superset of them).
+static void slab_image_rows(const astcenc_context* ctx, unsigned int dim_y, unsigned int block_row0, unsigned int block_rows, size_t& y0, size_t& y1) {
+	const unsigned int by = ctx->tables->bsd.dim_y;
+	y0 = (size_t)block_row0 * by;
+	y1 = (size_t)(block_row0 + block_rows) * by;
+	if (y1 > dim_y) y1 = dim_y;
+	const unsigned int radius = ctx->tables->bsd.dim_z > 1 ? 0 : ctx->config.a_scale_radius;
+	if (radius != 0 && y1 > y0) {
+		AlphaWindow w = alpha_window(dim_y, radius, (unsigned int)y0, (unsigned int)y1);
+		y0 = w.read_row0;
+		y1 = w.read_row1;
+	}
+}
+
+static astcenc_error upload_rows(astcenc_context* ctx, const UploadPlan& up, size_t y0, size_t y1, cudaStream_t stream) {
+	CUDA_TRY(cudaMemcpyAsync(up.device + y0 * up.row_bytes, up.host + y0 * up.row_bytes, up.row_bytes * (y1 - y0), cudaMemcpyHostToDevice, ctx->copy_stream),
+	         return ASTCENC_ERR_BAD_CONTEXT);
 	CUDA_TRY(cudaEventRecord(ctx->band_ready[0], ctx->copy_stream), return ASTCENC_ERR_BAD_CONTEXT);
 	CUDA_TRY(cudaStreamWaitEvent(stream, ctx->band_ready[0], 0), return ASTCENC_ERR_BAD_CONTEXT);
 	return ASTCENC_SUCCESS;
@@ -1019,22 +1037,24 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 	int pipes = ctx->knobs.pipes;
 	bool use_pipes = pipes > 1 && ctx->driver == 0 && !ctx->stage_timing && single_batch && block_rows >= (unsigned int)pipes * 4 &&
 	                 blocks_x * block_rows >= (size_t)pipes * 8192;
-	// banded uploads need the whole slab in one batch on the wave pipeline, and no pre-pass that reads the whole image first
+	// banded uploads need the whole slab in one batch on the wave pipeline, and no pre-pass that reads the window first
 	bool banded = up != nullptr && radius == 0 && ctx->driver == 0 && single_batch && (use_pipes || (up->bands > 1 && block_rows >= (unsigned int)up->bands * 4));
 	if (up != nullptr && !banded) {
 		// the upload streams on the copy stream; it must not overtake a pass that still reads the image buffer
 		if (ctx->scratch_used) {
 			CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 		}
-		astcenc_error st = upload_whole(ctx, *up, dim_y, stream);
+		size_t y0, y1;
+		slab_image_rows(ctx, dim_y, block_row0, block_rows, y0, y1);
+		astcenc_error st = upload_rows(ctx, *up, y0, y1, stream);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
 		up = nullptr;
 	}
 	if (radius != 0) {
-		// alpha-scale pre-pass over the whole image (every slab needs the averages of its own texels only, but the
-		// box filter reaches across slab borders, so the pass always reads the full image)
+		// alpha-scale pre-pass over the tiles that cover the slab's rows: the box filter reaches across slab borders, so
+		// the window reads up to `radius` rows beyond the tiles (alpha_window); the averages stay at their image positions
 		size_t need = (size_t)dim_x * dim_y * sizeof(float);
 		if (need > ctx->d_alpha_bytes) {
 			cudaFree(ctx->d_alpha);
@@ -1060,8 +1080,10 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 			aimg.swz[i] = swz[i];
 		}
 		aimg.cancel = ctx->pass_cancel;
-		unsigned int tiles_x = (dim_x + ALPHA_TILE - 1) / ALPHA_TILE, tiles_y = (dim_y + ALPHA_TILE - 1) / ALPHA_TILE;
-		astc_alpha_average_kernel<<<tiles_x * tiles_y, ASTC_ALPHA_THREADS, smem, stream>>>(aimg, radius, tiles_x, ctx->d_alpha);
+		unsigned int tiles_x = (dim_x + ALPHA_TILE - 1) / ALPHA_TILE;
+		size_t y1 = (size_t)(block_row0 + block_rows) * bsd.dim_y;
+		AlphaWindow win = alpha_window(dim_y, radius, block_row0 * bsd.dim_y, y1 < dim_y ? (unsigned int)y1 : dim_y);
+		astc_alpha_average_kernel<<<tiles_x * win.tile_rows, ASTC_ALPHA_THREADS, smem, stream>>>(aimg, radius, tiles_x, win.tile_row0, ctx->d_alpha);
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		ctx->launches++;
 		// astcenc_entry.cpp:983-988

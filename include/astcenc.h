@@ -196,8 +196,12 @@ ASTCENC_PUBLIC const char* astcenc_get_error_string(enum astcenc_error status);
  *  - Block sizes: the fourteen 2D and the ten 3D footprints (block_z > 1: 3x3x3 .. 6x6x6, astcenc_block_sizes.cpp:1025). With a
  *    3D block size the slices of astcenc_image::data are uploaded into one volume and compressed in one pass, blocks in
  *    (z, y, x) order like the reference's (astcenc_entry.cpp:1036); a_scale_radius is ignored like the reference does
- *    (astcenc_entry.cpp:975). The astcenc_b200_* device-resident and multi-GPU entry points take 2D block sizes only
- *    (ASTCENC_ERR_NOT_IMPLEMENTED otherwise).
+ *    (astcenc_entry.cpp:975). The multi-GPU entry points (slab and batch mode) take the same images: 2D, texture arrays and
+ *    volumes. The device-resident entry astcenc_b200_compress_device and astcenc_b200_slab_rows stay 2D (3D block sizes:
+ *    ASTCENC_ERR_NOT_IMPLEMENTED).
+ *  - a_scale_radius with a 2D block size and dim_z > 1 gives ASTCENC_ERR_NOT_IMPLEMENTED from every compressing entry point.
+ *    The alpha-scale pre-pass of a pass over some block rows filters only the 32 x 32 tiles that cover those rows, and reads
+ *    the image rows of those tiles plus a_scale_radius rows on either side; nothing else of the image is read.
  *  - A context owns ONE set of search scratch buffers: passes of the same context are serialised - on the host by a mutex,
  *    on the device by an event chain - whatever streams they are enqueued on. Use one context per concurrent stream.
  */
@@ -219,15 +223,20 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device(struct astcenc_co
  *
  * astcenc_b200_comm_unique_id   rank 0 makes the 128-byte rendezvous id; the caller ships it to the other ranks
  * astcenc_b200_comm_init        collective: joins `world` ranks (world == 1: no communicator, the calls below run locally)
- * astcenc_b200_slab_rows        the block rows [first, first + rows) rank `rank` of `world` owns for an image of height dim_y
+ * astcenc_b200_slab_rows        the block rows [first, first + rows) rank `rank` of `world` owns for a 2D image of height dim_y
  * astcenc_b200_compress_image_sharded
- *     collective, SLAB MODE: every rank passes the same 2D image (host pointer, only the rows of its own slab are read and
- *     uploaded), compresses its slab, and the slabs are gathered into the root's device buffer (grouped ncclSend/ncclRecv)
- *     and copied to data_out on the root (data_out is ignored elsewhere). Bytes are identical to astcenc_compress_image().
+ *     collective, SLAB MODE: every rank passes the same image (host pointers) and compresses its slab of the COMBINED block
+ *     rows: layer * blocks_y + row for 3D block sizes, slice * blocks_y + row for a texture array (2D block size, dim_z > 1),
+ *     the rows of a 2D image. A rank reads and uploads only what its slab needs: the image rows of its block rows (with
+ *     a_scale_radius, the pre-pass window around them), or the slices of its layers. The slabs are gathered into the root's
+ *     device buffer (grouped ncclSend/ncclRecv) and copied to data_out on the root (data_out is ignored elsewhere); bytes are
+ *     identical to astcenc_compress_image(). astcenc_b200_last_timing() reports the bytes this rank uploaded.
  * astcenc_b200_compress_batch
  *     collective, BATCH MODE: image i of `images` belongs to rank i % world (other entries are not touched on this rank and
- *     may be NULL); all images share size and type. Each rank searches its images one after the other with the upload of
- *     the next image overlapped (two device image buffers); payload i arrives in data_out[i] on the root.
+ *     may be NULL); all images share dim_x, dim_y, dim_z and type (ASTCENC_ERR_BAD_PARAM otherwise) and data_len_each must
+ *     hold one image's payload. Each rank searches its images one after the other with the upload of the next image
+ *     overlapped (two device image buffers), a volume in one pass, a texture array slice by slice; payload i arrives in
+ *     data_out[i] on the root.
  * astcenc_b200_comm_last_timing device milliseconds of the last sharded call on this rank: search, and the gather alone
  */
 ASTCENC_PUBLIC enum astcenc_error astcenc_b200_comm_unique_id(void* id_out, size_t id_bytes);

@@ -111,6 +111,9 @@ def lib():
         l.astcenc_get_error_string.restype = C.c_char_p
         l.astcenc_b200_compress_device.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.POINTER(Swizzle), C.c_uint, C.c_uint, C.c_void_p, C.c_void_p]
         l.astcenc_b200_compress_device.restype = C.c_int
+        l.astcenc_b200_compress_device_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.POINTER(Swizzle), C.c_void_p,
+                                                          C.c_uint, C.c_void_p, C.c_void_p]
+        l.astcenc_b200_compress_device_blocks.restype = C.c_int
         l.astcenc_b200_launch_count.argtypes = [C.c_void_p]
         l.astcenc_b200_launch_count.restype = C.c_ulonglong
         l.astcenc_b200_last_timing.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
@@ -260,6 +263,20 @@ class Context:
                                                  C.c_void_p(d_out_ptr), C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compress_device")
+
+    def compress_device_blocks(self, d_pixels_ptr, data_type, dim_x, dim_y, dim_z, indices, d_payload_ptr, swizzle=(0, 1, 2, 3), stream=0):
+        """Block-list path (astcenc_b200_compress_device_blocks): recompress the listed blocks of a device-resident image into its
+        device-resident payload, in place. indices: any integer array-like of block positions in payload order (z, y, x);
+        enqueued on `stream`, no sync."""
+        idx = np.asarray(indices).reshape(-1)
+        if idx.size and (idx.min() < 0 or idx.max() > 0xFFFFFFFF):
+            raise AstcencError(ERR_BAD_PARAM, "astcenc_b200_compress_device_blocks")      # (no position the C interface could take)
+        idx = np.ascontiguousarray(idx, dtype=np.uint32)
+        sw = Swizzle(*swizzle)
+        err = lib().astcenc_b200_compress_device_blocks(self.handle, C.c_void_p(d_pixels_ptr), data_type, dim_x, dim_y, dim_z, C.byref(sw),
+                                                        idx.ctypes.data if idx.size else None, idx.size, C.c_void_p(d_payload_ptr), C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compress_device_blocks")
 
     def launch_count(self):
         return int(lib().astcenc_b200_launch_count(self.handle))

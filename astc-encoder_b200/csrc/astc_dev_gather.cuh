@@ -1,0 +1,70 @@
+// CUDA-native ASTC: block lists (astcenc_b200_compress_device_blocks). A block's 16 bytes depend on its texels after clamp-to-edge,
+// the alpha-scale test over its footprint and the context - not on where it sits (void extents carry no coordinates, partition
+// tables are indexed by seed). So the listed blocks are copied, footprint by footprint, into a staging image that is ONE ROW of
+// blocks, an ordinary pass of the wave pipeline compresses that row, and a scatter puts staging block i at the listed position.
+// The stage kernels never see the list.
+//
+// Staging layout of n listed blocks of a bx x by (x bz) footprint: (n * bx) x by texels (x bz slices for 3D block sizes), block i
+// at x = i * bx. Every staged texel lies inside the staging image, so load_block reads it without clamping; the gather has done
+// the clamping against the source image, exactly as load_block clamps in place (astcenc_image.cpp:162-342).
+#pragma once
+
+struct GatherArgs {
+	const void* src;            // the caller's image: dim_z slices of dim_x * dim_y texels, contiguous
+	void* dst;                  // the staging image
+	const float* avg_src;       // alpha-scale averages of source slice 0 at image positions (dim_x * dim_y), or null
+	float* avg_dst;             // the averages in the staging layout ((n * bx) x by), or null
+	const uint32_t* indices;    // the listed blocks (positions in z, y, x order: astcenc_entry.cpp:1036)
+	unsigned int n;             // listed blocks of this gather
+	unsigned int words;         // 32-bit words per texel: 1 (U8), 2 (F16), 4 (F32)
+	unsigned int dim_x, dim_y, dim_z;
+	unsigned int blocks_x, blocks_y;
+	unsigned int bx, by, bz;    // footprint; bz = 1 for 2D block sizes, whose block index then counts slice z of a texture array
+};
+
+// Texel t (x fastest, then y, then z) of listed block i: where it comes from in the source image (a texel index, clamped to the
+// image's edges) and where it goes in the staging image. inside: the unclamped texel lies in the image (block_has_alpha counts
+// only those).
+struct GatherTexel {
+	size_t src, dst;
+	bool inside;
+};
+
+ASTC_FN GatherTexel gather_texel(const GatherArgs& g, unsigned int i, uint32_t index, unsigned int t) {
+	unsigned int col = index % g.blocks_x;
+	unsigned int rest = index / g.blocks_x;
+	unsigned int row = rest % g.blocks_y;
+	unsigned int layer = rest / g.blocks_y;
+	unsigned int tx = t % g.bx;
+	unsigned int ty = (t / g.bx) % g.by;
+	unsigned int tz = t / (g.bx * g.by);
+	unsigned int x = col * g.bx + tx, y = row * g.by + ty, z = layer * g.bz + tz;
+	unsigned int xi = x < g.dim_x - 1 ? x : g.dim_x - 1;
+	unsigned int yi = y < g.dim_y - 1 ? y : g.dim_y - 1;
+	unsigned int zi = z < g.dim_z - 1 ? z : g.dim_z - 1;
+	GatherTexel r;
+	r.src = ((size_t)zi * g.dim_y + yi) * g.dim_x + xi;
+	r.dst = ((size_t)tz * g.by + ty) * ((size_t)g.n * g.bx) + (size_t)i * g.bx + tx;
+	r.inside = x < g.dim_x && y < g.dim_y;
+	return r;
+}
+
+// Listed block i, by the lanes of one warp (lane / lanes): the texels word by word, so that consecutive lanes read consecutive
+// words of a footprint row; then the alpha averages (0 for texels outside the image). The host simulation calls it with 0 / 1.
+ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lanes) {
+	const uint32_t index = ASTC_LDG(g.indices + i);
+	const unsigned int T = g.bx * g.by * g.bz;
+	const uint32_t* src = static_cast<const uint32_t*>(g.src);
+	uint32_t* dst = static_cast<uint32_t*>(g.dst);
+	for (unsigned int w = (unsigned int)lane; w < T * g.words; w += (unsigned int)lanes) {
+		unsigned int t = w / g.words, k = w - t * g.words;
+		GatherTexel p = gather_texel(g, i, index, t);
+		dst[p.dst * g.words + k] = ASTC_LDG(src + p.src * g.words + k);
+	}
+	if (g.avg_dst != nullptr) {
+		for (unsigned int t = (unsigned int)lane; t < T; t += (unsigned int)lanes) {
+			GatherTexel p = gather_texel(g, i, index, t);
+			g.avg_dst[p.dst] = p.inside ? ASTC_LDG(g.avg_src + p.src) : 0.0f;
+		}
+	}
+}

@@ -22,6 +22,7 @@
 
 #include "astc_dev_search.cuh"
 #include "astc_dev_metrics.cuh"
+#include "astc_dev_gather.cuh"
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
 
@@ -209,6 +210,35 @@ astc_alpha_average_kernel(const __grid_constant__ DevImage img, unsigned int rad
 	alpha_average_tile(img, radius, tx * ALPHA_TILE, ty * ALPHA_TILE, 0, averages, (int)threadIdx.x, (int)blockDim.x);
 }
 
+// ---- block lists (astc_dev_gather.cuh): one warp per listed block, grid-stride ----
+#define ASTC_GATHER_THREADS 256
+__global__ void __launch_bounds__(ASTC_GATHER_THREADS)
+astc_gather_blocks_kernel(const __grid_constant__ GatherArgs g) {
+	const unsigned int warps = blockDim.x >> 5;
+	for (unsigned int i = blockIdx.x * warps + (threadIdx.x >> 5); i < g.n; i += gridDim.x * warps) {
+		gather_block(g, i, (int)(threadIdx.x & 31), 32);
+	}
+}
+
+// staging block i -> payload block indices[i] (duplicates write the same bytes); one thread per block
+__global__ void __launch_bounds__(ASTC_GATHER_THREADS)
+astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const uint32_t* __restrict__ indices, unsigned int n, uint8_t* payload, int aligned16) {
+	unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) {
+		return;
+	}
+	uint8_t* dst = payload + (size_t)__ldg(indices + i) * 16;
+	uint4 v = __ldg(reinterpret_cast<const uint4*>(staged) + i);
+	if (aligned16) {
+		*reinterpret_cast<uint4*>(dst) = v;
+	} else {
+		const uint8_t* b = reinterpret_cast<const uint8_t*>(&v);
+		for (int k = 0; k < 16; k++) {
+			dst[k] = b[k];
+		}
+	}
+}
+
 // ---- decompression (SURVEY.md section 8f): one warp per block, grid-stride ----
 #define ASTC_DECODE_THREADS 256
 __global__ void __launch_bounds__(ASTC_DECODE_THREADS, 2)
@@ -366,6 +396,7 @@ struct astcenc_context {
 	unsigned int volume_dim_z;      // slices of the volume the current pass reads (3D block sizes; 1 otherwise), set under launch_mtx
 	uint32_t* pass_cancel;          // the progress words the current pass's kernels see (null for the device-resident paths), set under launch_mtx
 	uint32_t* pass_done;
+	bool pass_alpha_staged;         // the pass reads averages gathered into d_alpha beforehand and runs no pre-pass (block lists), set under launch_mtx
 	// wave pipeline buffers, grown on demand
 	uint8_t* d_records;
 	size_t d_records_bytes;
@@ -384,6 +415,16 @@ struct astcenc_context {
 	size_t d_image_bytes;
 	uint8_t* d_out;
 	size_t d_out_bytes;
+	// block lists (astcenc_b200_compress_device_blocks), grown on demand: the list, the staging image and payload of one chunk,
+	// the pre-pass averages of the source image
+	uint8_t* d_list;
+	size_t d_list_bytes;
+	uint8_t* d_list_image;
+	size_t d_list_image_bytes;
+	uint8_t* d_list_out;
+	size_t d_list_out_bytes;
+	uint8_t* d_list_alpha;
+	size_t d_list_alpha_bytes;
 	Knobs knobs;
 	// The per-context scratch (records, queues, counters, alpha averages) serves ONE pipeline pass at a time: launch_mtx
 	// serialises the host side, scratch_done orders a pass on one stream behind the previous pass on another.
@@ -522,6 +563,8 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	ctx->d_image2 = nullptr;
 	ctx->d_out = nullptr;
 	ctx->d_image_bytes = ctx->d_image2_bytes = ctx->d_out_bytes = 0;
+	ctx->d_list = ctx->d_list_image = ctx->d_list_out = ctx->d_list_alpha = nullptr;
+	ctx->d_list_bytes = ctx->d_list_image_bytes = ctx->d_list_out_bytes = ctx->d_list_alpha_bytes = 0;
 	ctx->nccl_comm = nullptr;
 	ctx->rank = 0;
 	ctx->world = 1;
@@ -538,6 +581,7 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	ctx->ctl_ready = nullptr;
 	ctx->flag_raised = false;
 	ctx->pass_cancel = ctx->pass_done = nullptr;
+	ctx->pass_alpha_staged = false;
 	ctx->launches = 0;
 	ctx->last_kernel_ms = 0.0f;
 	ctx->last_h2d = ctx->last_d2h = 0;
@@ -775,6 +819,10 @@ void astcenc_context_free(astcenc_context* ctx) {
 	cudaFree(ctx->d_image);
 	cudaFree(ctx->d_image2);
 	cudaFree(ctx->d_out);
+	cudaFree(ctx->d_list);
+	cudaFree(ctx->d_list_image);
+	cudaFree(ctx->d_list_out);
+	cudaFree(ctx->d_list_alpha);
 	if (ctx->ev0) cudaEventDestroy(ctx->ev0);
 	if (ctx->ev1) cudaEventDestroy(ctx->ev1);
 	if (ctx->ev_g0) cudaEventDestroy(ctx->ev_g0);
@@ -1025,6 +1073,43 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d
 	return ASTCENC_SUCCESS;
 }
 
+// The alpha-scale pre-pass over image rows [y0, y1) of a 2D image (alpha_window: the 32 x 32 tiles that cover them, reading up to
+// a_scale_radius rows beyond); the averages land at their image positions in `averages` (dim_x * dim_y floats). Sets the
+// threshold the set-up stage compares them with.
+static astcenc_error alpha_prepass(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
+                                   unsigned int y0, unsigned int y1, float* averages, cudaStream_t stream) {
+	const DevBsd& bsd = ctx->tables->bsd;
+	const unsigned int radius = ctx->config.a_scale_radius;
+	size_t pad = (size_t)ALPHA_TILE + 2 * (size_t)radius + 1;
+	size_t smem = pad * pad * sizeof(float);
+	if (smem > 200 * 1024) {
+		return ASTCENC_ERR_NOT_IMPLEMENTED;      // radius > ~94: the padded tile no longer fits shared memory
+	}
+	if (smem > 48 * 1024) {
+		CUDA_TRY(cudaFuncSetAttribute(astc_alpha_average_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), return ASTCENC_ERR_BAD_CONTEXT);
+	}
+	DevImage aimg{};
+	aimg.data = d_pixels;
+	aimg.data_type = data_type;
+	aimg.dim_x = dim_x;
+	aimg.dim_y = dim_y;
+	for (int i = 0; i < 4; i++) {
+		aimg.swz[i] = swz[i];
+	}
+	aimg.cancel = ctx->pass_cancel;
+	unsigned int tiles_x = (dim_x + ALPHA_TILE - 1) / ALPHA_TILE;
+	AlphaWindow win = alpha_window(dim_y, radius, y0, y1);
+	astc_alpha_average_kernel<<<tiles_x * win.tile_rows, ASTC_ALPHA_THREADS, smem, stream>>>(aimg, radius, tiles_x, win.tile_row0, averages);
+	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+	ctx->launches++;
+	// astcenc_entry.cpp:983-988
+	size_t x_footprint = bsd.dim_x + 2 * ((size_t)radius - 1);
+	size_t y_footprint = bsd.dim_y + 2 * ((size_t)radius - 1);
+	float footprint = static_cast<float>(x_footprint * y_footprint);
+	ctx->alpha_threshold = 0.9f / (255.0f * footprint);
+	return ASTCENC_SUCCESS;
+}
+
 static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
                                         unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up) {
 	const DevBsd& bsd = ctx->tables->bsd;
@@ -1052,7 +1137,7 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 		}
 		up = nullptr;
 	}
-	if (radius != 0) {
+	if (radius != 0 && !ctx->pass_alpha_staged) {
 		// alpha-scale pre-pass over the tiles that cover the slab's rows: the box filter reaches across slab borders, so
 		// the window reads up to `radius` rows beyond the tiles (alpha_window); the averages stay at their image positions
 		size_t need = (size_t)dim_x * dim_y * sizeof(float);
@@ -1063,34 +1148,11 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 			CUDA_TRY(cudaMalloc(&ctx->d_alpha, need), return ASTCENC_ERR_OUT_OF_MEM);
 			ctx->d_alpha_bytes = need;
 		}
-		size_t pad = (size_t)ALPHA_TILE + 2 * (size_t)radius + 1;
-		size_t smem = pad * pad * sizeof(float);
-		if (smem > 200 * 1024) {
-			return ASTCENC_ERR_NOT_IMPLEMENTED;      // radius > ~94: the padded tile no longer fits shared memory
-		}
-		if (smem > 48 * 1024) {
-			CUDA_TRY(cudaFuncSetAttribute(astc_alpha_average_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), return ASTCENC_ERR_BAD_CONTEXT);
-		}
-		DevImage aimg{};
-		aimg.data = d_pixels;
-		aimg.data_type = data_type;
-		aimg.dim_x = dim_x;
-		aimg.dim_y = dim_y;
-		for (int i = 0; i < 4; i++) {
-			aimg.swz[i] = swz[i];
-		}
-		aimg.cancel = ctx->pass_cancel;
-		unsigned int tiles_x = (dim_x + ALPHA_TILE - 1) / ALPHA_TILE;
 		size_t y1 = (size_t)(block_row0 + block_rows) * bsd.dim_y;
-		AlphaWindow win = alpha_window(dim_y, radius, block_row0 * bsd.dim_y, y1 < dim_y ? (unsigned int)y1 : dim_y);
-		astc_alpha_average_kernel<<<tiles_x * win.tile_rows, ASTC_ALPHA_THREADS, smem, stream>>>(aimg, radius, tiles_x, win.tile_row0, ctx->d_alpha);
-		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
-		ctx->launches++;
-		// astcenc_entry.cpp:983-988
-		size_t x_footprint = bsd.dim_x + 2 * ((size_t)radius - 1);
-		size_t y_footprint = bsd.dim_y + 2 * ((size_t)radius - 1);
-		float footprint = static_cast<float>(x_footprint * y_footprint);
-		ctx->alpha_threshold = 0.9f / (255.0f * footprint);
+		astcenc_error st = alpha_prepass(ctx, d_pixels, data_type, dim_x, dim_y, swz, block_row0 * bsd.dim_y, y1 < dim_y ? (unsigned int)y1 : dim_y, ctx->d_alpha, stream);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
 	}
 	if (use_pipes) {
 		return launch_pipes(ctx, pipes, d_pixels, data_type, dim_x, dim_y, swz, block_row0, block_rows, d_out, stream, banded ? up : nullptr);
@@ -1929,6 +1991,137 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 	int swz[4] = {(int)swizzle->r, (int)swizzle->g, (int)swizzle->b, (int)swizzle->a};
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return launch_slab(ctx, d_pixels, (int)data_type, dim_x, dim_y, swz, block_row0, block_rows, d_out, s);
+}
+
+// Block lists (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk (a staging row is
+// one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks blocks). The
+// whole call is one turn of the context's scratch (launch_mtx, scratch_done), like a launch_slab.
+static astcenc_error launch_blocks(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, unsigned int dim_z,
+                                   const int swz[4], const std::vector<uint32_t>& list, unsigned int row_lo, unsigned int row_hi, uint8_t* d_payload, cudaStream_t stream) {
+	const DevBsd& bsd = ctx->tables->bsd;
+	const bool volume = bsd.dim_z > 1;
+	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
+	const size_t n = list.size();
+	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
+	const unsigned int words = data_type == ASTCENC_TYPE_U8 ? 1 : data_type == ASTCENC_TYPE_F16 ? 2 : 4;
+	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
+	ctx->volume_dim_z = volume ? bsd.dim_z : 1;      // (the staging volume is one layer deep)
+	ctx->pass_cancel = ctx->pass_done = nullptr;
+	if (ctx->scratch_used) {
+		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
+	}
+	astcenc_error st = ensure_buffer(ctx->d_list, ctx->d_list_bytes, n * sizeof(uint32_t));
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_list_image, ctx->d_list_image_bytes, chunk * bsd.texel_count * words * 4);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_list_out, ctx->d_list_out_bytes, chunk * 16);
+	if (st == ASTCENC_SUCCESS && radius != 0) {
+		st = ensure_buffer(ctx->d_list_alpha, ctx->d_list_alpha_bytes, (size_t)dim_x * dim_y * sizeof(float));
+		if (st == ASTCENC_SUCCESS && chunk * bsd.texel_count * sizeof(float) > ctx->d_alpha_bytes) {
+			cudaFree(ctx->d_alpha);
+			ctx->d_alpha = nullptr;
+			ctx->d_alpha_bytes = 0;
+			CUDA_TRY(cudaMalloc(&ctx->d_alpha, chunk * bsd.texel_count * sizeof(float)), st = ASTCENC_ERR_OUT_OF_MEM);
+			if (st == ASTCENC_SUCCESS) ctx->d_alpha_bytes = chunk * bsd.texel_count * sizeof(float);
+		}
+	}
+	if (st == ASTCENC_SUCCESS) {
+		// (from pageable memory: staged by the driver before the call returns, so `list` may go when this function does)
+		CUDA_TRY(cudaMemcpyAsync(ctx->d_list, list.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+	}
+	if (st == ASTCENC_SUCCESS && radius != 0) {
+		// the averages of the listed blocks' rows, at their image positions; the staging pass must not filter its own image,
+		// whose box filter would reach across the seams between unrelated blocks
+		unsigned int y1 = (row_hi + 1) * bsd.dim_y;
+		st = alpha_prepass(ctx, d_pixels, data_type, dim_x, dim_y, swz, row_lo * bsd.dim_y, y1 < dim_y ? y1 : dim_y,
+		                   reinterpret_cast<float*>(ctx->d_list_alpha), stream);
+	}
+	GatherArgs g;
+	g.src = d_pixels;
+	g.dst = ctx->d_list_image;
+	g.avg_src = radius != 0 ? reinterpret_cast<const float*>(ctx->d_list_alpha) : nullptr;
+	g.avg_dst = radius != 0 ? ctx->d_alpha : nullptr;
+	g.words = words;
+	g.dim_x = dim_x;
+	g.dim_y = dim_y;
+	g.dim_z = dim_z;
+	g.blocks_x = (unsigned int)block_count_axis(dim_x, bsd.dim_x);
+	g.blocks_y = (unsigned int)block_count_axis(dim_y, bsd.dim_y);
+	g.bx = bsd.dim_x;
+	g.by = bsd.dim_y;
+	g.bz = bsd.dim_z;
+	const int aligned16 = (reinterpret_cast<uintptr_t>(d_payload) & 15) == 0;
+	for (size_t first = 0; first < n && st == ASTCENC_SUCCESS; first += chunk) {
+		const unsigned int m = (unsigned int)(n - first < chunk ? n - first : chunk);
+		const uint32_t* d_idx = reinterpret_cast<const uint32_t*>(ctx->d_list) + first;
+		g.indices = d_idx;
+		g.n = m;
+		const unsigned int warps = ASTC_GATHER_THREADS / 32;
+		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
+		ctx->launches++;
+		ctx->pass_alpha_staged = radius != 0;
+		st = launch_slab_locked(ctx, ctx->d_list_image, data_type, m * bsd.dim_x, bsd.dim_y, swz, 0, 1, ctx->d_list_out, stream, nullptr);
+		ctx->pass_alpha_staged = false;
+		if (st == ASTCENC_SUCCESS) {
+			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->d_list_out, d_idx, m, d_payload, aligned16);
+			ctx->launches++;
+			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
+		}
+	}
+	CUDA_TRY(cudaEventRecord(ctx->scratch_done, stream), return ASTCENC_ERR_BAD_CONTEXT);
+	ctx->scratch_used = true;
+	return st;
+}
+
+astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const void* d_pixels, astcenc_type data_type, unsigned int dim_x, unsigned int dim_y,
+                                                  unsigned int dim_z, const astcenc_swizzle* swizzle, const uint32_t* block_indices, unsigned int block_count,
+                                                  uint8_t* d_payload, void* cuda_stream) {
+	if (ctx->config.flags & ASTCENC_FLG_DECOMPRESS_ONLY) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	if (!swizzle) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	astcenc_error status = validate_compression_swizzle(*swizzle);
+	if (status != ASTCENC_SUCCESS) {
+		return status;
+	}
+	if (dim_x == 0 || dim_y == 0 || dim_z == 0 || !d_pixels || !d_payload || (block_count != 0 && !block_indices)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if ((int)data_type < 0 || (int)data_type > 2) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (ctx->config.a_scale_radius != 0 && dim_z != 1 && ctx->config.block_z <= 1) {
+		return ASTCENC_ERR_NOT_IMPLEMENTED;      // as astcenc_compress_image: the pre-pass is built for 2D images
+	}
+	size_t blocks_x = block_count_axis(dim_x, ctx->config.block_x);
+	size_t blocks_y = block_count_axis(dim_y, ctx->config.block_y);
+	size_t blocks_z = block_count_axis(dim_z, ctx->config.block_z);
+	bool overflow = false;
+	size_t total = mul_safe(mul_safe(blocks_x, blocks_y, overflow), blocks_z, overflow);
+	if (overflow) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	// the list is checked whole before anything is enqueued, and copied: the caller may free it when the call returns
+	std::vector<uint32_t> list(block_indices, block_indices + block_count);
+	unsigned int row_lo = 0xFFFFFFFFu, row_hi = 0;
+	for (uint32_t b : list) {
+		if (b >= total) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		unsigned int row = (unsigned int)(b / blocks_x);      // (2D images: the block row, for the alpha-scale pre-pass window)
+		row_lo = row < row_lo ? row : row_lo;
+		row_hi = row > row_hi ? row : row_hi;
+	}
+	if (block_count == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	int swz[4] = {(int)swizzle->r, (int)swizzle->g, (int)swizzle->b, (int)swizzle->a};
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return launch_blocks(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, swz, list, row_lo, row_hi, d_payload, s);
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

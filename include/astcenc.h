@@ -198,7 +198,7 @@ ASTCENC_PUBLIC const char* astcenc_get_error_string(enum astcenc_error status);
  *    (z, y, x) order like the reference's (astcenc_entry.cpp:1036); a_scale_radius is ignored like the reference does
  *    (astcenc_entry.cpp:975). The multi-GPU entry points (slab and batch mode) take the same images: 2D, texture arrays and
  *    volumes. The device-resident entry astcenc_b200_compress_device and astcenc_b200_slab_rows stay 2D (3D block sizes:
- *    ASTCENC_ERR_NOT_IMPLEMENTED).
+ *    ASTCENC_ERR_NOT_IMPLEMENTED); the device-resident block-list entry astcenc_b200_compress_device_blocks takes volumes.
  *  - a_scale_radius with a 2D block size and dim_z > 1 gives ASTCENC_ERR_NOT_IMPLEMENTED from every compressing entry point.
  *    The alpha-scale pre-pass of a pass over some block rows filters only the 32 x 32 tiles that cover those rows, and reads
  *    the image rows of those tiles plus a_scale_radius rows on either side; nothing else of the image is read.
@@ -214,6 +214,27 @@ ASTCENC_PUBLIC const char* astcenc_get_error_string(enum astcenc_error status);
 ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device(struct astcenc_context* context, const void* d_pixels, enum astcenc_type data_type,
                                                                unsigned int dim_x, unsigned int dim_y, const struct astcenc_swizzle* swizzle,
                                                                unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, void* cuda_stream);
+
+/* Recompress a list of blocks of an image that is ALREADY RESIDENT in device memory, in place in its device-resident payload:
+ * for a texture whose source changes a few tiles at a time (painting tools, procedural or virtual-texture pages, atlases).
+ *  - d_pixels: the whole image, dim_z slices of dim_x * dim_y texels, contiguous. Image shapes are those astcenc_compress_image
+ *    takes: 2D images, texture arrays (2D block size, dim_z > 1) and volumes of 3D block sizes.
+ *  - d_payload: the whole image's payload in astcenc_compress_image's order (blocks in z, y, x order; for 2D block sizes z
+ *    counts slices). block_indices (a HOST array, which the caller may free as soon as the call returns) are positions in that
+ *    order. Exactly the 16 bytes of each listed block are written - the bytes astcenc_compress_image produces for that block -
+ *    and every other byte of d_payload is left untouched. Duplicate indices write the same bytes; block_count == 0 does nothing.
+ *  - Errors, in this order: ASTCENC_ERR_BAD_CONTEXT for a decompress-only context, ASTCENC_ERR_BAD_SWIZZLE, ASTCENC_ERR_BAD_PARAM
+ *    for NULL or zero-sized arguments, ASTCENC_ERR_NOT_IMPLEMENTED for a_scale_radius on a texture array (with a 3D block size
+ *    the radius is ignored), ASTCENC_ERR_BAD_PARAM for an index at or beyond the image's block count. On error nothing is
+ *    launched and nothing is written.
+ *  - Enqueued on `cuda_stream` (0 = the context's own stream), without synchronising, in order with every other pass of the
+ *    context (see above). No progress callback, no cancellation.
+ * The listed blocks are gathered into a staging row of blocks, compressed by one ordinary pass of the wave pipeline (one per
+ * ASTCENC_B200_BATCH_BLOCKS blocks of a longer list) and scattered to their positions; the block count of the list, not the
+ * image's, sets the cost. */
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device_blocks(struct astcenc_context* context, const void* d_pixels, enum astcenc_type data_type,
+                                                                      unsigned int dim_x, unsigned int dim_y, unsigned int dim_z, const struct astcenc_swizzle* swizzle,
+                                                                      const uint32_t* block_indices, unsigned int block_count, uint8_t* d_payload, void* cuda_stream);
 
 /**
  * Multi-GPU sharding: one process per GPU, each with its own context; the only exchange is the gather of the compressed

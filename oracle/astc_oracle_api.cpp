@@ -72,6 +72,17 @@ void oracle_get_config(void* ctx, Config* out) {
 	*out = static_cast<Context*>(ctx)->config;
 }
 
+// pack_color_endpoints on n vectors. colors: 16 floats per vector (color0, color1, rgbs_color, rgbo_color);
+// fmt_quant: (format, quant_level) per vector; out: 8 bytes per vector, bytes the format does not define are left as
+// they are; out_format: the format used. The caller checks the inputs (finite values, quant level 4..20, a known format).
+void oracle_pack_color_endpoints(unsigned int n, const float* colors, const int* fmt_quant, uint8_t* out, uint8_t* out_format) {
+	for (unsigned int i = 0; i < n; i++) {
+		const float* c = colors + 16 * (size_t)i;
+		out_format[i] = pack_color_endpoints(mk4(c[0], c[1], c[2], c[3]), mk4(c[4], c[5], c[6], c[7]), mk4(c[8], c[9], c[10], c[11]),
+		                                     mk4(c[12], c[13], c[14], c[15]), fmt_quant[2 * i], out + 8 * (size_t)i, fmt_quant[2 * i + 1]);
+	}
+}
+
 }
 
 #include "astc_error_metrics.inl"

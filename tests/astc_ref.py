@@ -310,6 +310,24 @@ def have_ref_metrics():
     return os.path.exists(REF_METRICS_SO)
 
 
+# ---- endpoint packing (the reference's pack_color_endpoints, oracle/ref_pack_shim.cpp) --------------------------------
+REF_PACK_SO = os.path.join(ROOT, "oracle", "_ref", "libastcenc_ref_pack.so")
+
+
+def have_ref_pack():
+    return os.path.exists(REF_PACK_SO)
+
+
+def ref_pack_color_endpoints():
+    """ref_pack_color_endpoints(n, colors, fmt_quant, out, out_format): the UNMODIFIED reference pack_color_endpoints on n
+    vectors (colors: 16 float32 each, fmt_quant: 2 int32 each, out: 8 bytes each, out_format: 1 byte each)."""
+    lib = C.CDLL(REF_PACK_SO, mode=os.RTLD_LOCAL)
+    fn = lib.ref_pack_color_endpoints
+    fn.argtypes = [C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    fn.restype = None
+    return fn
+
+
 def ref_error_metrics(img1, img2, hdr=False, normal=False, components=4, fstop_lo=-10, fstop_hi=10):
     """Runs the UNMODIFIED reference compute_error_metrics() and parses what it prints (4 decimals)."""
     import re, sys, tempfile

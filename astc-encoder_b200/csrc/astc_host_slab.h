@@ -6,10 +6,32 @@
 // astcenc_entry.cpp:1036). A 2D image is the case of one slice.
 #pragma once
 
-// combined block rows [first, last) of rank g when `rows` of them are cut into `world` slabs (the same rule on every rank)
+// combined block rows [first, last) of rank g when `rows` of them are cut into `world` slabs (the same rule on every rank); the
+// sub-slab pipelines of one pass cut its rows the same way
 static inline void slab_of(unsigned int rows, int world, int g, unsigned int& first, unsigned int& last) {
 	first = (unsigned int)((size_t)rows * (size_t)g / (size_t)world);
 	last = (unsigned int)((size_t)rows * (size_t)(g + 1) / (size_t)world);
+}
+
+// Image rows [y0, y1) of block rows [r0, r1) of a 2D image of dim_y rows cut into block rows of block_y.
+static inline void image_rows(unsigned int r0, unsigned int r1, unsigned int block_y, unsigned int dim_y, size_t& y0, size_t& y1) {
+	y0 = (size_t)r0 * block_y;
+	y1 = (size_t)r1 * block_y;
+	if (y1 > dim_y) y1 = dim_y;
+}
+
+// Band k of `bands` upload bands over `rows` block rows: [first, last), growing 1 : 3 : 4 : 8 : 8 ... so that the first copy -
+// the only one nothing hides - is short; the last band takes the rest. False for an empty band, which is not launched.
+static inline bool band_of(unsigned int rows, int bands, int k, unsigned int& first, unsigned int& last) {
+	static const unsigned int shares[8] = {1, 3, 4, 8, 8, 8, 8, 8};
+	unsigned int sum = 0, acc = 0;
+	for (int i = 0; i < bands; i++) {
+		sum += shares[i];
+		acc += i < k ? shares[i] : 0;
+	}
+	first = (unsigned int)((size_t)rows * acc / sum);
+	last = k == bands - 1 ? rows : (unsigned int)((size_t)rows * (acc + shares[k]) / sum);
+	return last > first;
 }
 
 // The image slices [z0, z1) that combined rows [r0, r1) (r0 < r1) read: the slices of the layers they touch, block_z of them per

@@ -25,6 +25,7 @@
 #include "astc_dev_gather.cuh"
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
+#include "astc_host_slab.h"
 
 // ---------------------------------------------------------------------------------------------
 // The kernel: persistent warps, one block per warp at a time, dynamic ticket scheduling (the GPU analogue
@@ -389,23 +390,18 @@ struct astcenc_context {
 	int warps_setup, warps_small;   // warps per CTA of the setup / refine+prepare kernels
 	int refine_ctas;                // CTAs per SM of the refine kernel (experiment: ASTCENC_B200_REFINE_CTAS)
 	int warps_setup_1p;             // set-up kernel on the compact one-plane plan (0 = plan not used)
-	size_t smem_setup, smem_setup_1p, smem_small, smem_refine;
+	size_t smem_setup, smem_setup_1p, smem_refine;
 	uint32_t setup_stage_bytes;
 	uint32_t refine_stage_bytes;   // tables staged behind the header of the refine kernel's shared window (0 = none)
 	int max_waves;
-	unsigned int volume_dim_z;      // slices of the volume the current pass reads (3D block sizes; 1 otherwise), set under launch_mtx
-	uint32_t* pass_cancel;          // the progress words the current pass's kernels see (null for the device-resident paths), set under launch_mtx
-	uint32_t* pass_done;
-	bool pass_alpha_staged;         // the pass reads averages gathered into d_alpha beforehand and runs no pre-pass (block lists), set under launch_mtx
 	// wave pipeline buffers, grown on demand
 	uint8_t* d_records;
 	size_t d_records_bytes;
-	uint32_t* d_queues;          // ASTC_Q_KINDS x capacity
-	size_t queue_capacity;
+	uint32_t* d_queues;          // ASTC_Q_KINDS lists of one entry per block
+	size_t d_queues_bytes;
 	uint32_t* d_counters;        // count[ASTC_Q_KINDS][MAX_WAVES] head[ASTC_Q_KINDS][MAX_WAVES]
 	float* d_alpha;              // alpha-scale pre-pass: one average per texel
 	size_t d_alpha_bytes;
-	float alpha_threshold;
 	// optional per-stage timing (astcenc_b200_stage_timing): an event after every launch of the next call
 	int stage_timing;
 	std::vector<cudaEvent_t> stage_events;
@@ -434,7 +430,6 @@ struct astcenc_context {
 	// host-pointer path: uploads run on copy_stream, band by band, under the set-up of the previous band
 	cudaStream_t copy_stream;
 	cudaEvent_t band_ready[ASTC_MAX_BANDS];
-	cudaEvent_t out_ready;
 	// sub-slab pipelines of one pass (launch_pipes): one stream each, joined to the caller's stream by events
 	cudaStream_t pipe_stream[ASTC_MAX_PIPES];
 	cudaEvent_t pipe_done[ASTC_MAX_PIPES];
@@ -501,6 +496,19 @@ static void release_tables(DeviceTables* t) {
 	}
 }
 
+// device buffers grown on demand (never shrunk): `have` bytes at `buf`
+template <typename T>
+static astcenc_error ensure_buffer(T*& buf, size_t& have, size_t need) {
+	if (have < need) {
+		cudaFree(buf);
+		buf = nullptr;
+		have = 0;
+		CUDA_TRY(cudaMalloc(&buf, need), return ASTCENC_ERR_OUT_OF_MEM);
+		have = need;
+	}
+	return ASTCENC_SUCCESS;
+}
+
 extern "C" {
 
 astcenc_error astcenc_config_init(astcenc_profile profile, unsigned int block_x, unsigned int block_y, unsigned int block_z, float quality,
@@ -540,7 +548,6 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	ctx->ev0 = ctx->ev1 = nullptr;
 	ctx->scratch_done = nullptr;
 	ctx->scratch_used = false;
-	ctx->out_ready = nullptr;
 	for (int i = 0; i < ASTC_MAX_BANDS; i++) {
 		ctx->band_ready[i] = nullptr;
 	}
@@ -553,11 +560,10 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	ctx->d_records = nullptr;
 	ctx->d_records_bytes = 0;
 	ctx->d_queues = nullptr;
-	ctx->queue_capacity = 0;
+	ctx->d_queues_bytes = 0;
 	ctx->d_counters = nullptr;
 	ctx->d_alpha = nullptr;
 	ctx->d_alpha_bytes = 0;
-	ctx->alpha_threshold = 0.0f;
 	ctx->stage_timing = 0;
 	ctx->d_image = nullptr;
 	ctx->d_image2 = nullptr;
@@ -580,15 +586,12 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	ctx->ctl_stream = nullptr;
 	ctx->ctl_ready = nullptr;
 	ctx->flag_raised = false;
-	ctx->pass_cancel = ctx->pass_done = nullptr;
-	ctx->pass_alpha_staged = false;
 	ctx->launches = 0;
 	ctx->last_kernel_ms = 0.0f;
 	ctx->last_h2d = ctx->last_d2h = 0;
 	ctx->warps_per_cta = ctx->grid = 0;
 	ctx->warps_setup_1p = 0;
 	ctx->max_waves = 0;
-	ctx->volume_dim_z = 1;
 	// environment knobs: read here, once
 	ctx->knobs.batch_blocks = (size_t)1 << 20;
 	if (const char* e = getenv("ASTCENC_B200_BATCH_BLOCKS")) {
@@ -743,7 +746,6 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 				ctx->warps_setup_1p = w1 > ws ? w1 : 0;      // only when it buys warps
 				ctx->smem_setup_1p = ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + ctx->setup_stage_bytes + arena1 * (size_t)w1;
 			}
-			ctx->smem_small = ASTC_SMEM_HDR + arena_small * wr;
 			ctx->smem_refine = ASTC_SMEM_HDR + ctx->refine_stage_bytes + arena_small * wr + (size_t)ASTC_REFINE_STATE_BYTES * wr;
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
@@ -779,7 +781,6 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	CUDA_TRY(cudaEventCreate(&ctx->ev_g0), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 	CUDA_TRY(cudaEventCreate(&ctx->ev_g1), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 	CUDA_TRY(cudaEventCreateWithFlags(&ctx->scratch_done, cudaEventDisableTiming), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-	CUDA_TRY(cudaEventCreateWithFlags(&ctx->out_ready, cudaEventDisableTiming), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 	for (int i = 0; i < ASTC_MAX_BANDS; i++) {
 		CUDA_TRY(cudaEventCreateWithFlags(&ctx->band_ready[i], cudaEventDisableTiming), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 	}
@@ -828,7 +829,6 @@ void astcenc_context_free(astcenc_context* ctx) {
 	if (ctx->ev_g0) cudaEventDestroy(ctx->ev_g0);
 	if (ctx->ev_g1) cudaEventDestroy(ctx->ev_g1);
 	if (ctx->scratch_done) cudaEventDestroy(ctx->scratch_done);
-	if (ctx->out_ready) cudaEventDestroy(ctx->out_ready);
 	for (int i = 0; i < ASTC_MAX_BANDS; i++) {
 		if (ctx->band_ready[i]) cudaEventDestroy(ctx->band_ready[i]);
 	}
@@ -877,6 +877,37 @@ static size_t block_count_axis(size_t dim, size_t blk) {
 	return n;
 }
 
+// The scratch of a pass, grown on demand: records and queues for `blocks` blocks of the wave pipeline, `alpha` averages of the
+// alpha-scale pre-pass.
+static astcenc_error ensure_scratch(astcenc_context* ctx, size_t blocks, size_t alpha) {
+	astcenc_error st = ensure_buffer(ctx->d_queues, ctx->d_queues_bytes, sizeof(uint32_t) * ASTC_Q_KINDS * blocks);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_records, ctx->d_records_bytes, blocks * (size_t)ctx->tables->bsd.record_bytes);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_alpha, ctx->d_alpha_bytes, alpha * sizeof(float));
+	return st;
+}
+
+// The image a pass reads: dim_x x dim_y texels at `pixels`, `dim_z` slices of them for a volume pass (3D block sizes; 1
+// otherwise), no alpha averages and no progress words. The pass fills in the block rows it covers and where their payload goes.
+static DevImage pass_image(const astcenc_context* ctx, const void* pixels, int data_type, unsigned int dim_x, unsigned int dim_y, unsigned int dim_z,
+                           const astcenc_swizzle& swizzle) {
+	const DevBsd& bsd = ctx->tables->bsd;
+	DevImage img{};
+	img.data = pixels;
+	img.data_type = data_type;
+	img.dim_x = dim_x;
+	img.dim_y = dim_y;
+	img.dim_z = dim_z;
+	img.blocks_x = (dim_x + bsd.dim_x - 1) / bsd.dim_x;
+	img.blocks_y = (dim_y + bsd.dim_y - 1) / bsd.dim_y;
+	img.swz[0] = (int)swizzle.r;
+	img.swz[1] = (int)swizzle.g;
+	img.swz[2] = (int)swizzle.b;
+	img.swz[3] = (int)swizzle.a;
+	img.cancel = nullptr;
+	img.done = nullptr;
+	return img;
+}
+
 // Upload plan of the host-pointer path: the image (one 2D slice) is copied to the device in bands of block rows on the
 // context's copy stream; wave 0 of the pipeline - the only reader of the image - is launched band by band, each launch
 // waiting for its band only, so the copy of band k+1 runs under the set-up of band k.
@@ -887,41 +918,29 @@ struct UploadPlan {
 	int bands;                   // 1 .. ASTC_MAX_BANDS
 };
 
-static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                  unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up);
-
-// A slab of block rows is processed in batches of at most ~1 M blocks: the per-block search records (a few KB each)
-// are the only buffer that grows with the image, and the batches reuse them in stream order.
-// The context's scratch buffers serve one pass at a time. Calls may come from several host threads and on different
-// streams: launch_mtx serialises the enqueueing, and every pass starts by making its stream wait for the event that
-// closes the previous pass (a no-op when both ran on the same stream).
-static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                        unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up);
-
-// d_cancel / d_done: the progress words of an astcenc_compress_image pass (null: no progress, no cancellation).
-static astcenc_error launch_slab(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                 unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up = nullptr,
-                                 unsigned int volume_dim_z = 1, uint32_t* d_cancel = nullptr, uint32_t* d_done = nullptr) {
-	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
-	ctx->volume_dim_z = volume_dim_z;
-	ctx->pass_cancel = d_cancel;
-	ctx->pass_done = d_done;
-	if (ctx->scratch_used) {
-		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
+// Image rows [y0, y1) go up on the copy stream; band event k marks their arrival, and `stream` waits for it.
+static astcenc_error upload_rows(astcenc_context* ctx, const UploadPlan& up, size_t y0, size_t y1, int k, cudaStream_t stream) {
+	if (y1 > y0) {
+		CUDA_TRY(cudaMemcpyAsync(up.device + y0 * up.row_bytes, up.host + y0 * up.row_bytes, (y1 - y0) * up.row_bytes, cudaMemcpyHostToDevice, ctx->copy_stream),
+		         return ASTCENC_ERR_BAD_CONTEXT);
 	}
-	astcenc_error st = launch_slab_locked(ctx, d_pixels, data_type, dim_x, dim_y, swz, block_row0, block_rows, d_out, stream, up);
-	CUDA_TRY(cudaEventRecord(ctx->scratch_done, stream), return ASTCENC_ERR_BAD_CONTEXT);
-	ctx->scratch_used = true;
-	return st;
+	CUDA_TRY(cudaEventRecord(ctx->band_ready[k], ctx->copy_stream), return ASTCENC_ERR_BAD_CONTEXT);
+	CUDA_TRY(cudaStreamWaitEvent(stream, ctx->band_ready[k], 0), return ASTCENC_ERR_BAD_CONTEXT);
+	return ASTCENC_SUCCESS;
+}
+
+// Slices [z0, z1) of a host image to their places in a device buffer of slice_bytes per slice, one copy each on `stream`.
+static astcenc_error upload_slices(uint8_t* device, void* const* slices, unsigned int z0, unsigned int z1, size_t slice_bytes, cudaStream_t stream) {
+	for (unsigned int z = z0; z < z1; z++) {
+		CUDA_TRY(cudaMemcpyAsync(device + (size_t)z * slice_bytes, slices[z], slice_bytes, cudaMemcpyHostToDevice, stream), return ASTCENC_ERR_BAD_CONTEXT);
+	}
+	return ASTCENC_SUCCESS;
 }
 
 // Image rows [y0, y1) that a pass over block rows [block_row0, block_row0 + block_rows) of a 2D image reads: the slab's own
 // rows, or with alpha-scale the rows its pre-pass window reads (a superset of them).
 static void slab_image_rows(const astcenc_context* ctx, unsigned int dim_y, unsigned int block_row0, unsigned int block_rows, size_t& y0, size_t& y1) {
-	const unsigned int by = ctx->tables->bsd.dim_y;
-	y0 = (size_t)block_row0 * by;
-	y1 = (size_t)(block_row0 + block_rows) * by;
-	if (y1 > dim_y) y1 = dim_y;
+	image_rows(block_row0, block_row0 + block_rows, ctx->tables->bsd.dim_y, dim_y, y0, y1);
 	const unsigned int radius = ctx->tables->bsd.dim_z > 1 ? 0 : ctx->config.a_scale_radius;
 	if (radius != 0 && y1 > y0) {
 		AlphaWindow w = alpha_window(dim_y, radius, (unsigned int)y0, (unsigned int)y1);
@@ -930,11 +949,141 @@ static void slab_image_rows(const astcenc_context* ctx, unsigned int dim_y, unsi
 	}
 }
 
-static astcenc_error upload_rows(astcenc_context* ctx, const UploadPlan& up, size_t y0, size_t y1, cudaStream_t stream) {
-	CUDA_TRY(cudaMemcpyAsync(up.device + y0 * up.row_bytes, up.host + y0 * up.row_bytes, up.row_bytes * (y1 - y0), cudaMemcpyHostToDevice, ctx->copy_stream),
-	         return ASTCENC_ERR_BAD_CONTEXT);
-	CUDA_TRY(cudaEventRecord(ctx->band_ready[0], ctx->copy_stream), return ASTCENC_ERR_BAD_CONTEXT);
-	CUDA_TRY(cudaStreamWaitEvent(stream, ctx->band_ready[0], 0), return ASTCENC_ERR_BAD_CONTEXT);
+// Per-stage timing (astcenc_b200_stage_timing): an event on `stream` behind the launches of one stage of a batch (kind 0 set-up,
+// 1 refine, 2 prepare, 3 emit; -1 opens the batch).
+static void stage_mark(astcenc_context* ctx, int kind, cudaStream_t stream) {
+	if (!ctx->stage_timing) {
+		return;
+	}
+	const size_t i = ctx->stage_kinds.size();
+	if (i == ctx->stage_events.size()) {
+		cudaEvent_t e;
+		if (cudaEventCreate(&e) != cudaSuccess) {
+			return;
+		}
+		ctx->stage_events.push_back(e);
+	}
+	ctx->stage_kinds.push_back(kind);
+	cudaEventRecord(ctx->stage_events[i], stream);
+}
+
+// The WaveArgs of one pipeline over `blocks` blocks (blocks_x per row): its counter block, and its first block `first` in the
+// context's records and queues.
+static WaveArgs wave_args(const astcenc_context* ctx, uint32_t* counters, size_t first, unsigned int blocks, unsigned int blocks_x) {
+	const DevBsd& bsd = ctx->tables->bsd;
+	WaveArgs a;
+	a.records = ctx->d_records + first * (size_t)bsd.record_bytes;
+	a.queues = ctx->d_queues + first;
+	a.queue_stride = ctx->d_queues_bytes / (sizeof(uint32_t) * ASTC_Q_KINDS);
+	a.count = counters;
+	a.head = counters + ASTC_Q_KINDS * ASTC_MAX_WAVES;
+	a.total = blocks;
+	a.blocks_x = blocks_x;
+	a.ticket = counters + 2 * ASTC_Q_KINDS * ASTC_MAX_WAVES;
+	a.first_block = 0;
+	a.band_blocks = blocks;
+	a.cls_lo = 0;
+	a.cls_hi = ASTC_Q_CLASSES;
+	a.wave = 0;
+	a.sync_mask = ctx->knobs.sync_mask;
+	a.stage_bytes_setup = ctx->setup_stage_bytes;
+	a.refine_state_off = (uint32_t)(ASTC_SMEM_HDR + ctx->refine_stage_bytes + (size_t)bsd.arena_bytes_small * ctx->warps_small);
+	a.stage_bytes = ctx->refine_stage_bytes;
+	return a;
+}
+
+// The set-up launch(es) of wave a.wave of one pipeline. Wave 0 of a banded upload (`up`) runs one launch per band, each behind
+// the copy of its band's rows and taking the band's blocks from its own ticket. On the compact one-plane plan, class 0 of the
+// later waves (the two-plane trials) runs on the general plan; wave 0 and the n-partition classes have one weight plane and run
+// on the compact plan with more warps per SM.
+static astcenc_error enqueue_setup(astcenc_context* ctx, const DevImage& img, WaveArgs a, cudaStream_t stream, const UploadPlan* up) {
+	const SetupKernel kernel = setup_kernel(ctx->dcfg, a.wave);
+	const bool compact = ctx->warps_setup_1p != 0;
+	auto launch = [&](bool on_compact) {
+		if (on_compact) {
+			kernel<<<ctx->grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
+		} else {
+			kernel<<<ctx->grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(ctx->tables->bsd, ctx->dcfg, img, a);
+		}
+		ctx->launches++;
+	};
+	if (a.wave == 0 && up != nullptr) {
+		uint32_t* const ticket = a.ticket;
+		for (int k = 0; k < up->bands; k++) {
+			unsigned int r0, r1;
+			if (!band_of(img.block_rows, up->bands, k, r0, r1)) {
+				continue;
+			}
+			size_t y0, y1;
+			image_rows(img.block_row0 + r0, img.block_row0 + r1, ctx->tables->bsd.dim_y, img.dim_y, y0, y1);
+			astcenc_error st = upload_rows(ctx, *up, y0, y1, k, stream);
+			if (st != ASTCENC_SUCCESS) {
+				return st;
+			}
+			a.ticket = ticket + k;
+			a.first_block = r0 * img.blocks_x;
+			a.band_blocks = (r1 - r0) * img.blocks_x;
+			launch(compact);
+		}
+	} else {
+		if (compact && a.wave != 0) {
+			a.cls_lo = 0;
+			a.cls_hi = 1;
+			launch(false);
+			a.cls_lo = 1;
+			a.cls_hi = ASTC_Q_CLASSES;
+		}
+		launch(compact);
+	}
+	stage_mark(ctx, 0, stream);
+	return ASTCENC_SUCCESS;
+}
+
+// Refinement and preparation of wave a.wave of one pipeline.
+static void enqueue_refine_prepare(astcenc_context* ctx, const DevImage& img, const WaveArgs& a, cudaStream_t stream) {
+	const DevBsd& bsd = ctx->tables->bsd;
+	const int grid = ctx->grid;
+	if (refine_l1_step(ctx->dcfg)) {
+		astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+	} else {
+		astc_wave_refine_kernel<false><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+	}
+	ctx->launches++;
+	stage_mark(ctx, 1, stream);
+	// (statistics / partition search gain nothing from phase alignment: two half-size CTAs per SM wait less)
+	const int wp = ctx->warps_small >= 2 ? ctx->warps_small / 2 : 1;
+	astc_wave_prepare_kernel<<<grid * 2, wp * 32, ASTC_SMEM_HDR + (size_t)bsd.arena_bytes_small * wp, stream>>>(bsd, ctx->dcfg, img, a);
+	ctx->launches++;
+	stage_mark(ctx, 2, stream);
+}
+
+// The emit launch of one pipeline: the chosen encoding of every block into the payload.
+static void enqueue_emit(astcenc_context* ctx, const DevImage& img, WaveArgs a, cudaStream_t stream) {
+	a.wave = 0;
+	astc_wave_emit_kernel<<<ctx->grid * 4, ASTC_EMIT_THREADS, ASTC_SMEM_HDR + (ASTC_EMIT_THREADS / 32) * 32 * EMIT_SLICE, stream>>>(ctx->tables->bsd, ctx->dcfg, img, a);
+	ctx->launches++;
+	stage_mark(ctx, 3, stream);
+}
+
+// One batch of a slab on the wave pipeline: the waves of the search, then emit, on `stream`.
+static astcenc_error launch_batch(astcenc_context* ctx, const DevImage& img, cudaStream_t stream, const UploadPlan* up) {
+	CUDA_TRY(cudaMemsetAsync(ctx->d_counters, 0, sizeof(uint32_t) * ASTC_COUNTER_WORDS, stream), return ASTCENC_ERR_BAD_CONTEXT);
+	WaveArgs a = wave_args(ctx, ctx->d_counters, 0, img.blocks_x * img.block_rows, img.blocks_x);
+	if (ctx->stage_timing) {
+		ctx->stage_kinds.clear();
+	}
+	stage_mark(ctx, -1, stream);
+	for (int wave = 0; wave < ctx->max_waves; wave++) {
+		a.wave = wave;
+		a.sync_mask = wave == 0 ? ctx->knobs.sync_mask : ctx->knobs.sync_mask_tail;
+		astcenc_error st = enqueue_setup(ctx, img, a, stream, up);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
+		enqueue_refine_prepare(ctx, img, a, stream);
+	}
+	enqueue_emit(ctx, img, a, stream);
+	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 	return ASTCENC_SUCCESS;
 }
 
@@ -945,88 +1094,32 @@ static astcenc_error upload_rows(astcenc_context* ctx, const UploadPlan& up, siz
 // chain drains, the CTAs of the next chain's kernel take over the SMs that became free (every kernel is one CTA per SM,
 // so the hardware block scheduler does the interleaving). Same kernels, same results; wave 0 of chain p waits only for the
 // upload of its own rows (the band scheme of the host-pointer path with bands = pipelines).
-static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                  unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up) {
-	const DevBsd& bsd = ctx->tables->bsd;
-	unsigned int blocks_x = (dim_x + bsd.dim_x - 1) / bsd.dim_x;
-	size_t total = (size_t)blocks_x * block_rows;
-	if (total > ctx->queue_capacity) {
-		cudaFree(ctx->d_queues);
-		ctx->d_queues = nullptr;
-		ctx->queue_capacity = 0;
-		CUDA_TRY(cudaMalloc(&ctx->d_queues, sizeof(uint32_t) * ASTC_Q_KINDS * total), return ASTCENC_ERR_OUT_OF_MEM);
-		ctx->queue_capacity = total;
-	}
-	size_t rec_bytes = total * (size_t)bsd.record_bytes;
-	if (rec_bytes > ctx->d_records_bytes) {
-		cudaFree(ctx->d_records);
-		ctx->d_records = nullptr;
-		ctx->d_records_bytes = 0;
-		CUDA_TRY(cudaMalloc(&ctx->d_records, rec_bytes), return ASTCENC_ERR_OUT_OF_MEM);
-		ctx->d_records_bytes = rec_bytes;
-	}
+static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const DevImage& slab, cudaStream_t stream, const UploadPlan* up) {
 	DevImage img[ASTC_MAX_PIPES];
 	WaveArgs a[ASTC_MAX_PIPES];
-	if (up != nullptr && ctx->scratch_used) {
-		CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
-	}
 	CUDA_TRY(cudaEventRecord(ctx->pipe_start, stream), return ASTCENC_ERR_BAD_CONTEXT);
 	for (int p = 0; p < pipes; p++) {
-		unsigned int r0 = (unsigned int)((size_t)block_rows * p / pipes), r1 = (unsigned int)((size_t)block_rows * (p + 1) / pipes);
-		size_t first = (size_t)r0 * blocks_x;
+		unsigned int r0, r1;
+		slab_of(slab.block_rows, pipes, p, r0, r1);
 		cudaStream_t ps = ctx->pipe_stream[p];
 		CUDA_TRY(cudaStreamWaitEvent(ps, ctx->pipe_start, 0), return ASTCENC_ERR_BAD_CONTEXT);
-		DevImage& im = img[p];
-		im.data = d_pixels;
-		im.data_type = data_type;
-		im.dim_x = dim_x;
-		im.dim_y = dim_y;
-		im.dim_z = ctx->volume_dim_z;
-		im.blocks_x = blocks_x;
-		im.blocks_y = (dim_y + bsd.dim_y - 1) / bsd.dim_y;
-		im.block_row0 = block_row0 + r0;
-		im.block_rows = r1 - r0;
-		for (int i = 0; i < 4; i++) {
-			im.swz[i] = swz[i];
-		}
-		im.out = d_out + first * 16;
-		im.alpha_avg = ctx->config.a_scale_radius != 0 && bsd.dim_z == 1 ? ctx->d_alpha : nullptr;
-		im.alpha_threshold = ctx->alpha_threshold;
-		im.cancel = ctx->pass_cancel;
-		im.done = ctx->pass_done;
+		img[p] = slab;
+		img[p].block_row0 = slab.block_row0 + r0;
+		img[p].block_rows = r1 - r0;
+		img[p].out = slab.out + (size_t)r0 * slab.blocks_x * 16;
 		uint32_t* counters = ctx->d_counters + (size_t)p * ASTC_COUNTER_WORDS;
 		CUDA_TRY(cudaMemsetAsync(counters, 0, sizeof(uint32_t) * ASTC_COUNTER_WORDS, ps), return ASTCENC_ERR_BAD_CONTEXT);
-		WaveArgs& w = a[p];
-		w.records = ctx->d_records + first * (size_t)bsd.record_bytes;
-		w.queues = ctx->d_queues + first;
-		w.queue_stride = ctx->queue_capacity;
-		w.count = counters;
-		w.head = counters + ASTC_Q_KINDS * ASTC_MAX_WAVES;
-		w.total = (r1 - r0) * blocks_x;
-		w.blocks_x = blocks_x;
-		w.ticket = counters + 2 * ASTC_Q_KINDS * ASTC_MAX_WAVES;
-		w.first_block = 0;
-		w.band_blocks = w.total;
-		w.cls_lo = 0;
-		w.cls_hi = ASTC_Q_CLASSES;
-		w.stage_bytes = ctx->refine_stage_bytes;
-		w.refine_state_off = (uint32_t)(ASTC_SMEM_HDR + ctx->refine_stage_bytes + (size_t)bsd.arena_bytes_small * ctx->warps_small);
-		w.stage_bytes_setup = ctx->setup_stage_bytes;
-		w.sync_mask = ctx->knobs.sync_mask;
+		a[p] = wave_args(ctx, counters, (size_t)r0 * slab.blocks_x, (r1 - r0) * slab.blocks_x, slab.blocks_x);
 		if (up != nullptr) {
 			// this pipeline's rows go up on the copy stream; only its wave 0 waits for them
-			size_t y0 = (size_t)(block_row0 + r0) * bsd.dim_y, y1 = (size_t)(block_row0 + r1) * bsd.dim_y;
-			if (y1 > dim_y) y1 = dim_y;
-			if (y1 > y0) {
-				CUDA_TRY(cudaMemcpyAsync(up->device + y0 * up->row_bytes, up->host + y0 * up->row_bytes, (y1 - y0) * up->row_bytes, cudaMemcpyHostToDevice, ctx->copy_stream),
-				         return ASTCENC_ERR_BAD_CONTEXT);
+			size_t y0, y1;
+			image_rows(slab.block_row0 + r0, slab.block_row0 + r1, ctx->tables->bsd.dim_y, slab.dim_y, y0, y1);
+			astcenc_error st = upload_rows(ctx, *up, y0, y1, p, ps);
+			if (st != ASTCENC_SUCCESS) {
+				return st;
 			}
-			CUDA_TRY(cudaEventRecord(ctx->band_ready[p], ctx->copy_stream), return ASTCENC_ERR_BAD_CONTEXT);
-			CUDA_TRY(cudaStreamWaitEvent(ps, ctx->band_ready[p], 0), return ASTCENC_ERR_BAD_CONTEXT);
 		}
 	}
-	int grid = ctx->grid;
-	int wp = ctx->warps_small >= 2 ? ctx->warps_small / 2 : 1;
 	for (int wave = 0; wave < ctx->max_waves; wave++) {
 		for (int p = 0; p < pipes; p++) {
 			if (a[p].total == 0) {
@@ -1034,37 +1127,17 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d
 			}
 			a[p].wave = wave;
 			a[p].sync_mask = wave == 0 ? ctx->knobs.sync_mask : ctx->knobs.sync_mask_tail;
-			cudaStream_t ps = ctx->pipe_stream[p];
-			if (ctx->warps_setup_1p) {
-				if (wave != 0) {
-					a[p].cls_lo = 0;
-					a[p].cls_hi = 1;
-					astc_wave_setup_kernel<false><<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
-					ctx->launches++;
-					a[p].cls_lo = 1;
-					a[p].cls_hi = ASTC_Q_CLASSES;
-				}
-				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, ps>>>(ctx->tables->bsd_1p, ctx->dcfg, img[p], a[p]);
-				a[p].cls_lo = 0;
-				a[p].cls_hi = ASTC_Q_CLASSES;
-			} else {
-				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup * 32, ctx->smem_setup, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
+			astcenc_error st = enqueue_setup(ctx, img[p], a[p], ctx->pipe_stream[p], nullptr);
+			if (st != ASTCENC_SUCCESS) {
+				return st;
 			}
-			if (refine_l1_step(ctx->dcfg)) {
-				astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
-			} else {
-				astc_wave_refine_kernel<false><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
-			}
-			astc_wave_prepare_kernel<<<grid * 2, wp * 32, ASTC_SMEM_HDR + (size_t)bsd.arena_bytes_small * wp, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
-			ctx->launches += 3;
+			enqueue_refine_prepare(ctx, img[p], a[p], ctx->pipe_stream[p]);
 		}
 	}
 	for (int p = 0; p < pipes; p++) {
 		cudaStream_t ps = ctx->pipe_stream[p];
 		if (a[p].total != 0) {
-			a[p].wave = 0;
-			astc_wave_emit_kernel<<<grid * 4, ASTC_EMIT_THREADS, ASTC_SMEM_HDR + (ASTC_EMIT_THREADS / 32) * 32 * EMIT_SLICE, ps>>>(bsd, ctx->dcfg, img[p], a[p]);
-			ctx->launches++;
+			enqueue_emit(ctx, img[p], a[p], ps);
 		}
 		CUDA_TRY(cudaEventRecord(ctx->pipe_done[p], ps), return ASTCENC_ERR_BAD_CONTEXT);
 		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->pipe_done[p], 0), return ASTCENC_ERR_BAD_CONTEXT);
@@ -1073,11 +1146,26 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const void* d
 	return ASTCENC_SUCCESS;
 }
 
-// The alpha-scale pre-pass over image rows [y0, y1) of a 2D image (alpha_window: the 32 x 32 tiles that cover them, reading up to
-// a_scale_radius rows beyond); the averages land at their image positions in `averages` (dim_x * dim_y floats). Sets the
-// threshold the set-up stage compares them with.
-static astcenc_error alpha_prepass(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                   unsigned int y0, unsigned int y1, float* averages, cudaStream_t stream) {
+// One batch of a slab on a single-kernel driver (ASTCENC_B200_DRIVER=lockstep|warp).
+static astcenc_error launch_driver(astcenc_context* ctx, const DevImage& img, cudaStream_t stream) {
+	CUDA_TRY(cudaMemsetAsync(ctx->d_ticket, 0, sizeof(unsigned int), stream), return ASTCENC_ERR_BAD_CONTEXT);
+	int grid = ctx->grid;
+	size_t total = (size_t)img.blocks_x * img.block_rows;
+	size_t needed = (total + ctx->warps_per_cta - 1) / ctx->warps_per_cta;
+	if ((size_t)grid > needed) {
+		grid = (int)(needed ? needed : 1);
+	}
+	astc_compress_kernel<<<grid, ctx->warps_per_cta * 32, ctx->smem_bytes, stream>>>(ctx->tables->bsd, ctx->dcfg, img, ctx->d_ticket, ctx->knobs.coherence_probe, ctx->lockstep);
+	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+	ctx->launches++;
+	return ASTCENC_SUCCESS;
+}
+
+// The alpha-scale pre-pass over the image rows of block rows [r0, r1) of a 2D image (alpha_window: the 32 x 32 tiles that cover
+// them, reading up to a_scale_radius rows beyond); the averages land at their image positions in `averages` (dim_x * dim_y
+// floats), and `threshold` receives the value the set-up stage compares them with.
+static astcenc_error alpha_prepass(astcenc_context* ctx, const DevImage& src, unsigned int r0, unsigned int r1, float* averages, cudaStream_t stream,
+                                   float& threshold) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	const unsigned int radius = ctx->config.a_scale_radius;
 	size_t pad = (size_t)ALPHA_TILE + 2 * (size_t)radius + 1;
@@ -1088,32 +1176,32 @@ static astcenc_error alpha_prepass(astcenc_context* ctx, const void* d_pixels, i
 	if (smem > 48 * 1024) {
 		CUDA_TRY(cudaFuncSetAttribute(astc_alpha_average_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), return ASTCENC_ERR_BAD_CONTEXT);
 	}
-	DevImage aimg{};
-	aimg.data = d_pixels;
-	aimg.data_type = data_type;
-	aimg.dim_x = dim_x;
-	aimg.dim_y = dim_y;
-	for (int i = 0; i < 4; i++) {
-		aimg.swz[i] = swz[i];
-	}
-	aimg.cancel = ctx->pass_cancel;
-	unsigned int tiles_x = (dim_x + ALPHA_TILE - 1) / ALPHA_TILE;
-	AlphaWindow win = alpha_window(dim_y, radius, y0, y1);
-	astc_alpha_average_kernel<<<tiles_x * win.tile_rows, ASTC_ALPHA_THREADS, smem, stream>>>(aimg, radius, tiles_x, win.tile_row0, averages);
+	size_t y0, y1;
+	image_rows(r0, r1, bsd.dim_y, src.dim_y, y0, y1);
+	unsigned int tiles_x = (src.dim_x + ALPHA_TILE - 1) / ALPHA_TILE;
+	AlphaWindow win = alpha_window(src.dim_y, radius, (unsigned int)y0, (unsigned int)y1);
+	astc_alpha_average_kernel<<<tiles_x * win.tile_rows, ASTC_ALPHA_THREADS, smem, stream>>>(src, radius, tiles_x, win.tile_row0, averages);
 	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 	ctx->launches++;
 	// astcenc_entry.cpp:983-988
 	size_t x_footprint = bsd.dim_x + 2 * ((size_t)radius - 1);
 	size_t y_footprint = bsd.dim_y + 2 * ((size_t)radius - 1);
 	float footprint = static_cast<float>(x_footprint * y_footprint);
-	ctx->alpha_threshold = 0.9f / (255.0f * footprint);
+	threshold = 0.9f / (255.0f * footprint);
 	return ASTCENC_SUCCESS;
 }
 
-static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                        unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up) {
+// A slab of block rows is processed in batches of at most ~1 M blocks: the per-block search records (a few KB each)
+// are the only buffer that grows with the image, and the batches reuse them in stream order. A 2D pass given no alpha
+// averages with a_scale_radius set runs its own pre-pass over the slab's window first.
+static astcenc_error launch_slab_locked(astcenc_context* ctx, const DevImage& src, unsigned int block_row0, unsigned int block_rows, uint8_t* d_out,
+                                        cudaStream_t stream, const UploadPlan* up) {
 	const DevBsd& bsd = ctx->tables->bsd;
-	size_t blocks_x = (dim_x + bsd.dim_x - 1) / bsd.dim_x;
+	DevImage img = src;
+	img.block_row0 = block_row0;
+	img.block_rows = block_rows;
+	img.out = d_out;
+	const size_t blocks_x = img.blocks_x;
 	size_t rows_per_batch = ctx->knobs.batch_blocks / (blocks_x ? blocks_x : 1);
 	if (rows_per_batch < 1) rows_per_batch = 1;
 	const unsigned int radius = bsd.dim_z > 1 ? 0 : ctx->config.a_scale_radius;      // (the averages only steer 2D block sizes, astcenc_entry.cpp:975)
@@ -1124,234 +1212,67 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const void* d_pixe
 	                 blocks_x * block_rows >= (size_t)pipes * 8192;
 	// banded uploads need the whole slab in one batch on the wave pipeline, and no pre-pass that reads the window first
 	bool banded = up != nullptr && radius == 0 && ctx->driver == 0 && single_batch && (use_pipes || (up->bands > 1 && block_rows >= (unsigned int)up->bands * 4));
-	if (up != nullptr && !banded) {
+	if (up != nullptr && ctx->scratch_used) {
 		// the upload streams on the copy stream; it must not overtake a pass that still reads the image buffer
-		if (ctx->scratch_used) {
-			CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
-		}
+		CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
+	}
+	if (up != nullptr && !banded) {
 		size_t y0, y1;
-		slab_image_rows(ctx, dim_y, block_row0, block_rows, y0, y1);
-		astcenc_error st = upload_rows(ctx, *up, y0, y1, stream);
+		slab_image_rows(ctx, img.dim_y, block_row0, block_rows, y0, y1);
+		astcenc_error st = upload_rows(ctx, *up, y0, y1, 0, stream);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
 		up = nullptr;
 	}
-	if (radius != 0 && !ctx->pass_alpha_staged) {
-		// alpha-scale pre-pass over the tiles that cover the slab's rows: the box filter reaches across slab borders, so
-		// the window reads up to `radius` rows beyond the tiles (alpha_window); the averages stay at their image positions
-		size_t need = (size_t)dim_x * dim_y * sizeof(float);
-		if (need > ctx->d_alpha_bytes) {
-			cudaFree(ctx->d_alpha);
-			ctx->d_alpha = nullptr;
-			ctx->d_alpha_bytes = 0;
-			CUDA_TRY(cudaMalloc(&ctx->d_alpha, need), return ASTCENC_ERR_OUT_OF_MEM);
-			ctx->d_alpha_bytes = need;
+	if (radius != 0 && img.alpha_avg == nullptr) {
+		// the box filter reaches across slab borders: the window reads up to `radius` rows beyond the tiles that cover the
+		// slab's rows (alpha_window); the averages stay at their image positions
+		astcenc_error st = ensure_scratch(ctx, 0, (size_t)img.dim_x * img.dim_y);
+		if (st == ASTCENC_SUCCESS) {
+			st = alpha_prepass(ctx, img, block_row0, block_row0 + block_rows, ctx->d_alpha, stream, img.alpha_threshold);
 		}
-		size_t y1 = (size_t)(block_row0 + block_rows) * bsd.dim_y;
-		astcenc_error st = alpha_prepass(ctx, d_pixels, data_type, dim_x, dim_y, swz, block_row0 * bsd.dim_y, y1 < dim_y ? (unsigned int)y1 : dim_y, ctx->d_alpha, stream);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
+		img.alpha_avg = ctx->d_alpha;
+	}
+	if (ctx->driver == 0) {
+		astcenc_error st = ensure_scratch(ctx, blocks_x * (single_batch ? block_rows : rows_per_batch), 0);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
 	}
 	if (use_pipes) {
-		return launch_pipes(ctx, pipes, d_pixels, data_type, dim_x, dim_y, swz, block_row0, block_rows, d_out, stream, banded ? up : nullptr);
+		return launch_pipes(ctx, pipes, img, stream, up);
 	}
-	unsigned int done = 0;
-	while (done < block_rows) {
-		unsigned int rows = block_rows - done;
-		if ((size_t)rows > rows_per_batch) rows = (unsigned int)rows_per_batch;
-		astcenc_error st = launch_batch(ctx, d_pixels, data_type, dim_x, dim_y, swz, block_row0 + done, rows, d_out + (size_t)done * blocks_x * 16, stream, banded ? up : nullptr);
+	for (unsigned int done = 0; done < block_rows;) {
+		DevImage batch = img;
+		batch.block_row0 = block_row0 + done;
+		batch.block_rows = block_rows - done < rows_per_batch ? block_rows - done : (unsigned int)rows_per_batch;
+		batch.out = d_out + (size_t)done * blocks_x * 16;
+		astcenc_error st = ctx->driver == 0 ? launch_batch(ctx, batch, stream, up) : launch_driver(ctx, batch, stream);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
-		done += rows;
+		done += batch.block_rows;
 	}
 	return ASTCENC_SUCCESS;
 }
 
-static astcenc_error launch_batch(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, const int swz[4],
-                                  unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream, const UploadPlan* up) {
-	const DevBsd& bsd = ctx->tables->bsd;
-	DevImage img;
-	img.data = d_pixels;
-	img.data_type = data_type;
-	img.dim_x = dim_x;
-	img.dim_y = dim_y;
-	img.dim_z = ctx->volume_dim_z;
-	img.blocks_x = (dim_x + bsd.dim_x - 1) / bsd.dim_x;
-	img.blocks_y = (dim_y + bsd.dim_y - 1) / bsd.dim_y;
-	img.block_row0 = block_row0;
-	img.block_rows = block_rows;
-	for (int i = 0; i < 4; i++) {
-		img.swz[i] = swz[i];
+// The context's scratch buffers serve one pass at a time. Calls may come from several host threads and on different
+// streams: launch_mtx serialises the enqueueing, and every pass starts by making its stream wait for the event that
+// closes the previous pass (a no-op when both ran on the same stream).
+static astcenc_error launch_slab(astcenc_context* ctx, const DevImage& src, unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream,
+                                 const UploadPlan* up = nullptr) {
+	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
+	if (ctx->scratch_used) {
+		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
-	img.out = d_out;
-	img.alpha_avg = ctx->config.a_scale_radius != 0 && bsd.dim_z == 1 ? ctx->d_alpha : nullptr;
-	img.alpha_threshold = ctx->alpha_threshold;
-	img.cancel = ctx->pass_cancel;
-	img.done = ctx->pass_done;
-	size_t total = (size_t)img.blocks_x * block_rows;
-	if (ctx->driver == 0) {
-		// ---- wave pipeline ----
-		if (total > ctx->queue_capacity) {
-			cudaFree(ctx->d_queues);
-			ctx->d_queues = nullptr;
-			ctx->queue_capacity = 0;
-			CUDA_TRY(cudaMalloc(&ctx->d_queues, sizeof(uint32_t) * ASTC_Q_KINDS * total), return ASTCENC_ERR_OUT_OF_MEM);
-			ctx->queue_capacity = total;
-		}
-		size_t rec_bytes = total * (size_t)bsd.record_bytes;
-		if (rec_bytes > ctx->d_records_bytes) {
-			cudaFree(ctx->d_records);
-			ctx->d_records = nullptr;
-			ctx->d_records_bytes = 0;
-			CUDA_TRY(cudaMalloc(&ctx->d_records, rec_bytes), return ASTCENC_ERR_OUT_OF_MEM);
-			ctx->d_records_bytes = rec_bytes;
-		}
-		CUDA_TRY(cudaMemsetAsync(ctx->d_counters, 0, sizeof(uint32_t) * ASTC_COUNTER_WORDS, stream), return ASTCENC_ERR_BAD_CONTEXT);
-		WaveArgs a;
-		a.records = ctx->d_records;
-		a.queues = ctx->d_queues;
-		a.queue_stride = ctx->queue_capacity;
-		a.count = ctx->d_counters;
-		a.head = ctx->d_counters + ASTC_Q_KINDS * ASTC_MAX_WAVES;
-		a.total = (unsigned int)total;
-		a.blocks_x = img.blocks_x;
-		a.ticket = ctx->d_counters + 2 * ASTC_Q_KINDS * ASTC_MAX_WAVES;
-		a.first_block = 0;
-		a.band_blocks = (unsigned int)total;
-		a.cls_lo = 0;
-		a.cls_hi = ASTC_Q_CLASSES;
-		a.stage_bytes = ctx->refine_stage_bytes;
-		a.refine_state_off = (uint32_t)(ASTC_SMEM_HDR + ctx->refine_stage_bytes + (size_t)bsd.arena_bytes_small * ctx->warps_small);
-		a.stage_bytes_setup = ctx->setup_stage_bytes;
-		a.sync_mask = ctx->knobs.sync_mask;
-		int grid = ctx->grid;
-		size_t ev_used = 0;
-		auto mark = [&](int kind) {
-			if (!ctx->stage_timing) {
-				return;
-			}
-			if (ev_used == ctx->stage_events.size()) {
-				cudaEvent_t e;
-				if (cudaEventCreate(&e) != cudaSuccess) {
-					return;
-				}
-				ctx->stage_events.push_back(e);
-				ctx->stage_kinds.push_back(kind);
-			}
-			ctx->stage_kinds[ev_used] = kind;
-			cudaEventRecord(ctx->stage_events[ev_used++], stream);
-		};
-		if (ctx->stage_timing) {
-			ctx->stage_kinds.clear();
-			ctx->stage_kinds.resize(ctx->stage_events.size(), -1);
-		}
-		mark(-1);
-		for (int wave = 0; wave < ctx->max_waves; wave++) {
-			a.wave = wave;
-			a.sync_mask = wave == 0 ? ctx->knobs.sync_mask : ctx->knobs.sync_mask_tail;
-			if (wave == 0 && up != nullptr) {
-				// bands of block rows, growing (1 : 3 : 4 : 8 ...) so that the first copy - the only one nothing hides - is short
-				static const unsigned int shares[ASTC_MAX_BANDS] = {1, 3, 4, 8, 8, 8, 8, 8};
-				unsigned int sum = 0;
-				for (int k = 0; k < up->bands; k++) sum += shares[k];
-				if (ctx->scratch_used) {
-					CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
-				}
-				unsigned int row = 0, acc = 0;
-				for (int k = 0; k < up->bands; k++) {
-					acc += shares[k];
-					unsigned int row_end = k == up->bands - 1 ? block_rows : (unsigned int)((size_t)block_rows * acc / sum);
-					if (row_end <= row) {
-						continue;
-					}
-					// image rows of block rows [row, row_end) of this slab
-					size_t y0 = (size_t)(block_row0 + row) * bsd.dim_y;
-					size_t y1 = (size_t)(block_row0 + row_end) * bsd.dim_y;
-					if (y1 > dim_y) y1 = dim_y;
-					if (y1 > y0) {
-						CUDA_TRY(cudaMemcpyAsync(up->device + y0 * up->row_bytes, up->host + y0 * up->row_bytes, (y1 - y0) * up->row_bytes, cudaMemcpyHostToDevice, ctx->copy_stream),
-						         return ASTCENC_ERR_BAD_CONTEXT);
-					}
-					CUDA_TRY(cudaEventRecord(ctx->band_ready[k], ctx->copy_stream), return ASTCENC_ERR_BAD_CONTEXT);
-					CUDA_TRY(cudaStreamWaitEvent(stream, ctx->band_ready[k], 0), return ASTCENC_ERR_BAD_CONTEXT);
-					a.ticket = ctx->d_counters + 2 * ASTC_Q_KINDS * ASTC_MAX_WAVES + k;
-					a.first_block = row * img.blocks_x;
-					a.band_blocks = (row_end - row) * img.blocks_x;
-					if (ctx->warps_setup_1p) {
-						setup_kernel(ctx->dcfg, 0)<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
-					} else {
-						setup_kernel(ctx->dcfg, 0)<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
-					}
-					ctx->launches++;
-					row = row_end;
-				}
-				mark(0);
-				ctx->launches--;      // (the loop below counts one set-up launch per wave)
-			} else if (ctx->warps_setup_1p) {
-				// class 0 of the later waves holds the two-plane trials (general plan); wave 0 and the n-partition classes have
-				// one weight plane and run on the compact plan with more warps per SM
-				if (wave != 0) {
-					a.cls_lo = 0;
-					a.cls_hi = 1;
-					astc_wave_setup_kernel<false><<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
-					ctx->launches++;
-					a.cls_lo = 1;
-					a.cls_hi = ASTC_Q_CLASSES;
-				}
-				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
-				a.cls_lo = 0;
-				a.cls_hi = ASTC_Q_CLASSES;
-				mark(0);
-			} else {
-				setup_kernel(ctx->dcfg, wave)<<<grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(bsd, ctx->dcfg, img, a);
-				mark(0);
-			}
-			if (refine_l1_step(ctx->dcfg)) {
-				astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
-			} else {
-				astc_wave_refine_kernel<false><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
-			}
-			mark(1);
-			// (statistics / partition search gain nothing from phase alignment: two half-size CTAs per SM wait less)
-			int wp = ctx->warps_small >= 2 ? ctx->warps_small / 2 : 1;
-			astc_wave_prepare_kernel<<<grid * 2, wp * 32, ASTC_SMEM_HDR + (size_t)bsd.arena_bytes_small * wp, stream>>>(bsd, ctx->dcfg, img, a);
-			mark(2);
-			ctx->launches += 3;
-		}
-		a.wave = 0;
-		astc_wave_emit_kernel<<<grid * 4, ASTC_EMIT_THREADS, ASTC_SMEM_HDR + (ASTC_EMIT_THREADS / 32) * 32 * EMIT_SLICE, stream>>>(bsd, ctx->dcfg, img, a);
-		mark(3);
-		if (ctx->stage_timing) {
-			ctx->stage_kinds.resize(ev_used);
-		}
-		ctx->launches++;
-		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
-		return ASTCENC_SUCCESS;
-	}
-	CUDA_TRY(cudaMemsetAsync(ctx->d_ticket, 0, sizeof(unsigned int), stream), return ASTCENC_ERR_BAD_CONTEXT);
-	int grid = ctx->grid;
-	size_t needed = (total + ctx->warps_per_cta - 1) / ctx->warps_per_cta;
-	if ((size_t)grid > needed) {
-		grid = (int)(needed ? needed : 1);
-	}
-	astc_compress_kernel<<<grid, ctx->warps_per_cta * 32, ctx->smem_bytes, stream>>>(bsd, ctx->dcfg, img, ctx->d_ticket, ctx->knobs.coherence_probe, ctx->lockstep);
-	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
-	ctx->launches++;
-	return ASTCENC_SUCCESS;
-}
-
-static astcenc_error ensure_buffer(uint8_t*& buf, size_t& have, size_t need) {
-	if (have < need) {
-		cudaFree(buf);
-		buf = nullptr;
-		have = 0;
-		CUDA_TRY(cudaMalloc(&buf, need), return ASTCENC_ERR_OUT_OF_MEM);
-		have = need;
-	}
-	return ASTCENC_SUCCESS;
+	astcenc_error st = launch_slab_locked(ctx, src, block_row0, block_rows, d_out, stream, up);
+	CUDA_TRY(cudaEventRecord(ctx->scratch_done, stream), return ASTCENC_ERR_BAD_CONTEXT);
+	ctx->scratch_used = true;
+	return st;
 }
 
 // Progress of one astcenc_compress_image call, reported like the reference's task pool (astcenc_internal_entry.h:199-295):
@@ -1407,88 +1328,53 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
+	// 3D block sizes (astcenc_entry.cpp:906-1043): one pass over the volume, whose slices go up into one contiguous buffer before
+	// it; its blocks come out in (z, y, x) order and its "block rows" count layer * blocks_y + row. 3D images with 2D blocks are
+	// an array of independent 2D slices (astcenc.h:94-100): one banded pass per slice. Progress runs over all passes.
+	const bool volume = bsd.dim_z > 1;
+	const unsigned int passes = volume ? 1 : image.dim_z;
+	const unsigned int pass_slices = volume ? image.dim_z : 1;
 	size_t bpt = image.data_type == ASTCENC_TYPE_U8 ? 4 : image.data_type == ASTCENC_TYPE_F16 ? 8 : 16;
 	size_t slice_bytes = (size_t)image.dim_x * image.dim_y * bpt;
 	size_t blocks_x = block_count_axis(image.dim_x, bsd.dim_x);
 	size_t blocks_y = block_count_axis(image.dim_y, bsd.dim_y);
-	size_t out_bytes = blocks_x * blocks_y * 16;
-	astcenc_error st = ensure_buffer(ctx->d_image, ctx->d_image_bytes, slice_bytes);
+	size_t layers = volume ? block_count_axis(image.dim_z, bsd.dim_z) : 1;
+	size_t out_bytes = blocks_x * blocks_y * layers * 16;      // payload of one pass
+	astcenc_error st = ensure_buffer(ctx->d_image, ctx->d_image_bytes, slice_bytes * pass_slices);
 	if (st == ASTCENC_SUCCESS) {
 		st = ensure_buffer(ctx->d_out, ctx->d_out_bytes, out_bytes);
 	}
 	if (st != ASTCENC_SUCCESS) {
 		return st;
 	}
-	int swz[4] = {(int)swizzle.r, (int)swizzle.g, (int)swizzle.b, (int)swizzle.a};
 	ctx->last_h2d = ctx->last_d2h = 0;
 	ctx->last_kernel_ms = 0.0f;
 	float total_ms = 0.0f;
 	// the pass starts behind the last flag clear (astcenc_compress_reset), with its done counter at zero
-	uint32_t* d_cancel = ctx->d_words;
-	uint32_t* d_done = ctx->d_words + 1;
+	DevImage src = pass_image(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, pass_slices, swizzle);
+	src.cancel = ctx->d_words;
+	src.done = ctx->d_words + 1;
 	CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ctl_ready, 0), return ASTCENC_ERR_BAD_CONTEXT);
-	CUDA_TRY(cudaMemsetAsync(d_done, 0, sizeof(uint32_t), ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+	CUDA_TRY(cudaMemsetAsync(src.done, 0, sizeof(uint32_t), ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	PassProgress pp;
 	pp.callback = ctx->config.progress_callback;
-	pp.total = static_cast<float>(blocks_x * blocks_y * (bsd.dim_z > 1 ? block_count_axis(image.dim_z, bsd.dim_z) : (size_t)image.dim_z));
+	pp.total = static_cast<float>(blocks_x * blocks_y * layers * passes);
 	pp.min_diff = (4096.0f / pp.total) * 100.0f;
 	pp.min_diff = pp.min_diff > 1.0f ? pp.min_diff : 1.0f;
 	pp.last = 0.0f;
-	if (bsd.dim_z > 1) {
-		// 3D block sizes (astcenc_entry.cpp:906-1043): the slices go up into one contiguous volume, the blocks come out in (z, y, x)
-		// order; "block rows" of the pass count layer * blocks_y + row
-		size_t blocks_z = block_count_axis(image.dim_z, bsd.dim_z);
-		size_t vol_out = out_bytes * blocks_z;
-		st = ensure_buffer(ctx->d_image, ctx->d_image_bytes, slice_bytes * image.dim_z);
-		if (st == ASTCENC_SUCCESS) {
-			st = ensure_buffer(ctx->d_out, ctx->d_out_bytes, vol_out);
-		}
-		if (st != ASTCENC_SUCCESS) {
-			return st;
-		}
+	for (unsigned int z = 0; z < passes; z++) {
 		if (ctx->cancel.load()) {
 			return ASTCENC_SUCCESS;
 		}
-		for (unsigned int z = 0; z < image.dim_z; z++) {
-			CUDA_TRY(cudaMemcpyAsync(ctx->d_image + (size_t)z * slice_bytes, image.data[z], slice_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		UploadPlan up = {static_cast<const uint8_t*>(image.data[z]), ctx->d_image, (size_t)image.dim_x * bpt, ctx->knobs.upload_bands};
+		if (volume) {
+			st = upload_slices(ctx->d_image, image.data, 0, image.dim_z, slice_bytes, ctx->stream);
+			if (st != ASTCENC_SUCCESS) {
+				return st;
+			}
 		}
 		CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		st = launch_slab(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, swz, 0, (unsigned int)(blocks_y * blocks_z), ctx->d_out, ctx->stream, nullptr, image.dim_z,
-		                 d_cancel, d_done);
-		if (st != ASTCENC_SUCCESS) {
-			return st;
-		}
-		CUDA_TRY(cudaEventRecord(ctx->ev1, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		st = wait_pass(ctx, ctx->ev1, pp);
-		if (st != ASTCENC_SUCCESS) {
-			return st;
-		}
-		if (ctx->cancel.load()) {
-			return ASTCENC_SUCCESS;
-		}
-		CUDA_TRY(cudaMemcpyAsync(data_out, ctx->d_out, vol_out, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		cudaEventElapsedTime(&total_ms, ctx->ev0, ctx->ev1);
-		ctx->last_kernel_ms = total_ms;
-		ctx->last_h2d = slice_bytes * image.dim_z;
-		ctx->last_d2h = vol_out;
-		if (pp.callback) {
-			pp.callback(100.0f);
-		}
-		return ASTCENC_SUCCESS;
-	}
-	// 3D images with 2D blocks are an array of independent 2D slices (astcenc.h:94-100); progress runs over all of them
-	for (unsigned int z = 0; z < image.dim_z; z++) {
-		if (ctx->cancel.load()) {
-			return ASTCENC_SUCCESS;
-		}
-		UploadPlan up;
-		up.host = static_cast<const uint8_t*>(image.data[z]);
-		up.device = ctx->d_image;
-		up.row_bytes = (size_t)image.dim_x * bpt;
-		up.bands = ctx->knobs.upload_bands;
-		CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		st = launch_slab(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, swz, 0, (unsigned int)blocks_y, ctx->d_out, ctx->stream, &up, 1, d_cancel, d_done);
+		st = launch_slab(ctx, src, 0, (unsigned int)(blocks_y * layers), ctx->d_out, ctx->stream, volume ? nullptr : &up);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
@@ -1505,7 +1391,7 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 		float ms = 0.0f;
 		cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
 		total_ms += ms;
-		ctx->last_h2d += slice_bytes;
+		ctx->last_h2d += slice_bytes * pass_slices;
 		ctx->last_d2h += out_bytes;
 	}
 	ctx->last_kernel_ms = total_ms;
@@ -1988,25 +1874,23 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	int swz[4] = {(int)swizzle->r, (int)swizzle->g, (int)swizzle->b, (int)swizzle->a};
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_slab(ctx, d_pixels, (int)data_type, dim_x, dim_y, swz, block_row0, block_rows, d_out, s);
+	return launch_slab(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, 1, *swizzle), block_row0, block_rows, d_out, s);
 }
 
 // Block lists (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk (a staging row is
 // one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks blocks). The
-// whole call is one turn of the context's scratch (launch_mtx, scratch_done), like a launch_slab.
-static astcenc_error launch_blocks(astcenc_context* ctx, const void* d_pixels, int data_type, unsigned int dim_x, unsigned int dim_y, unsigned int dim_z,
-                                   const int swz[4], const std::vector<uint32_t>& list, unsigned int row_lo, unsigned int row_hi, uint8_t* d_payload, cudaStream_t stream) {
+// whole call is one turn of the context's scratch (launch_mtx, scratch_done), like a launch_slab. `src` is the whole source
+// image, dim_z slices of it.
+static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, const astcenc_swizzle& swizzle, const std::vector<uint32_t>& list,
+                                   unsigned int row_lo, unsigned int row_hi, uint8_t* d_payload, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	const bool volume = bsd.dim_z > 1;
 	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
 	const size_t n = list.size();
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
-	const unsigned int words = data_type == ASTCENC_TYPE_U8 ? 1 : data_type == ASTCENC_TYPE_F16 ? 2 : 4;
+	const unsigned int words = src.data_type == ASTCENC_TYPE_U8 ? 1 : src.data_type == ASTCENC_TYPE_F16 ? 2 : 4;
 	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
-	ctx->volume_dim_z = volume ? bsd.dim_z : 1;      // (the staging volume is one layer deep)
-	ctx->pass_cancel = ctx->pass_done = nullptr;
 	if (ctx->scratch_used) {
 		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
@@ -2014,37 +1898,30 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const void* d_pixels, i
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_list_image, ctx->d_list_image_bytes, chunk * bsd.texel_count * words * 4);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_list_out, ctx->d_list_out_bytes, chunk * 16);
 	if (st == ASTCENC_SUCCESS && radius != 0) {
-		st = ensure_buffer(ctx->d_list_alpha, ctx->d_list_alpha_bytes, (size_t)dim_x * dim_y * sizeof(float));
-		if (st == ASTCENC_SUCCESS && chunk * bsd.texel_count * sizeof(float) > ctx->d_alpha_bytes) {
-			cudaFree(ctx->d_alpha);
-			ctx->d_alpha = nullptr;
-			ctx->d_alpha_bytes = 0;
-			CUDA_TRY(cudaMalloc(&ctx->d_alpha, chunk * bsd.texel_count * sizeof(float)), st = ASTCENC_ERR_OUT_OF_MEM);
-			if (st == ASTCENC_SUCCESS) ctx->d_alpha_bytes = chunk * bsd.texel_count * sizeof(float);
-		}
+		st = ensure_buffer(ctx->d_list_alpha, ctx->d_list_alpha_bytes, (size_t)src.dim_x * src.dim_y * sizeof(float));
+		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
 	if (st == ASTCENC_SUCCESS) {
 		// (from pageable memory: staged by the driver before the call returns, so `list` may go when this function does)
 		CUDA_TRY(cudaMemcpyAsync(ctx->d_list, list.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
+	// The staging pass reads averages gathered from the source's, so it runs no pre-pass of its own: its box filter would reach
+	// across the seams between unrelated blocks. The source's averages cover the listed blocks' rows, at their image positions.
+	float threshold = 0.0f;
 	if (st == ASTCENC_SUCCESS && radius != 0) {
-		// the averages of the listed blocks' rows, at their image positions; the staging pass must not filter its own image,
-		// whose box filter would reach across the seams between unrelated blocks
-		unsigned int y1 = (row_hi + 1) * bsd.dim_y;
-		st = alpha_prepass(ctx, d_pixels, data_type, dim_x, dim_y, swz, row_lo * bsd.dim_y, y1 < dim_y ? y1 : dim_y,
-		                   reinterpret_cast<float*>(ctx->d_list_alpha), stream);
+		st = alpha_prepass(ctx, src, row_lo, row_hi + 1, reinterpret_cast<float*>(ctx->d_list_alpha), stream, threshold);
 	}
 	GatherArgs g;
-	g.src = d_pixels;
+	g.src = src.data;
 	g.dst = ctx->d_list_image;
 	g.avg_src = radius != 0 ? reinterpret_cast<const float*>(ctx->d_list_alpha) : nullptr;
 	g.avg_dst = radius != 0 ? ctx->d_alpha : nullptr;
 	g.words = words;
-	g.dim_x = dim_x;
-	g.dim_y = dim_y;
-	g.dim_z = dim_z;
-	g.blocks_x = (unsigned int)block_count_axis(dim_x, bsd.dim_x);
-	g.blocks_y = (unsigned int)block_count_axis(dim_y, bsd.dim_y);
+	g.dim_x = src.dim_x;
+	g.dim_y = src.dim_y;
+	g.dim_z = src.dim_z;
+	g.blocks_x = src.blocks_x;
+	g.blocks_y = src.blocks_y;
 	g.bx = bsd.dim_x;
 	g.by = bsd.dim_y;
 	g.bz = bsd.dim_z;
@@ -2057,9 +1934,11 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const void* d_pixels, i
 		const unsigned int warps = ASTC_GATHER_THREADS / 32;
 		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
 		ctx->launches++;
-		ctx->pass_alpha_staged = radius != 0;
-		st = launch_slab_locked(ctx, ctx->d_list_image, data_type, m * bsd.dim_x, bsd.dim_y, swz, 0, 1, ctx->d_list_out, stream, nullptr);
-		ctx->pass_alpha_staged = false;
+		// (the staging volume is one layer deep)
+		DevImage staged = pass_image(ctx, ctx->d_list_image, src.data_type, m * bsd.dim_x, bsd.dim_y, volume ? bsd.dim_z : 1, swizzle);
+		staged.alpha_avg = radius != 0 ? ctx->d_alpha : nullptr;
+		staged.alpha_threshold = threshold;
+		st = launch_slab_locked(ctx, staged, 0, 1, ctx->d_list_out, stream, nullptr);
 		if (st == ASTCENC_SUCCESS) {
 			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->d_list_out, d_idx, m, d_payload, aligned16);
 			ctx->launches++;
@@ -2119,9 +1998,8 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	int swz[4] = {(int)swizzle->r, (int)swizzle->g, (int)swizzle->b, (int)swizzle->a};
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_blocks(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, swz, list, row_lo, row_hi, d_payload, s);
+	return launch_blocks(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, *swizzle), *swizzle, list, row_lo, row_hi, d_payload, s);
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

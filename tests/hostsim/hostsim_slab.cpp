@@ -47,3 +47,14 @@ extern "C" void hostsim_slab_slices(unsigned int r0, unsigned int r1, unsigned i
 extern "C" void hostsim_slab_part(unsigned int r0, unsigned int r1, unsigned int blocks_y, unsigned int s, unsigned int* out) {
 	slab_part(r0, r1, blocks_y, s, out[0], out[1]);
 }
+
+extern "C" void hostsim_image_rows(unsigned int r0, unsigned int r1, unsigned int block_y, unsigned int dim_y, unsigned int* out) {
+	size_t y0, y1;
+	image_rows(r0, r1, block_y, dim_y, y0, y1);
+	out[0] = (unsigned int)y0;
+	out[1] = (unsigned int)y1;
+}
+
+extern "C" void hostsim_band_of(unsigned int rows, int bands, int k, unsigned int* out) {
+	out[2] = band_of(rows, bands, k, out[0], out[1]) ? 1 : 0;
+}

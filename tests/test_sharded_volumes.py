@@ -57,6 +57,8 @@ def slab_sim():
     lib.hostsim_slab_of.argtypes = [C.c_uint, C.c_int, C.c_int, u4]
     lib.hostsim_slab_slices.argtypes = [C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, u4]
     lib.hostsim_slab_part.argtypes = [C.c_uint, C.c_uint, C.c_uint, C.c_uint, u4]
+    lib.hostsim_image_rows.argtypes = [C.c_uint, C.c_uint, C.c_uint, C.c_uint, u4]
+    lib.hostsim_band_of.argtypes = [C.c_uint, C.c_int, C.c_int, u4]
     _SIM.append(lib)
     return lib
 

@@ -26,12 +26,12 @@
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
 #include "astc_host_slab.h"
+#include "astc_host_launch.h"
 
 // ---------------------------------------------------------------------------------------------
 // The kernel: persistent warps, one block per warp at a time, dynamic ticket scheduling (the GPU analogue
 // of the reference's ParallelManager::get_task_assignment ticket counter).
 // ---------------------------------------------------------------------------------------------
-#define ASTC_CTA_THREADS_MAX 512
 
 // Shared window: [0, ASTC_SMEM_HDR) launch constants, then one arena per warp.
 static __device__ __forceinline__ void stage_launch_constants(const DevBsd& bsd, const DevConfig& cfg, const DevImage& img) {
@@ -59,7 +59,6 @@ static __device__ __forceinline__ void stage_launch_constants(const DevBsd& bsd,
 // Refinement reads the packed decimation tables (infill in every score / refit / realignment) and, from single lanes in
 // long dependent chains, the colour quantisation tables; its arenas leave ~50 KB of the shared window free at 6x6, so
 // both are copied behind the header once per CTA and read from there (when they fit without costing a warp).
-#define ASTC_CQ_BYTES (17 * 512)
 static __device__ __forceinline__ void stage_tables(uint32_t stage_bytes, uint32_t at, bool with_colour) {
 	if (stage_bytes == 0) {
 		return;
@@ -119,10 +118,6 @@ static __device__ __forceinline__ bool wave_setup_queues_empty(const WaveArgs& a
 	return __syncthreads_or(any ? 1 : 0) == 0;
 }
 
-#define ASTC_SETUP_THREADS_MAX 640      /* 20 warps x <= 102 registers (registers are granted per 4 warps: 21 warps would be charged as 24 and cap the kernel at 80) */
-#ifndef ASTC_REFINE_THREADS_MAX
-#define ASTC_REFINE_THREADS_MAX 768      /* 24 warps x 80 registers; 28 warps x 72 registers: 71.6 vs 71.1 ms per pass (H100 80GB HBM3 at 400 W, 4K 6x6 -medium) */
-#endif
 #define ASTC_EMIT_THREADS 256
 
 // Two instantiations: S1 = true for the wave-0 launches of the LDR profiles (the first trial of every block, one partition and
@@ -351,119 +346,127 @@ struct DeviceGuard {
 	}
 };
 
-// Tuning / experiment knobs, read ONCE when the context is created (INTEGRATION.md lists them).
-struct Knobs {
-	size_t batch_blocks;         // ASTCENC_B200_BATCH_BLOCKS: blocks per batch of a slab (records are reused batch after batch)
-	unsigned int sync_mask;      // ASTCENC_B200_SYNC_MASK: stage barriers of the wave kernels
-	unsigned int sync_mask_tail; // ASTCENC_B200_SYNC_MASK_TAIL: the same for the waves after the first (default: the same mask)
-	int coherence_probe;         // ASTCENC_B200_COHERENCE_PROBE (single-kernel driver experiment)
-	int upload_bands;            // ASTCENC_B200_UPLOAD_BANDS: bands the host-pointer path cuts an image into (1 = one copy)
-	int stage_print;             // ASTCENC_B200_STAGE_PRINT
-	int pipes;                   // ASTCENC_B200_PIPES: independent sub-slab pipelines of one pass (1 = the plain wave loop)
-};
-#define ASTC_MAX_PIPES 8
-#define ASTC_MAX_BANDS 8
 #define ASTC_COUNTER_WORDS (2 * ASTC_Q_KINDS * ASTC_MAX_WAVES + ASTC_MAX_BANDS)
 
 struct DeviceTables {            // shared between a parent context and its children
-	std::atomic<int> refcount;
-	uint8_t* d_blob;
+	std::atomic<int> refcount{1};
+	uint8_t* d_blob = nullptr;
 	DevBsd bsd;                  // device pointers
 	DevBsd bsd_1p;               // the same tables, compact one-plane arena plan (wave 0 of the pipeline)
-	astc_host::BlockSizeTables* host_tables;
+	astc_host::BlockSizeTables* host_tables = nullptr;
 };
 
+// A device buffer grown on demand (never shrunk): `bytes` bytes at `ptr`.
+struct DevBuffer {
+	uint8_t* ptr = nullptr;
+	size_t bytes = 0;
+	template <typename T> T* as() const { return reinterpret_cast<T*>(ptr); }
+};
+
+static astcenc_error ensure_buffer(DevBuffer& b, size_t need) {
+	if (b.bytes < need) {
+		cudaFree(b.ptr);
+		b.ptr = nullptr;
+		b.bytes = 0;
+		CUDA_TRY(cudaMalloc(&b.ptr, need), return ASTCENC_ERR_OUT_OF_MEM);
+		b.bytes = need;
+	}
+	return ASTCENC_SUCCESS;
+}
+
+// "The first caller does the work, the others wait for its result" (the reference's ParallelManager): one per kind of call.
+struct CallerGate {
+	int state = 0;               // 0 idle, 1 running, 2 done
+	astcenc_error result = ASTCENC_SUCCESS;
+	void reset() {               // (under astcenc_context::mtx) ready for the next image, unless a call is running
+		if (state != 1) {
+			state = 0;
+		}
+	}
+};
+
+// Every member starts out null / idle, so that astcenc_context_free() can release a partially built context.
 struct astcenc_context {
 	astcenc_config config;
-	unsigned int thread_count;
-	int device;
-	DeviceTables* tables;
+	unsigned int thread_count = 0;
+	int device = -1;
+	DeviceTables* tables = nullptr;
 	DevConfig dcfg;
-	cudaStream_t stream;
-	cudaEvent_t ev0, ev1;
-	unsigned int* d_ticket;
-	int warps_per_cta;
-	int grid;
-	size_t smem_bytes;
-	int lockstep;                // single-kernel drivers: phase-aligned CTA (1) or independent warps (0)
-	int driver;                  // 0 = wave pipeline (default), 1 = single kernel
-	int warps_setup, warps_small;   // warps per CTA of the setup / refine+prepare kernels
-	int refine_ctas;                // CTAs per SM of the refine kernel (experiment: ASTCENC_B200_REFINE_CTAS)
-	int warps_setup_1p;             // set-up kernel on the compact one-plane plan (0 = plan not used)
-	size_t smem_setup, smem_setup_1p, smem_refine;
-	uint32_t setup_stage_bytes;
-	uint32_t refine_stage_bytes;   // tables staged behind the header of the refine kernel's shared window (0 = none)
-	int max_waves;
+	cudaStream_t stream = nullptr;
+	cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+	unsigned int* d_ticket = nullptr;
+	Knobs knobs;
+	KernelPlan plan;
 	// wave pipeline buffers, grown on demand
-	uint8_t* d_records;
-	size_t d_records_bytes;
-	uint32_t* d_queues;          // ASTC_Q_KINDS lists of one entry per block
-	size_t d_queues_bytes;
-	uint32_t* d_counters;        // count[ASTC_Q_KINDS][MAX_WAVES] head[ASTC_Q_KINDS][MAX_WAVES]
-	float* d_alpha;              // alpha-scale pre-pass: one average per texel
-	size_t d_alpha_bytes;
+	DevBuffer records;
+	DevBuffer queues;            // ASTC_Q_KINDS lists of one entry per block (uint32_t)
+	uint32_t* d_counters = nullptr;   // count[ASTC_Q_KINDS][MAX_WAVES] head[ASTC_Q_KINDS][MAX_WAVES]
+	DevBuffer alpha;             // alpha-scale pre-pass: one average per texel (float)
 	// optional per-stage timing (astcenc_b200_stage_timing): an event after every launch of the next call
-	int stage_timing;
+	int stage_timing = 0;
 	std::vector<cudaEvent_t> stage_events;
 	std::vector<int> stage_kinds;
-	// staging buffers for the host-pointer API, grown on demand
-	uint8_t* d_image;
-	size_t d_image_bytes;
-	uint8_t* d_out;
-	size_t d_out_bytes;
+	// staging buffers for the host-pointer API, grown on demand; image2 is the second image buffer of the batch API
+	// (double-buffered uploads)
+	DevBuffer image, image2, out;
 	// block lists (astcenc_b200_compress_device_blocks), grown on demand: the list, the staging image and payload of one chunk,
 	// the pre-pass averages of the source image
-	uint8_t* d_list;
-	size_t d_list_bytes;
-	uint8_t* d_list_image;
-	size_t d_list_image_bytes;
-	uint8_t* d_list_out;
-	size_t d_list_out_bytes;
-	uint8_t* d_list_alpha;
-	size_t d_list_alpha_bytes;
-	Knobs knobs;
+	DevBuffer list, list_image, list_out, list_alpha;
 	// The per-context scratch (records, queues, counters, alpha averages) serves ONE pipeline pass at a time: launch_mtx
 	// serialises the host side, scratch_done orders a pass on one stream behind the previous pass on another.
 	std::mutex launch_mtx;
-	cudaEvent_t scratch_done;
-	bool scratch_used;
+	cudaEvent_t scratch_done = nullptr;
+	bool scratch_used = false;
 	// host-pointer path: uploads run on copy_stream, band by band, under the set-up of the previous band
-	cudaStream_t copy_stream;
-	cudaEvent_t band_ready[ASTC_MAX_BANDS];
+	cudaStream_t copy_stream = nullptr;
+	cudaEvent_t band_ready[ASTC_MAX_BANDS] = {};
 	// sub-slab pipelines of one pass (launch_pipes): one stream each, joined to the caller's stream by events
-	cudaStream_t pipe_stream[ASTC_MAX_PIPES];
-	cudaEvent_t pipe_done[ASTC_MAX_PIPES];
-	cudaEvent_t pipe_start;
-	uint8_t* d_image2;           // second image buffer of the batch API (double-buffered uploads)
-	size_t d_image2_bytes;
+	cudaStream_t pipe_stream[ASTC_MAX_PIPES] = {};
+	cudaEvent_t pipe_done[ASTC_MAX_PIPES] = {};
+	cudaEvent_t pipe_start = nullptr;
 	// multi-GPU (astc_host_multi.inl): one process per GPU, NCCL for the payload gather
-	void* nccl_comm;
-	int rank, world;
-	cudaEvent_t ev_g0, ev_g1;
-	float last_gather_ms, last_compress_ms;
+	void* nccl_comm = nullptr;
+	int rank = 0, world = 1;
+	cudaEvent_t ev_g0 = nullptr, ev_g1 = nullptr;
+	float last_gather_ms = 0.0f, last_compress_ms = 0.0f;
 	// caller protocol
 	std::mutex mtx;
 	std::condition_variable cv;
-	int state;                   // 0 idle, 1 running, 2 done
-	astcenc_error result;
-	int dstate;                  // the same for decompression
-	astcenc_error dresult;
-	std::atomic<bool> cancel;
+	CallerGate compress_gate, decompress_gate;
+	std::atomic<bool> cancel{false};
 	// Progress and cancellation of astcenc_compress_image (astc_dev_lockstep.cuh, pass_cancelled): d_words = {cancel flag, done
 	// counter}; h_words (pinned) = {0, 1, counter read-back}: the flag is written by 4-byte DMAs from h_words[0] / [1] and the
 	// counter read by one into h_words[2], all on ctl_stream, which never waits for the pass. flag_mtx makes "set ctx->cancel,
 	// enqueue the matching flag write" one step, so that the device flag always ends on the value ctx->cancel holds.
-	uint32_t* d_words;
-	uint32_t* h_words;
-	cudaStream_t ctl_stream;
-	cudaEvent_t ctl_ready;          // after the last flag clear: a pass starts behind it
+	uint32_t* d_words = nullptr;
+	uint32_t* h_words = nullptr;
+	cudaStream_t ctl_stream = nullptr;
+	cudaEvent_t ctl_ready = nullptr;          // after the last flag clear: a pass starts behind it
 	std::mutex flag_mtx;
-	bool flag_raised;               // a raise was enqueued since the last clear (under flag_mtx)
+	bool flag_raised = false;                 // a raise was enqueued since the last clear (under flag_mtx)
 	// stats
-	unsigned long long launches;
-	float last_kernel_ms;
-	size_t last_h2d, last_d2h;
+	unsigned long long launches = 0;
+	float last_kernel_ms = 0.0f;
+	size_t last_h2d = 0, last_d2h = 0;
 };
+
+// Runs `work` for the first caller through `gate`; every other caller waits for that call and returns its result.
+template <typename F>
+static astcenc_error run_once(astcenc_context* ctx, CallerGate& gate, F work) {
+	std::unique_lock<std::mutex> lk(ctx->mtx);
+	if (gate.state == 0) {
+		gate.state = 1;
+		lk.unlock();
+		astcenc_error r = work();
+		lk.lock();
+		gate.result = r;
+		gate.state = 2;
+		ctx->cv.notify_all();
+		return r;
+	}
+	ctx->cv.wait(lk, [&gate] { return gate.state == 2; });
+	return gate.result;
+}
 
 static std::mutex g_const_mtx;
 static DevConstTables* g_d_consts[64];
@@ -496,19 +499,6 @@ static void release_tables(DeviceTables* t) {
 	}
 }
 
-// device buffers grown on demand (never shrunk): `have` bytes at `buf`
-template <typename T>
-static astcenc_error ensure_buffer(T*& buf, size_t& have, size_t need) {
-	if (have < need) {
-		cudaFree(buf);
-		buf = nullptr;
-		have = 0;
-		CUDA_TRY(cudaMalloc(&buf, need), return ASTCENC_ERR_OUT_OF_MEM);
-		have = need;
-	}
-	return ASTCENC_SUCCESS;
-}
-
 extern "C" {
 
 astcenc_error astcenc_config_init(astcenc_profile profile, unsigned int block_x, unsigned int block_y, unsigned int block_z, float quality,
@@ -538,89 +528,9 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	if (!ctx) {
 		return ASTCENC_ERR_OUT_OF_MEM;
 	}
-	// every resource starts out null, so that astcenc_context_free() can release a partially built context
 	ctx->config = *configp;
 	ctx->thread_count = thread_count;
-	ctx->device = -1;
-	ctx->tables = nullptr;
-	ctx->stream = nullptr;
-	ctx->copy_stream = nullptr;
-	ctx->ev0 = ctx->ev1 = nullptr;
-	ctx->scratch_done = nullptr;
-	ctx->scratch_used = false;
-	for (int i = 0; i < ASTC_MAX_BANDS; i++) {
-		ctx->band_ready[i] = nullptr;
-	}
-	for (int i = 0; i < ASTC_MAX_PIPES; i++) {
-		ctx->pipe_stream[i] = nullptr;
-		ctx->pipe_done[i] = nullptr;
-	}
-	ctx->pipe_start = nullptr;
-	ctx->d_ticket = nullptr;
-	ctx->d_records = nullptr;
-	ctx->d_records_bytes = 0;
-	ctx->d_queues = nullptr;
-	ctx->d_queues_bytes = 0;
-	ctx->d_counters = nullptr;
-	ctx->d_alpha = nullptr;
-	ctx->d_alpha_bytes = 0;
-	ctx->stage_timing = 0;
-	ctx->d_image = nullptr;
-	ctx->d_image2 = nullptr;
-	ctx->d_out = nullptr;
-	ctx->d_image_bytes = ctx->d_image2_bytes = ctx->d_out_bytes = 0;
-	ctx->d_list = ctx->d_list_image = ctx->d_list_out = ctx->d_list_alpha = nullptr;
-	ctx->d_list_bytes = ctx->d_list_image_bytes = ctx->d_list_out_bytes = ctx->d_list_alpha_bytes = 0;
-	ctx->nccl_comm = nullptr;
-	ctx->rank = 0;
-	ctx->world = 1;
-	ctx->ev_g0 = ctx->ev_g1 = nullptr;
-	ctx->last_gather_ms = ctx->last_compress_ms = 0.0f;
-	ctx->state = 0;
-	ctx->result = ASTCENC_SUCCESS;
-	ctx->dstate = 0;
-	ctx->dresult = ASTCENC_SUCCESS;
-	ctx->cancel = false;
-	ctx->d_words = nullptr;
-	ctx->h_words = nullptr;
-	ctx->ctl_stream = nullptr;
-	ctx->ctl_ready = nullptr;
-	ctx->flag_raised = false;
-	ctx->launches = 0;
-	ctx->last_kernel_ms = 0.0f;
-	ctx->last_h2d = ctx->last_d2h = 0;
-	ctx->warps_per_cta = ctx->grid = 0;
-	ctx->warps_setup_1p = 0;
-	ctx->max_waves = 0;
-	// environment knobs: read here, once
-	ctx->knobs.batch_blocks = (size_t)1 << 20;
-	if (const char* e = getenv("ASTCENC_B200_BATCH_BLOCKS")) {
-		long v = atol(e);
-		if (v > 0) ctx->knobs.batch_blocks = (size_t)v;
-	}
-	// stage barriers of the wave kernels (bit i = i-th barrier of the kernel loop): the one in front of the endpoint-format stage
-	// of the set-up kernel (bit 3) is on. With the queues sorted by cost the mask hardly matters: no barrier at all measures
-	// 71.35 against 71.57 ms per pass (H100 80GB HBM3 at 400 W, 4K 6x6 -medium), inside the run-to-run spread of 71.1-71.7 ms
-	ctx->knobs.sync_mask = 8;
-	if (const char* e = getenv("ASTCENC_B200_SYNC_MASK")) {
-		ctx->knobs.sync_mask = (unsigned int)strtoul(e, nullptr, 0);
-	}
-	ctx->knobs.sync_mask_tail = ctx->knobs.sync_mask;
-	if (const char* e = getenv("ASTCENC_B200_SYNC_MASK_TAIL")) {
-		ctx->knobs.sync_mask_tail = (unsigned int)strtoul(e, nullptr, 0);
-	}
-	ctx->knobs.coherence_probe = getenv("ASTCENC_B200_COHERENCE_PROBE") ? 1 : 0;
-	ctx->knobs.stage_print = getenv("ASTCENC_B200_STAGE_PRINT") ? 1 : 0;
-	ctx->knobs.pipes = 1;      // 1 / 2 / 4 pipelines = 71.6 / 71.9 / 73.7 ms per pass (H100 80GB HBM3 at 400 W, 4K 6x6 -medium): the idle warps are inside the CTAs, not between kernels
-	if (const char* e = getenv("ASTCENC_B200_PIPES")) {
-		int v = atoi(e);
-		if (v >= 1 && v <= ASTC_MAX_PIPES) ctx->knobs.pipes = v;
-	}
-	ctx->knobs.upload_bands = 4;
-	if (const char* e = getenv("ASTCENC_B200_UPLOAD_BANDS")) {
-		int v = atoi(e);
-		if (v >= 1 && v <= ASTC_MAX_BANDS) ctx->knobs.upload_bands = v;
-	}
+	ctx->knobs = read_knobs();      // environment knobs: read here, once
 	// one exit for every failure: whatever was built so far is released by astcenc_context_free()
 	#define ALLOC_FAIL(code) do { astcenc_context_free(ctx); return (code); } while (0)
 	status = astc_host::validate_config(ctx->config);
@@ -641,9 +551,6 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 		ctx->tables->refcount.fetch_add(1);
 	} else {
 		DeviceTables* t = new DeviceTables;
-		t->refcount = 1;
-		t->d_blob = nullptr;
-		t->host_tables = nullptr;
 		ctx->tables = t;
 		astc_host::PackedTables pk;
 		t->host_tables = astc_host::build_packed_tables(cfg, pk);
@@ -658,111 +565,19 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 	if (!(cfg.flags & ASTCENC_FLG_DECOMPRESS_ONLY)) {
 		cudaDeviceProp prop;
 		CUDA_TRY(cudaGetDeviceProperties(&prop, device), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-		// The per-warp arena lives in shared memory only: one CTA per SM with as many warps as fit (at most 16).
-		size_t smem_limit = prop.sharedMemPerBlockOptin;
-		size_t arena = ctx->tables->bsd.arena_bytes;
-		int warps = (int)((smem_limit - ASTC_SMEM_HDR - ASTC_SMEM_SINCOS_BYTES) / (arena + ASTC_REFINE_STATE_BYTES));
-		if (warps > ASTC_CTA_THREADS_MAX / 32) warps = ASTC_CTA_THREADS_MAX / 32;
-		if (warps < 1) {
-			// block sizes / presets whose working set exceeds one SM's shared memory are not supported by this build
-			ALLOC_FAIL(ASTCENC_ERR_NOT_IMPLEMENTED);
+		status = plan_kernels(ctx->tables->bsd, ctx->tables->bsd_1p, cfg, prop.sharedMemPerBlockOptin, prop.multiProcessorCount, ctx->knobs, ctx->plan);
+		if (status != ASTCENC_SUCCESS) {
+			ALLOC_FAIL(status);
 		}
-		ctx->warps_per_cta = warps;
-		ctx->grid = prop.multiProcessorCount;
-		// tuning overrides (experiments): warps per CTA and CTAs per SM
-		if (const char* e = getenv("ASTCENC_B200_WARPS")) {
-			int v = atoi(e);
-			if (v >= 1 && v <= warps) ctx->warps_per_cta = v;
-		}
-		if (const char* e = getenv("ASTCENC_B200_CTAS_PER_SM")) {
-			int v = atoi(e);
-			if (v >= 1 && v <= 8) ctx->grid = prop.multiProcessorCount * v;
-		}
-		ctx->lockstep = 1;
-		ctx->driver = 0;
-		if (const char* e = getenv("ASTCENC_B200_DRIVER")) {
-			if (!strcmp(e, "lockstep")) { ctx->driver = 1; ctx->lockstep = 1; }
-			else if (!strcmp(e, "warp")) { ctx->driver = 1; ctx->lockstep = 0; }
-		}
-		ctx->smem_bytes = ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + (arena + ASTC_REFINE_STATE_BYTES) * ctx->warps_per_cta;
-		CUDA_TRY(cudaFuncSetAttribute(astc_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-		// wave pipeline: the setup kernel needs the full arena, refinement / preparation only up to the union scratch
-		{
-			size_t arena_small = ctx->tables->bsd.arena_bytes_small;
-			int ws = (int)((smem_limit - ASTC_SMEM_HDR - ASTC_SMEM_SINCOS_BYTES) / arena);
-			if (ws > ASTC_SETUP_THREADS_MAX / 32) ws = ASTC_SETUP_THREADS_MAX / 32;
-			ctx->refine_ctas = 1;
-			if (const char* e = getenv("ASTCENC_B200_REFINE_CTAS")) {
-				int v = atoi(e);
-				if (v >= 1 && v <= 4) ctx->refine_ctas = v;
-			}
-			// (per CTA: 1 KB of shared memory is reserved by the system)
-			int wr = (int)((smem_limit / ctx->refine_ctas - (ctx->refine_ctas > 1 ? 1024 : 0) - ASTC_SMEM_HDR) / (arena_small + ASTC_REFINE_STATE_BYTES));
-			if (wr > ASTC_REFINE_THREADS_MAX / 32) wr = ASTC_REFINE_THREADS_MAX / 32;
-			// Staging the decimation (+ colour quantisation) tables in the refine kernel's spare shared memory is possible
-			// without losing a warp at 6x6, but gains nothing (71.63 vs 71.57 ms per pass, H100 80GB HBM3 at 400 W, 4K 6x6 -medium: L1 already serves these loads): opt-in.
-			size_t stage = (((size_t)ctx->tables->bsd.dec_stage_bytes + 15) & ~(size_t)15) + ASTC_CQ_BYTES;
-			ctx->refine_stage_bytes = 0;
-			if (getenv("ASTCENC_B200_STAGE_REFINE") && smem_limit > ASTC_SMEM_HDR + stage && (int)((smem_limit - ASTC_SMEM_HDR - stage) / (arena_small + ASTC_REFINE_STATE_BYTES)) >= wr) {
-				ctx->refine_stage_bytes = (uint32_t)stage;
-			}
-			if (const char* e = getenv("ASTCENC_B200_WARPS_SETUP")) {
-				int v = atoi(e);
-				if (v >= 1 && v <= ws) ws = v;
-			}
-			if (const char* e = getenv("ASTCENC_B200_WARPS_REFINE")) {
-				int v = atoi(e);
-				if (v >= 1 && v <= wr) wr = v;
-			}
-			ctx->warps_setup = ws;
-			ctx->warps_small = wr;
-			// The set-up kernel walks the decimation tables of every grid for every block (decimated ideal weights, per-mode
-			// scoring): with them in shared memory it is faster even with one warp less (6x6 medium: 21 KB of tables, 15
-			// instead of 16 warps; 71.6 against 73.3 ms per pass unstaged, H100 80GB HBM3 at 400 W, 4K 6x6 -medium). Done when it costs at most one warp (ASTCENC_B200_STAGE_SETUP=0/1 forces).
-			ctx->setup_stage_bytes = 0;
-			{
-				size_t st = ((size_t)ctx->tables->bsd.dec_stage_bytes + 15) & ~(size_t)15;
-				int ws2 = smem_limit > ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + st ? (int)((smem_limit - ASTC_SMEM_HDR - ASTC_SMEM_SINCOS_BYTES - st) / arena) : 0;
-				bool want = ws2 >= 1 && ws2 >= ws - 1;
-				if (const char* e = getenv("ASTCENC_B200_STAGE_SETUP")) {
-					want = atoi(e) != 0 && ws2 >= 1;
-				}
-				if (want) {
-					if (ws2 < ws) ws = ws2;
-					ctx->warps_setup = ws;
-					ctx->setup_stage_bytes = (uint32_t)st;
-				}
-			}
-			ctx->smem_setup = ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + ctx->setup_stage_bytes + arena * ws;
-			// wave 0 (every block's first trial has one weight plane) runs on the compact plan: more arenas per SM
-			{
-				size_t arena1 = ctx->tables->bsd_1p.arena_bytes;
-				int w1 = (int)((smem_limit - ASTC_SMEM_HDR - ASTC_SMEM_SINCOS_BYTES - ctx->setup_stage_bytes) / arena1);
-				if (w1 > ASTC_SETUP_THREADS_MAX / 32) w1 = ASTC_SETUP_THREADS_MAX / 32;
-				if (const char* e = getenv("ASTCENC_B200_WARPS_SETUP_1P")) {
-					int v = atoi(e);
-					if (v >= 0 && v < w1) w1 = v;
-				}
-				ctx->warps_setup_1p = w1 > ws ? w1 : 0;      // only when it buys warps
-				ctx->smem_setup_1p = ASTC_SMEM_HDR + ASTC_SMEM_SINCOS_BYTES + ctx->setup_stage_bytes + arena1 * (size_t)w1;
-			}
-			ctx->smem_refine = ASTC_SMEM_HDR + ctx->refine_stage_bytes + arena_small * wr + (size_t)ASTC_REFINE_STATE_BYTES * wr;
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-			CUDA_TRY(cudaFuncSetAttribute(astc_wave_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-			// a block runs at most this many trials (compress_block: mode-0 + full 1-plane, 4 two-plane, then the partition candidates)
-			int waves = 2 + 4;
-			const unsigned int cl[3] = {cfg.tune_2partitioning_candidate_limit, cfg.tune_3partitioning_candidate_limit, cfg.tune_4partitioning_candidate_limit};
-			for (unsigned int pc = 2; pc <= cfg.tune_partition_count_limit && pc <= 4; pc++) {
-				waves += (int)cl[pc - 2];
-			}
-			if (waves > ASTC_MAX_WAVES - 1) waves = ASTC_MAX_WAVES - 1;
-			ctx->max_waves = waves;
-			// count[kinds][waves], head[kinds][waves], then one image ticket per upload band
-			CUDA_TRY(cudaMalloc(&ctx->d_counters, sizeof(uint32_t) * ASTC_COUNTER_WORDS * ASTC_MAX_PIPES), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
-		}
+		const int smem_limit = (int)prop.sharedMemPerBlockOptin;
+		CUDA_TRY(cudaFuncSetAttribute(astc_compress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaFuncSetAttribute(astc_wave_setup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaFuncSetAttribute(astc_wave_refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		CUDA_TRY(cudaFuncSetAttribute(astc_wave_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_limit), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
+		// count[kinds][waves], head[kinds][waves], then one image ticket per upload band
+		CUDA_TRY(cudaMalloc(&ctx->d_counters, sizeof(uint32_t) * ASTC_COUNTER_WORDS * ASTC_MAX_PIPES), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
 		CUDA_TRY(cudaMalloc(&ctx->d_ticket, sizeof(unsigned int)), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
 		// progress and cancellation: the device words start cleared
 		CUDA_TRY(cudaMalloc(&ctx->d_words, 2 * sizeof(uint32_t)), ALLOC_FAIL(ASTCENC_ERR_OUT_OF_MEM));
@@ -810,20 +625,14 @@ void astcenc_context_free(astcenc_context* ctx) {
 	if (ctx->copy_stream) cudaStreamSynchronize(ctx->copy_stream);
 	comm_destroy(ctx);
 	cudaFree(ctx->d_ticket);
-	cudaFree(ctx->d_records);
-	cudaFree(ctx->d_queues);
 	cudaFree(ctx->d_counters);
-	cudaFree(ctx->d_alpha);
+	for (DevBuffer* b : {&ctx->records, &ctx->queues, &ctx->alpha, &ctx->image, &ctx->image2, &ctx->out, &ctx->list, &ctx->list_image, &ctx->list_out,
+	                     &ctx->list_alpha}) {
+		cudaFree(b->ptr);
+	}
 	for (cudaEvent_t e : ctx->stage_events) {
 		cudaEventDestroy(e);
 	}
-	cudaFree(ctx->d_image);
-	cudaFree(ctx->d_image2);
-	cudaFree(ctx->d_out);
-	cudaFree(ctx->d_list);
-	cudaFree(ctx->d_list_image);
-	cudaFree(ctx->d_list_out);
-	cudaFree(ctx->d_list_alpha);
 	if (ctx->ev0) cudaEventDestroy(ctx->ev0);
 	if (ctx->ev1) cudaEventDestroy(ctx->ev1);
 	if (ctx->ev_g0) cudaEventDestroy(ctx->ev_g0);
@@ -877,12 +686,69 @@ static size_t block_count_axis(size_t dim, size_t blk) {
 	return n;
 }
 
+// Geometry of one image in combined block rows (astc_host_slab.h): `layers` layers (3D block sizes) or slices of blocks_y rows.
+// A 3D block size takes the volume in one pass; a 2D one takes an array one slice per pass.
+struct SlabGeometry {
+	size_t blocks_x, blocks_y, layers;
+	size_t blocks;               // blocks_x * blocks_y * layers
+	bool overflow;               // the block count does not fit a size_t
+	size_t texel_bytes;          // bytes per texel of the image's data type
+	size_t slice_bytes;          // bytes of one image slice
+	size_t row_out;              // payload bytes of one combined row
+	unsigned int dim_z;
+	bool volume;
+	unsigned int rows() const { return (unsigned int)(blocks_y * layers); }
+	size_t out_bytes() const { return row_out * blocks_y * layers; }
+	unsigned int passes() const { return volume ? 1 : dim_z; }
+	unsigned int pass_slices() const { return volume ? dim_z : 1; }      // image slices one pass reads
+	unsigned int pass_rows() const { return volume ? rows() : (unsigned int)blocks_y; }
+	size_t pass_out_bytes() const { return row_out * pass_rows(); }
+	bool payload_overflow() const { return overflow || blocks > SIZE_MAX / 16; }      // block count or payload bytes
+};
+
+static SlabGeometry slab_geometry(const astcenc_context* ctx, unsigned int dim_x, unsigned int dim_y, unsigned int dim_z, int data_type) {
+	const DevBsd& bsd = ctx->tables->bsd;
+	SlabGeometry g;
+	g.volume = bsd.dim_z > 1;
+	g.dim_z = dim_z;
+	g.blocks_x = block_count_axis(dim_x, bsd.dim_x);
+	g.blocks_y = block_count_axis(dim_y, bsd.dim_y);
+	g.layers = g.volume ? block_count_axis(dim_z, bsd.dim_z) : dim_z;
+	g.overflow = false;
+	g.blocks = mul_safe(mul_safe(g.blocks_x, g.blocks_y, g.overflow), g.layers, g.overflow);
+	g.row_out = g.blocks_x * 16;
+	g.texel_bytes = data_type == ASTCENC_TYPE_U8 ? 4 : data_type == ASTCENC_TYPE_F16 ? 8 : 16;
+	g.slice_bytes = (size_t)dim_x * dim_y * g.texel_bytes;
+	return g;
+}
+
+// ---- argument checks: every entry point calls the ones it makes, in its own order (astcenc_compress_image in the reference's) ----
+static astcenc_error check_compress_context(const astcenc_context* ctx) {
+	return (ctx->config.flags & ASTCENC_FLG_DECOMPRESS_ONLY) ? ASTCENC_ERR_BAD_CONTEXT : ASTCENC_SUCCESS;
+}
+
+// texel count non-zero and free of overflow
+static astcenc_error check_texel_count(unsigned int dim_x, unsigned int dim_y, unsigned int dim_z) {
+	bool overflow = false;
+	size_t texels = mul_safe(mul_safe(dim_x, dim_y, overflow), dim_z, overflow);
+	return overflow || texels == 0 ? ASTCENC_ERR_BAD_PARAM : ASTCENC_SUCCESS;
+}
+
+static astcenc_error check_data_type(astcenc_type data_type) {
+	return (int)data_type < 0 || (int)data_type > 2 ? ASTCENC_ERR_BAD_PARAM : ASTCENC_SUCCESS;
+}
+
+// the alpha-scale pre-pass is built for 2D images; arrays would average across slices (compute_variance.cpp have_z)
+static astcenc_error check_alpha_scale(const astcenc_context* ctx, unsigned int dim_z) {
+	return ctx->config.a_scale_radius != 0 && dim_z != 1 && ctx->config.block_z <= 1 ? ASTCENC_ERR_NOT_IMPLEMENTED : ASTCENC_SUCCESS;
+}
+
 // The scratch of a pass, grown on demand: records and queues for `blocks` blocks of the wave pipeline, `alpha` averages of the
 // alpha-scale pre-pass.
 static astcenc_error ensure_scratch(astcenc_context* ctx, size_t blocks, size_t alpha) {
-	astcenc_error st = ensure_buffer(ctx->d_queues, ctx->d_queues_bytes, sizeof(uint32_t) * ASTC_Q_KINDS * blocks);
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_records, ctx->d_records_bytes, blocks * (size_t)ctx->tables->bsd.record_bytes);
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_alpha, ctx->d_alpha_bytes, alpha * sizeof(float));
+	astcenc_error st = ensure_buffer(ctx->queues, sizeof(uint32_t) * ASTC_Q_KINDS * blocks);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->records, blocks * (size_t)ctx->tables->bsd.record_bytes);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->alpha, alpha * sizeof(float));
 	return st;
 }
 
@@ -972,9 +838,9 @@ static void stage_mark(astcenc_context* ctx, int kind, cudaStream_t stream) {
 static WaveArgs wave_args(const astcenc_context* ctx, uint32_t* counters, size_t first, unsigned int blocks, unsigned int blocks_x) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	WaveArgs a;
-	a.records = ctx->d_records + first * (size_t)bsd.record_bytes;
-	a.queues = ctx->d_queues + first;
-	a.queue_stride = ctx->d_queues_bytes / (sizeof(uint32_t) * ASTC_Q_KINDS);
+	a.records = ctx->records.ptr + first * (size_t)bsd.record_bytes;
+	a.queues = ctx->queues.as<uint32_t>() + first;
+	a.queue_stride = ctx->queues.bytes / (sizeof(uint32_t) * ASTC_Q_KINDS);
 	a.count = counters;
 	a.head = counters + ASTC_Q_KINDS * ASTC_MAX_WAVES;
 	a.total = blocks;
@@ -986,9 +852,9 @@ static WaveArgs wave_args(const astcenc_context* ctx, uint32_t* counters, size_t
 	a.cls_hi = ASTC_Q_CLASSES;
 	a.wave = 0;
 	a.sync_mask = ctx->knobs.sync_mask;
-	a.stage_bytes_setup = ctx->setup_stage_bytes;
-	a.refine_state_off = (uint32_t)(ASTC_SMEM_HDR + ctx->refine_stage_bytes + (size_t)bsd.arena_bytes_small * ctx->warps_small);
-	a.stage_bytes = ctx->refine_stage_bytes;
+	a.stage_bytes_setup = ctx->plan.setup_stage_bytes;
+	a.refine_state_off = (uint32_t)(ASTC_SMEM_HDR + ctx->plan.refine_stage_bytes + (size_t)bsd.arena_bytes_small * ctx->plan.warps_small);
+	a.stage_bytes = ctx->plan.refine_stage_bytes;
 	return a;
 }
 
@@ -998,12 +864,13 @@ static WaveArgs wave_args(const astcenc_context* ctx, uint32_t* counters, size_t
 // on the compact plan with more warps per SM.
 static astcenc_error enqueue_setup(astcenc_context* ctx, const DevImage& img, WaveArgs a, cudaStream_t stream, const UploadPlan* up) {
 	const SetupKernel kernel = setup_kernel(ctx->dcfg, a.wave);
-	const bool compact = ctx->warps_setup_1p != 0;
+	const KernelPlan& p = ctx->plan;
+	const bool compact = p.warps_setup_1p != 0;
 	auto launch = [&](bool on_compact) {
 		if (on_compact) {
-			kernel<<<ctx->grid, ctx->warps_setup_1p * 32, ctx->smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
+			kernel<<<p.grid, p.warps_setup_1p * 32, p.smem_setup_1p, stream>>>(ctx->tables->bsd_1p, ctx->dcfg, img, a);
 		} else {
-			kernel<<<ctx->grid, ctx->warps_setup * 32, ctx->smem_setup, stream>>>(ctx->tables->bsd, ctx->dcfg, img, a);
+			kernel<<<p.grid, p.warps_setup * 32, p.smem_setup, stream>>>(ctx->tables->bsd, ctx->dcfg, img, a);
 		}
 		ctx->launches++;
 	};
@@ -1042,17 +909,17 @@ static astcenc_error enqueue_setup(astcenc_context* ctx, const DevImage& img, Wa
 // Refinement and preparation of wave a.wave of one pipeline.
 static void enqueue_refine_prepare(astcenc_context* ctx, const DevImage& img, const WaveArgs& a, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
-	const int grid = ctx->grid;
+	const KernelPlan& p = ctx->plan;
 	if (refine_l1_step(ctx->dcfg)) {
-		astc_wave_refine_kernel<true><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+		astc_wave_refine_kernel<true><<<p.grid * p.refine_ctas, p.warps_small * 32, p.smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
 	} else {
-		astc_wave_refine_kernel<false><<<grid * ctx->refine_ctas, ctx->warps_small * 32, ctx->smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
+		astc_wave_refine_kernel<false><<<p.grid * p.refine_ctas, p.warps_small * 32, p.smem_refine, stream>>>(bsd, ctx->dcfg, img, a);
 	}
 	ctx->launches++;
 	stage_mark(ctx, 1, stream);
 	// (statistics / partition search gain nothing from phase alignment: two half-size CTAs per SM wait less)
-	const int wp = ctx->warps_small >= 2 ? ctx->warps_small / 2 : 1;
-	astc_wave_prepare_kernel<<<grid * 2, wp * 32, ASTC_SMEM_HDR + (size_t)bsd.arena_bytes_small * wp, stream>>>(bsd, ctx->dcfg, img, a);
+	const int wp = p.warps_small >= 2 ? p.warps_small / 2 : 1;
+	astc_wave_prepare_kernel<<<p.grid * 2, wp * 32, ASTC_SMEM_HDR + (size_t)bsd.arena_bytes_small * wp, stream>>>(bsd, ctx->dcfg, img, a);
 	ctx->launches++;
 	stage_mark(ctx, 2, stream);
 }
@@ -1060,7 +927,7 @@ static void enqueue_refine_prepare(astcenc_context* ctx, const DevImage& img, co
 // The emit launch of one pipeline: the chosen encoding of every block into the payload.
 static void enqueue_emit(astcenc_context* ctx, const DevImage& img, WaveArgs a, cudaStream_t stream) {
 	a.wave = 0;
-	astc_wave_emit_kernel<<<ctx->grid * 4, ASTC_EMIT_THREADS, ASTC_SMEM_HDR + (ASTC_EMIT_THREADS / 32) * 32 * EMIT_SLICE, stream>>>(ctx->tables->bsd, ctx->dcfg, img, a);
+	astc_wave_emit_kernel<<<ctx->plan.grid * 4, ASTC_EMIT_THREADS, ASTC_SMEM_HDR + (ASTC_EMIT_THREADS / 32) * 32 * EMIT_SLICE, stream>>>(ctx->tables->bsd, ctx->dcfg, img, a);
 	ctx->launches++;
 	stage_mark(ctx, 3, stream);
 }
@@ -1073,7 +940,7 @@ static astcenc_error launch_batch(astcenc_context* ctx, const DevImage& img, cud
 		ctx->stage_kinds.clear();
 	}
 	stage_mark(ctx, -1, stream);
-	for (int wave = 0; wave < ctx->max_waves; wave++) {
+	for (int wave = 0; wave < ctx->plan.max_waves; wave++) {
 		a.wave = wave;
 		a.sync_mask = wave == 0 ? ctx->knobs.sync_mask : ctx->knobs.sync_mask_tail;
 		astcenc_error st = enqueue_setup(ctx, img, a, stream, up);
@@ -1120,7 +987,7 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const DevImag
 			}
 		}
 	}
-	for (int wave = 0; wave < ctx->max_waves; wave++) {
+	for (int wave = 0; wave < ctx->plan.max_waves; wave++) {
 		for (int p = 0; p < pipes; p++) {
 			if (a[p].total == 0) {
 				continue;
@@ -1149,13 +1016,14 @@ static astcenc_error launch_pipes(astcenc_context* ctx, int pipes, const DevImag
 // One batch of a slab on a single-kernel driver (ASTCENC_B200_DRIVER=lockstep|warp).
 static astcenc_error launch_driver(astcenc_context* ctx, const DevImage& img, cudaStream_t stream) {
 	CUDA_TRY(cudaMemsetAsync(ctx->d_ticket, 0, sizeof(unsigned int), stream), return ASTCENC_ERR_BAD_CONTEXT);
-	int grid = ctx->grid;
+	const KernelPlan& p = ctx->plan;
+	int grid = p.grid;
 	size_t total = (size_t)img.blocks_x * img.block_rows;
-	size_t needed = (total + ctx->warps_per_cta - 1) / ctx->warps_per_cta;
+	size_t needed = (total + p.warps_per_cta - 1) / p.warps_per_cta;
 	if ((size_t)grid > needed) {
 		grid = (int)(needed ? needed : 1);
 	}
-	astc_compress_kernel<<<grid, ctx->warps_per_cta * 32, ctx->smem_bytes, stream>>>(ctx->tables->bsd, ctx->dcfg, img, ctx->d_ticket, ctx->knobs.coherence_probe, ctx->lockstep);
+	astc_compress_kernel<<<grid, p.warps_per_cta * 32, p.smem_bytes, stream>>>(ctx->tables->bsd, ctx->dcfg, img, ctx->d_ticket, ctx->knobs.coherence_probe, p.lockstep);
 	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 	ctx->launches++;
 	return ASTCENC_SUCCESS;
@@ -1208,10 +1076,10 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const DevImage& sr
 	// big single-batch slabs run as independent sub-slab pipelines (launch_pipes); per-launch timing wants one stream
 	bool single_batch = (size_t)block_rows <= rows_per_batch;
 	int pipes = ctx->knobs.pipes;
-	bool use_pipes = pipes > 1 && ctx->driver == 0 && !ctx->stage_timing && single_batch && block_rows >= (unsigned int)pipes * 4 &&
+	bool use_pipes = pipes > 1 && ctx->plan.driver == 0 && !ctx->stage_timing && single_batch && block_rows >= (unsigned int)pipes * 4 &&
 	                 blocks_x * block_rows >= (size_t)pipes * 8192;
 	// banded uploads need the whole slab in one batch on the wave pipeline, and no pre-pass that reads the window first
-	bool banded = up != nullptr && radius == 0 && ctx->driver == 0 && single_batch && (use_pipes || (up->bands > 1 && block_rows >= (unsigned int)up->bands * 4));
+	bool banded = up != nullptr && radius == 0 && ctx->plan.driver == 0 && single_batch && (use_pipes || (up->bands > 1 && block_rows >= (unsigned int)up->bands * 4));
 	if (up != nullptr && ctx->scratch_used) {
 		// the upload streams on the copy stream; it must not overtake a pass that still reads the image buffer
 		CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
@@ -1230,14 +1098,14 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const DevImage& sr
 		// slab's rows (alpha_window); the averages stay at their image positions
 		astcenc_error st = ensure_scratch(ctx, 0, (size_t)img.dim_x * img.dim_y);
 		if (st == ASTCENC_SUCCESS) {
-			st = alpha_prepass(ctx, img, block_row0, block_row0 + block_rows, ctx->d_alpha, stream, img.alpha_threshold);
+			st = alpha_prepass(ctx, img, block_row0, block_row0 + block_rows, ctx->alpha.as<float>(), stream, img.alpha_threshold);
 		}
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
-		img.alpha_avg = ctx->d_alpha;
+		img.alpha_avg = ctx->alpha.as<float>();
 	}
-	if (ctx->driver == 0) {
+	if (ctx->plan.driver == 0) {
 		astcenc_error st = ensure_scratch(ctx, blocks_x * (single_batch ? block_rows : rows_per_batch), 0);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
@@ -1251,7 +1119,7 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const DevImage& sr
 		batch.block_row0 = block_row0 + done;
 		batch.block_rows = block_rows - done < rows_per_batch ? block_rows - done : (unsigned int)rows_per_batch;
 		batch.out = d_out + (size_t)done * blocks_x * 16;
-		astcenc_error st = ctx->driver == 0 ? launch_batch(ctx, batch, stream, up) : launch_driver(ctx, batch, stream);
+		astcenc_error st = ctx->plan.driver == 0 ? launch_batch(ctx, batch, stream, up) : launch_driver(ctx, batch, stream);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
@@ -1322,8 +1190,8 @@ static astcenc_error wait_pass(astcenc_context* ctx, cudaEvent_t end, PassProgre
 // the kernels of the earlier bands are running meanwhile).
 // A cancelled call (astcenc_compress_cancel) skips the remaining slices and copies no payload back: the caller's buffer keeps
 // its bytes, and the call still returns ASTCENC_SUCCESS (astcenc.h: the data is then undefined).
-static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_image& image, const astcenc_swizzle& swizzle, uint8_t* data_out) {
-	const DevBsd& bsd = ctx->tables->bsd;
+static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_image& image, const SlabGeometry& geo, const astcenc_swizzle& swizzle,
+                                        uint8_t* data_out) {
 	DeviceGuard guard(ctx->device);
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
@@ -1331,18 +1199,11 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 	// 3D block sizes (astcenc_entry.cpp:906-1043): one pass over the volume, whose slices go up into one contiguous buffer before
 	// it; its blocks come out in (z, y, x) order and its "block rows" count layer * blocks_y + row. 3D images with 2D blocks are
 	// an array of independent 2D slices (astcenc.h:94-100): one banded pass per slice. Progress runs over all passes.
-	const bool volume = bsd.dim_z > 1;
-	const unsigned int passes = volume ? 1 : image.dim_z;
-	const unsigned int pass_slices = volume ? image.dim_z : 1;
-	size_t bpt = image.data_type == ASTCENC_TYPE_U8 ? 4 : image.data_type == ASTCENC_TYPE_F16 ? 8 : 16;
-	size_t slice_bytes = (size_t)image.dim_x * image.dim_y * bpt;
-	size_t blocks_x = block_count_axis(image.dim_x, bsd.dim_x);
-	size_t blocks_y = block_count_axis(image.dim_y, bsd.dim_y);
-	size_t layers = volume ? block_count_axis(image.dim_z, bsd.dim_z) : 1;
-	size_t out_bytes = blocks_x * blocks_y * layers * 16;      // payload of one pass
-	astcenc_error st = ensure_buffer(ctx->d_image, ctx->d_image_bytes, slice_bytes * pass_slices);
+	const size_t slice_bytes = geo.slice_bytes;
+	const size_t out_bytes = geo.pass_out_bytes();
+	astcenc_error st = ensure_buffer(ctx->image, slice_bytes * geo.pass_slices());
 	if (st == ASTCENC_SUCCESS) {
-		st = ensure_buffer(ctx->d_out, ctx->d_out_bytes, out_bytes);
+		st = ensure_buffer(ctx->out, out_bytes);
 	}
 	if (st != ASTCENC_SUCCESS) {
 		return st;
@@ -1351,30 +1212,30 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 	ctx->last_kernel_ms = 0.0f;
 	float total_ms = 0.0f;
 	// the pass starts behind the last flag clear (astcenc_compress_reset), with its done counter at zero
-	DevImage src = pass_image(ctx, ctx->d_image, (int)image.data_type, image.dim_x, image.dim_y, pass_slices, swizzle);
+	DevImage src = pass_image(ctx, ctx->image.ptr, (int)image.data_type, image.dim_x, image.dim_y, geo.pass_slices(), swizzle);
 	src.cancel = ctx->d_words;
 	src.done = ctx->d_words + 1;
 	CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->ctl_ready, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	CUDA_TRY(cudaMemsetAsync(src.done, 0, sizeof(uint32_t), ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	PassProgress pp;
 	pp.callback = ctx->config.progress_callback;
-	pp.total = static_cast<float>(blocks_x * blocks_y * layers * passes);
+	pp.total = static_cast<float>(geo.blocks);
 	pp.min_diff = (4096.0f / pp.total) * 100.0f;
 	pp.min_diff = pp.min_diff > 1.0f ? pp.min_diff : 1.0f;
 	pp.last = 0.0f;
-	for (unsigned int z = 0; z < passes; z++) {
+	for (unsigned int z = 0; z < geo.passes(); z++) {
 		if (ctx->cancel.load()) {
 			return ASTCENC_SUCCESS;
 		}
-		UploadPlan up = {static_cast<const uint8_t*>(image.data[z]), ctx->d_image, (size_t)image.dim_x * bpt, ctx->knobs.upload_bands};
-		if (volume) {
-			st = upload_slices(ctx->d_image, image.data, 0, image.dim_z, slice_bytes, ctx->stream);
+		UploadPlan up = {static_cast<const uint8_t*>(image.data[z]), ctx->image.ptr, (size_t)image.dim_x * geo.texel_bytes, ctx->knobs.upload_bands};
+		if (geo.volume) {
+			st = upload_slices(ctx->image.ptr, image.data, 0, image.dim_z, slice_bytes, ctx->stream);
 			if (st != ASTCENC_SUCCESS) {
 				return st;
 			}
 		}
 		CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		st = launch_slab(ctx, src, 0, (unsigned int)(blocks_y * layers), ctx->d_out, ctx->stream, volume ? nullptr : &up);
+		st = launch_slab(ctx, src, 0, geo.pass_rows(), ctx->out.ptr, ctx->stream, geo.volume ? nullptr : &up);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
 		}
@@ -1386,12 +1247,12 @@ static astcenc_error compress_image_gpu(astcenc_context* ctx, const astcenc_imag
 		if (ctx->cancel.load()) {
 			return ASTCENC_SUCCESS;
 		}
-		CUDA_TRY(cudaMemcpyAsync(data_out + (size_t)z * out_bytes, ctx->d_out, out_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaMemcpyAsync(data_out + (size_t)z * out_bytes, ctx->out.ptr, out_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		float ms = 0.0f;
 		cudaEventElapsedTime(&ms, ctx->ev0, ctx->ev1);
 		total_ms += ms;
-		ctx->last_h2d += slice_bytes * pass_slices;
+		ctx->last_h2d += slice_bytes * geo.pass_slices();
 		ctx->last_d2h += out_bytes;
 	}
 	ctx->last_kernel_ms = total_ms;
@@ -1405,54 +1266,25 @@ astcenc_error astcenc_compress_reset(astcenc_context* ctx);
 
 astcenc_error astcenc_compress_image(astcenc_context* ctx, astcenc_image* imagep, const astcenc_swizzle* swizzle, uint8_t* data_out, size_t data_len,
                                      unsigned int thread_index) {
-	if (ctx->config.flags & ASTCENC_FLG_DECOMPRESS_ONLY) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	astcenc_error status = validate_compression_swizzle(*swizzle);
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS && thread_index >= ctx->thread_count) status = ASTCENC_ERR_BAD_PARAM;
 	if (status != ASTCENC_SUCCESS) {
 		return status;
 	}
-	if (thread_index >= ctx->thread_count) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
 	const astcenc_image& image = *imagep;
-	bool overflow = false;
-	size_t texel_count = mul_safe(mul_safe(image.dim_x, image.dim_y, overflow), image.dim_z, overflow);
-	if (overflow || texel_count == 0) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	size_t blocks_x = block_count_axis(image.dim_x, ctx->config.block_x);
-	size_t blocks_y = block_count_axis(image.dim_y, ctx->config.block_y);
-	size_t blocks_z = block_count_axis(image.dim_z, ctx->config.block_z);
-	overflow = false;
-	size_t block_count = mul_safe(mul_safe(blocks_x, blocks_y, overflow), blocks_z, overflow);
-	mul_safe(block_count, 16, overflow);
-	if (overflow || block_count == 0) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	if (data_len < block_count * 16) {
-		return ASTCENC_ERR_OUT_OF_MEM;
-	}
-	if (ctx->config.a_scale_radius != 0 && image.dim_z != 1 && ctx->config.block_z <= 1) {
-		// the alpha-scale pre-pass is built for 2D images; volumes would average across slices (compute_variance.cpp have_z)
-		return ASTCENC_ERR_NOT_IMPLEMENTED;
+	const SlabGeometry geo = slab_geometry(ctx, image.dim_x, image.dim_y, image.dim_z, (int)image.data_type);
+	status = check_texel_count(image.dim_x, image.dim_y, image.dim_z);
+	if (status == ASTCENC_SUCCESS && geo.payload_overflow()) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS && data_len < geo.out_bytes()) status = ASTCENC_ERR_OUT_OF_MEM;
+	if (status == ASTCENC_SUCCESS) status = check_alpha_scale(ctx, image.dim_z);
+	if (status != ASTCENC_SUCCESS) {
+		return status;
 	}
 	if (ctx->thread_count == 1) {
 		astcenc_compress_reset(ctx);
 	}
-	std::unique_lock<std::mutex> lk(ctx->mtx);
-	if (ctx->state == 0) {
-		ctx->state = 1;
-		lk.unlock();
-		astcenc_error r = compress_image_gpu(ctx, image, *swizzle, data_out);
-		lk.lock();
-		ctx->result = r;
-		ctx->state = 2;
-		ctx->cv.notify_all();
-		return r;
-	}
-	ctx->cv.wait(lk, [ctx] { return ctx->state == 2; });
-	return ctx->result;
+	return run_once(ctx, ctx->compress_gate, [&] { return compress_image_gpu(ctx, image, geo, *swizzle, data_out); });
 }
 
 astcenc_error astcenc_compress_reset(astcenc_context* ctx) {
@@ -1460,9 +1292,7 @@ astcenc_error astcenc_compress_reset(astcenc_context* ctx) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
 	std::lock_guard<std::mutex> lk(ctx->mtx);
-	if (ctx->state != 1) {
-		ctx->state = 0;
-	}
+	ctx->compress_gate.reset();
 	std::lock_guard<std::mutex> fl(ctx->flag_mtx);
 	ctx->cancel = false;
 	if (ctx->flag_raised) {
@@ -1501,84 +1331,54 @@ static astcenc_error validate_decompression_swizzle(const astcenc_swizzle& s) { 
 	return ASTCENC_SUCCESS;
 }
 
-static astcenc_error decompress_image_gpu(astcenc_context* ctx, const uint8_t* data, astcenc_image& image, const astcenc_swizzle& swizzle) {
+static astcenc_error decompress_image_gpu(astcenc_context* ctx, const uint8_t* data, astcenc_image& image, const SlabGeometry& geo, const astcenc_swizzle& swizzle) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	DeviceGuard guard(ctx->device);
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	std::lock_guard<std::mutex> launch_lock(ctx->launch_mtx);      // (shares d_image / d_out with the compression path)
+	std::lock_guard<std::mutex> launch_lock(ctx->launch_mtx);      // (shares image / out with the compression path)
 	if (ctx->scratch_used) {
 		CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
-	size_t bpt = image.data_type == ASTCENC_TYPE_U8 ? 4 : image.data_type == ASTCENC_TYPE_F16 ? 8 : 16;
-	size_t slice_bytes = (size_t)image.dim_x * image.dim_y * bpt;
-	size_t blocks_x = block_count_axis(image.dim_x, bsd.dim_x);
-	size_t blocks_y = block_count_axis(image.dim_y, bsd.dim_y);
 	// 3D block sizes decode the volume in one pass (blocks in z, y, x order); 2D block sizes take it slice by slice
-	const bool volume = bsd.dim_z > 1;
-	size_t blocks_z = volume ? block_count_axis(image.dim_z, bsd.dim_z) : 1;
-	size_t in_bytes = blocks_x * blocks_y * blocks_z * 16;
-	size_t image_bytes = volume ? slice_bytes * image.dim_z : slice_bytes;
-	if (ctx->d_image_bytes < image_bytes) {
-		cudaFree(ctx->d_image);
-		ctx->d_image = nullptr;
-		ctx->d_image_bytes = 0;
-		CUDA_TRY(cudaMalloc(&ctx->d_image, image_bytes), return ASTCENC_ERR_OUT_OF_MEM);
-		ctx->d_image_bytes = image_bytes;
+	const size_t slice_bytes = geo.slice_bytes;
+	const size_t in_bytes = geo.pass_out_bytes();
+	astcenc_error st = ensure_buffer(ctx->image, slice_bytes * geo.pass_slices());
+	if (st == ASTCENC_SUCCESS) {
+		st = ensure_buffer(ctx->out, in_bytes);
 	}
-	if (ctx->d_out_bytes < in_bytes) {
-		cudaFree(ctx->d_out);
-		ctx->d_out = nullptr;
-		ctx->d_out_bytes = 0;
-		CUDA_TRY(cudaMalloc(&ctx->d_out, in_bytes), return ASTCENC_ERR_OUT_OF_MEM);
-		ctx->d_out_bytes = in_bytes;
+	if (st != ASTCENC_SUCCESS) {
+		return st;
 	}
-	DevImage img;
-	img.data = ctx->d_image;
-	img.data_type = (int)image.data_type;
-	img.dim_x = image.dim_x;
-	img.dim_y = image.dim_y;
-	img.dim_z = volume ? image.dim_z : 1;
-	img.blocks_x = (unsigned int)blocks_x;
-	img.blocks_y = (unsigned int)blocks_y;
-	img.block_row0 = 0;
-	img.block_rows = (unsigned int)(blocks_y * blocks_z);
-	img.swz[0] = (int)swizzle.r;
-	img.swz[1] = (int)swizzle.g;
-	img.swz[2] = (int)swizzle.b;
-	img.swz[3] = (int)swizzle.a;
-	img.out = nullptr;
-	img.alpha_avg = nullptr;
-	img.alpha_threshold = 0.0f;
-	img.cancel = nullptr;
-	img.done = nullptr;
+	DevImage img = pass_image(ctx, ctx->image.ptr, (int)image.data_type, image.dim_x, image.dim_y, geo.pass_slices(), swizzle);
+	img.block_rows = geo.pass_rows();
 	cudaDeviceProp prop;
 	CUDA_TRY(cudaGetDeviceProperties(&prop, ctx->device), return ASTCENC_ERR_BAD_CONTEXT);
-	unsigned int nblocks = (unsigned int)(blocks_x * blocks_y * blocks_z);
+	unsigned int nblocks = (unsigned int)(geo.blocks_x * geo.pass_rows());
 	int warps = ASTC_DECODE_THREADS / 32;
 	int grid = (int)((nblocks + warps - 1) / warps);
 	if (grid > prop.multiProcessorCount * 8) {
 		grid = prop.multiProcessorCount * 8;
 	}
-	if (volume) {
-		CUDA_TRY(cudaMemcpyAsync(ctx->d_out, data, in_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		astc_decompress_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, ctx->stream>>>(bsd, ctx->dcfg, img, ctx->d_out, nblocks);
+	if (geo.volume) {
+		CUDA_TRY(cudaMemcpyAsync(ctx->out.ptr, data, in_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		astc_decompress_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, ctx->stream>>>(bsd, ctx->dcfg, img, ctx->out.ptr, nblocks);
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		ctx->launches++;
 		for (unsigned int z = 0; z < image.dim_z; z++) {
-			CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->d_image + (size_t)z * slice_bytes, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+			CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->image.ptr + (size_t)z * slice_bytes, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		}
 		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		return ASTCENC_SUCCESS;
 	}
 	// 3D images with 2D blocks are an array of independent 2D slices; blocks of slice z follow those of slice z - 1
 	for (unsigned int z = 0; z < image.dim_z; z++) {
-		CUDA_TRY(cudaMemcpyAsync(ctx->d_out, data + (size_t)z * in_bytes, in_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		astc_decompress_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, ctx->stream>>>(bsd, ctx->dcfg, img, ctx->d_out, nblocks);
+		CUDA_TRY(cudaMemcpyAsync(ctx->out.ptr, data + (size_t)z * in_bytes, in_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		astc_decompress_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, ctx->stream>>>(bsd, ctx->dcfg, img, ctx->out.ptr, nblocks);
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		ctx->launches++;
-		CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->d_image, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->image.ptr, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	}
 	return ASTCENC_SUCCESS;
@@ -1595,47 +1395,23 @@ astcenc_error astcenc_decompress_image(astcenc_context* ctx, const uint8_t* data
 		return status;
 	}
 	astcenc_image& image = *image_outp;
-	bool overflow = false;
-	size_t texel_count = mul_safe(mul_safe(image.dim_x, image.dim_y, overflow), image.dim_z, overflow);
-	if (overflow || texel_count == 0) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	size_t blocks_x = block_count_axis(image.dim_x, ctx->config.block_x);
-	size_t blocks_y = block_count_axis(image.dim_y, ctx->config.block_y);
-	size_t blocks_z = block_count_axis(image.dim_z, ctx->config.block_z);
-	overflow = false;
-	size_t block_count = mul_safe(mul_safe(blocks_x, blocks_y, overflow), blocks_z, overflow);
-	mul_safe(block_count, 16, overflow);
-	if (overflow || block_count == 0) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	if (data_len < block_count * 16) {
-		return ASTCENC_ERR_OUT_OF_MEM;
+	const SlabGeometry geo = slab_geometry(ctx, image.dim_x, image.dim_y, image.dim_z, (int)image.data_type);
+	status = check_texel_count(image.dim_x, image.dim_y, image.dim_z);
+	if (status == ASTCENC_SUCCESS && geo.payload_overflow()) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS && data_len < geo.out_bytes()) status = ASTCENC_ERR_OUT_OF_MEM;
+	if (status != ASTCENC_SUCCESS) {
+		return status;
 	}
 	// any subset of the thread_count callers may call; the image is decoded once, everybody returns when it is done
 	if (ctx->thread_count == 1) {
 		astcenc_decompress_reset(ctx);
 	}
-	std::unique_lock<std::mutex> lk(ctx->mtx);
-	if (ctx->dstate == 0) {
-		ctx->dstate = 1;
-		lk.unlock();
-		astcenc_error r = decompress_image_gpu(ctx, data, image, *swizzle);
-		lk.lock();
-		ctx->dresult = r;
-		ctx->dstate = 2;
-		ctx->cv.notify_all();
-		return r;
-	}
-	ctx->cv.wait(lk, [ctx] { return ctx->dstate == 2; });
-	return ctx->dresult;
+	return run_once(ctx, ctx->decompress_gate, [&] { return decompress_image_gpu(ctx, data, image, geo, *swizzle); });
 }
 
 astcenc_error astcenc_decompress_reset(astcenc_context* ctx) {
 	std::lock_guard<std::mutex> lk(ctx->mtx);
-	if (ctx->dstate != 1) {
-		ctx->dstate = 0;
-	}
+	ctx->decompress_gate.reset();
 	return ASTCENC_SUCCESS;
 }
 
@@ -1850,10 +1626,8 @@ const char* astcenc_get_error_string(astcenc_error status) {
 // ---- extensions ----
 astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_pixels, astcenc_type data_type, unsigned int dim_x, unsigned int dim_y,
                                            const astcenc_swizzle* swizzle, unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, void* cuda_stream) {
-	if (ctx->config.flags & ASTCENC_FLG_DECOMPRESS_ONLY) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	astcenc_error status = validate_compression_swizzle(*swizzle);
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
 	if (status != ASTCENC_SUCCESS) {
 		return status;
 	}
@@ -1882,40 +1656,40 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 // one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks blocks). The
 // whole call is one turn of the context's scratch (launch_mtx, scratch_done), like a launch_slab. `src` is the whole source
 // image, dim_z slices of it.
-static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, const astcenc_swizzle& swizzle, const std::vector<uint32_t>& list,
-                                   unsigned int row_lo, unsigned int row_hi, uint8_t* d_payload, cudaStream_t stream) {
+static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, const SlabGeometry& geo, const astcenc_swizzle& swizzle,
+                                   const std::vector<uint32_t>& list, unsigned int row_lo, unsigned int row_hi, uint8_t* d_payload, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
-	const bool volume = bsd.dim_z > 1;
+	const bool volume = geo.volume;
 	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
 	const size_t n = list.size();
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
-	const unsigned int words = src.data_type == ASTCENC_TYPE_U8 ? 1 : src.data_type == ASTCENC_TYPE_F16 ? 2 : 4;
+	const unsigned int words = (unsigned int)(geo.texel_bytes / 4);
 	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
 	if (ctx->scratch_used) {
 		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
-	astcenc_error st = ensure_buffer(ctx->d_list, ctx->d_list_bytes, n * sizeof(uint32_t));
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_list_image, ctx->d_list_image_bytes, chunk * bsd.texel_count * words * 4);
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->d_list_out, ctx->d_list_out_bytes, chunk * 16);
+	astcenc_error st = ensure_buffer(ctx->list, n * sizeof(uint32_t));
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * geo.texel_bytes);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
 	if (st == ASTCENC_SUCCESS && radius != 0) {
-		st = ensure_buffer(ctx->d_list_alpha, ctx->d_list_alpha_bytes, (size_t)src.dim_x * src.dim_y * sizeof(float));
+		st = ensure_buffer(ctx->list_alpha, (size_t)src.dim_x * src.dim_y * sizeof(float));
 		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
 	if (st == ASTCENC_SUCCESS) {
 		// (from pageable memory: staged by the driver before the call returns, so `list` may go when this function does)
-		CUDA_TRY(cudaMemcpyAsync(ctx->d_list, list.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, list.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
 	// The staging pass reads averages gathered from the source's, so it runs no pre-pass of its own: its box filter would reach
 	// across the seams between unrelated blocks. The source's averages cover the listed blocks' rows, at their image positions.
 	float threshold = 0.0f;
 	if (st == ASTCENC_SUCCESS && radius != 0) {
-		st = alpha_prepass(ctx, src, row_lo, row_hi + 1, reinterpret_cast<float*>(ctx->d_list_alpha), stream, threshold);
+		st = alpha_prepass(ctx, src, row_lo, row_hi + 1, ctx->list_alpha.as<float>(), stream, threshold);
 	}
 	GatherArgs g;
 	g.src = src.data;
-	g.dst = ctx->d_list_image;
-	g.avg_src = radius != 0 ? reinterpret_cast<const float*>(ctx->d_list_alpha) : nullptr;
-	g.avg_dst = radius != 0 ? ctx->d_alpha : nullptr;
+	g.dst = ctx->list_image.ptr;
+	g.avg_src = radius != 0 ? ctx->list_alpha.as<const float>() : nullptr;
+	g.avg_dst = radius != 0 ? ctx->alpha.as<float>() : nullptr;
 	g.words = words;
 	g.dim_x = src.dim_x;
 	g.dim_y = src.dim_y;
@@ -1928,19 +1702,19 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, co
 	const int aligned16 = (reinterpret_cast<uintptr_t>(d_payload) & 15) == 0;
 	for (size_t first = 0; first < n && st == ASTCENC_SUCCESS; first += chunk) {
 		const unsigned int m = (unsigned int)(n - first < chunk ? n - first : chunk);
-		const uint32_t* d_idx = reinterpret_cast<const uint32_t*>(ctx->d_list) + first;
+		const uint32_t* d_idx = ctx->list.as<const uint32_t>() + first;
 		g.indices = d_idx;
 		g.n = m;
 		const unsigned int warps = ASTC_GATHER_THREADS / 32;
-		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
+		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->plan.grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->plan.grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
 		ctx->launches++;
 		// (the staging volume is one layer deep)
-		DevImage staged = pass_image(ctx, ctx->d_list_image, src.data_type, m * bsd.dim_x, bsd.dim_y, volume ? bsd.dim_z : 1, swizzle);
-		staged.alpha_avg = radius != 0 ? ctx->d_alpha : nullptr;
+		DevImage staged = pass_image(ctx, ctx->list_image.ptr, src.data_type, m * bsd.dim_x, bsd.dim_y, volume ? bsd.dim_z : 1, swizzle);
+		staged.alpha_avg = radius != 0 ? ctx->alpha.as<float>() : nullptr;
 		staged.alpha_threshold = threshold;
-		st = launch_slab_locked(ctx, staged, 0, 1, ctx->d_list_out, stream, nullptr);
+		st = launch_slab_locked(ctx, staged, 0, 1, ctx->list_out.ptr, stream, nullptr);
 		if (st == ASTCENC_SUCCESS) {
-			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->d_list_out, d_idx, m, d_payload, aligned16);
+			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, d_idx, m, d_payload, aligned16);
 			ctx->launches++;
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 		}
@@ -1953,41 +1727,27 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, co
 astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const void* d_pixels, astcenc_type data_type, unsigned int dim_x, unsigned int dim_y,
                                                   unsigned int dim_z, const astcenc_swizzle* swizzle, const uint32_t* block_indices, unsigned int block_count,
                                                   uint8_t* d_payload, void* cuda_stream) {
-	if (ctx->config.flags & ASTCENC_FLG_DECOMPRESS_ONLY) {
-		return ASTCENC_ERR_BAD_CONTEXT;
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS && (dim_x == 0 || dim_y == 0 || dim_z == 0 || !d_pixels || !d_payload || (block_count != 0 && !block_indices))) {
+		status = ASTCENC_ERR_BAD_PARAM;
 	}
-	if (!swizzle) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	astcenc_error status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
+	if (status == ASTCENC_SUCCESS) status = check_alpha_scale(ctx, dim_z);
+	const SlabGeometry geo = slab_geometry(ctx, dim_x, dim_y, dim_z, (int)data_type);
+	if (status == ASTCENC_SUCCESS && geo.overflow) status = ASTCENC_ERR_BAD_PARAM;
 	if (status != ASTCENC_SUCCESS) {
 		return status;
-	}
-	if (dim_x == 0 || dim_y == 0 || dim_z == 0 || !d_pixels || !d_payload || (block_count != 0 && !block_indices)) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	if ((int)data_type < 0 || (int)data_type > 2) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	if (ctx->config.a_scale_radius != 0 && dim_z != 1 && ctx->config.block_z <= 1) {
-		return ASTCENC_ERR_NOT_IMPLEMENTED;      // as astcenc_compress_image: the pre-pass is built for 2D images
-	}
-	size_t blocks_x = block_count_axis(dim_x, ctx->config.block_x);
-	size_t blocks_y = block_count_axis(dim_y, ctx->config.block_y);
-	size_t blocks_z = block_count_axis(dim_z, ctx->config.block_z);
-	bool overflow = false;
-	size_t total = mul_safe(mul_safe(blocks_x, blocks_y, overflow), blocks_z, overflow);
-	if (overflow) {
-		return ASTCENC_ERR_BAD_PARAM;
 	}
 	// the list is checked whole before anything is enqueued, and copied: the caller may free it when the call returns
 	std::vector<uint32_t> list(block_indices, block_indices + block_count);
 	unsigned int row_lo = 0xFFFFFFFFu, row_hi = 0;
 	for (uint32_t b : list) {
-		if (b >= total) {
+		if (b >= geo.blocks) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
-		unsigned int row = (unsigned int)(b / blocks_x);      // (2D images: the block row, for the alpha-scale pre-pass window)
+		unsigned int row = (unsigned int)(b / geo.blocks_x);      // (2D images: the block row, for the alpha-scale pre-pass window)
 		row_lo = row < row_lo ? row : row_lo;
 		row_hi = row > row_hi ? row : row_hi;
 	}
@@ -1999,7 +1759,7 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_blocks(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, *swizzle), *swizzle, list, row_lo, row_hi, d_payload, s);
+	return launch_blocks(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, *swizzle), geo, *swizzle, list, row_lo, row_hi, d_payload, s);
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {
@@ -2043,9 +1803,9 @@ __attribute__((visibility("default"))) astcenc_error astcenc_b200_debug_records(
 	if (!ctx || !records || !record_bytes || !capacity_bytes) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
-	*records = ctx->d_records;
+	*records = ctx->records.ptr;
 	*record_bytes = ctx->tables->bsd.record_bytes;
-	*capacity_bytes = ctx->d_records_bytes;
+	*capacity_bytes = ctx->records.bytes;
 	return ASTCENC_SUCCESS;
 }
 

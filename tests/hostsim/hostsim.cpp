@@ -12,6 +12,7 @@
 #include "../../astc-encoder_b200/csrc/astc_dev_search.cuh"
 #include "../../astc-encoder_b200/csrc/astc_host_pack.h"
 #include "../../astc-encoder_b200/csrc/astc_host_config.h"
+#include "../../astc-encoder_b200/csrc/astc_host_launch.h"
 #include <vector>
 #include <cstdio>
 #include <cstring>
@@ -268,4 +269,18 @@ extern "C" unsigned int hostsim_arena_bytes(int profile, unsigned int bx, unsign
 		        pk.bsd.off_lowhigh, pk.bsd.off_mode_err, pk.bsd.record_bytes, pk.bsd.decimation_mode_count_selected, pk.bsd.block_mode_count_1plane_2plane_selected, pk.bsd.dec_stage_bytes);
 	}
 	return pk.bsd.arena_bytes;
+}
+
+// The launch plan (astc_host_launch.h) of a compressing context with these knobs on an SM of smem_limit bytes of opt-in shared memory.
+// Returns the astcenc_error of plan_kernels, or -1 when the configuration itself is refused.
+extern "C" int hostsim_kernel_plan(int profile, unsigned int bx, unsigned int by, unsigned int bz, float quality, unsigned int flags, size_t smem_limit,
+                                   int sm_count, const Knobs* knobs, KernelPlan* out) {
+	astcenc_config cfg;
+	if (astc_host::config_init((astcenc_profile)profile, bx, by, bz, quality, flags, &cfg) != ASTCENC_SUCCESS) return -1;
+	if (astc_host::validate_config(cfg) != ASTCENC_SUCCESS) return -1;
+	astc_host::PackedTables pk;
+	astc_host::BlockSizeTables* t = astc_host::build_packed_tables(cfg, pk);
+	int status = (int)plan_kernels(pk.bsd, pk.bsd_1p, cfg, smem_limit, sm_count, *knobs, *out);
+	astc_host::free_block_size_tables(t);
+	return status;
 }

@@ -62,6 +62,11 @@ class Swizzle(C.Structure):
     _fields_ = [("r", C.c_int), ("g", C.c_int), ("b", C.c_int), ("a", C.c_int)]
 
 
+class DeviceImage(C.Structure):
+    """struct astcenc_b200_device_image (include/astcenc.h)."""
+    _fields_ = [("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("payload", C.c_void_p)]
+
+
 class ErrorMetrics(C.Structure):
     """struct astcenc_b200_error_metrics (include/astcenc.h)."""
     _fields_ = [(n, C.c_double) for n in ("psnr", "alpha_psnr", "rgb_psnr", "rgb_peak", "peak_psnr", "mpsnr", "log_rmse",
@@ -114,6 +119,11 @@ def lib():
         l.astcenc_b200_compress_device_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.POINTER(Swizzle), C.c_void_p,
                                                           C.c_uint, C.c_void_p, C.c_void_p]
         l.astcenc_b200_compress_device_blocks.restype = C.c_int
+        l.astcenc_b200_compress_device_images.argtypes = [C.c_void_p, C.POINTER(DeviceImage), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
+        l.astcenc_b200_compress_device_images.restype = C.c_int
+        l.astcenc_b200_compress_images.argtypes = [C.c_void_p, C.POINTER(C.POINTER(Image)), C.c_uint, C.POINTER(Swizzle), C.POINTER(C.c_void_p),
+                                                   C.POINTER(C.c_size_t)]
+        l.astcenc_b200_compress_images.restype = C.c_int
         l.astcenc_b200_launch_count.argtypes = [C.c_void_p]
         l.astcenc_b200_launch_count.restype = C.c_ulonglong
         l.astcenc_b200_last_timing.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
@@ -277,6 +287,32 @@ class Context:
                                                         idx.ctypes.data if idx.size else None, idx.size, C.c_void_p(d_payload_ptr), C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compress_device_blocks")
+
+    def compress_device_images(self, images, data_type, swizzle=(0, 1, 2, 3), stream=0):
+        """Many device-resident images in shared passes (astcenc_b200_compress_device_images). images: a sequence of
+        (d_pixels_ptr, dim_x, dim_y, dim_z, d_payload_ptr); every payload receives its image's whole payload, the bytes
+        compress_image gives for that image. Enqueued on `stream`, no sync."""
+        n = len(images)
+        table = (DeviceImage * n)(*[DeviceImage(C.c_void_p(p), x, y, z, C.c_void_p(q)) for p, x, y, z, q in images])
+        sw = Swizzle(*swizzle)
+        err = lib().astcenc_b200_compress_device_images(self.handle, table if n else None, n, data_type, C.byref(sw), C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compress_device_images")
+
+    def compress_images(self, arrays, swizzle=(0, 1, 2, 3)):
+        """Host-pointer twin (astcenc_b200_compress_images): (H, W, 4) / (D, H, W, 4) numpy arrays of one dtype -> their payloads
+        (uint8 arrays), compressed in shared passes."""
+        n = len(arrays)
+        prepared = [self._image(a) for a in arrays]
+        ptrs = (C.POINTER(Image) * n)(*[C.pointer(p[2]) for p in prepared])
+        outs = [np.empty(p[3], dtype=np.uint8) for p in prepared]
+        optr = (C.c_void_p * n)(*[o.ctypes.data for o in outs])
+        lens = (C.c_size_t * n)(*[o.nbytes for o in outs])
+        sw = Swizzle(*swizzle)
+        err = lib().astcenc_b200_compress_images(self.handle, ptrs, n, C.byref(sw), optr, lens)
+        if err:
+            raise AstcencError(err, "astcenc_b200_compress_images")
+        return outs
 
     def launch_count(self):
         return int(lib().astcenc_b200_launch_count(self.handle))

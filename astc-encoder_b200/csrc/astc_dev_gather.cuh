@@ -1,4 +1,4 @@
-// CUDA-native ASTC: block lists (astcenc_b200_compress_device_blocks). A block's 16 bytes depend on its texels after clamp-to-edge,
+// CUDA-native ASTC: block lists (astcenc_b200_compress_device_blocks) and image tables. A block's 16 bytes depend on its texels after clamp-to-edge,
 // the alpha-scale test over its footprint and the context - not on where it sits (void extents carry no coordinates, partition
 // tables are indexed by seed). So the listed blocks are copied, footprint by footprint, into a staging image that is ONE ROW of
 // blocks, an ordinary pass of the wave pipeline compresses that row, and a scatter puts staging block i at the listed position.
@@ -7,7 +7,22 @@
 // Staging layout of n listed blocks of a bx x by (x bz) footprint: (n * bx) x by texels (x bz slices for 3D block sizes), block i
 // at x = i * bx. Every staged texel lies inside the staging image, so load_block reads it without clamping; the gather has done
 // the clamping against the source image, exactly as load_block clamps in place (astcenc_image.cpp:162-342).
+//
+// Image tables (astcenc_b200_compress_device_images) stage every block of several images the same way. Staging block c of a call
+// is block c - first[j] of image j, where first[] is the exclusive prefix sum of the images' block counts in call order; the
+// gather and the scatter find j by binary search over first[]. A chunk of the call (GatherArgs::base) may span several images,
+// and an image several chunks.
 #pragma once
+
+// One image of an image table.
+struct GatherImage {
+	const void* data;           // dim_z slices of dim_x * dim_y texels, contiguous
+	uint8_t* payload;           // the image's whole payload
+	size_t first;               // call block of the image's block 0
+	size_t avg_offset;          // where the image's alpha-scale averages start in GatherArgs::avg_src
+	unsigned int dim_x, dim_y, dim_z;
+	unsigned int blocks_x, blocks_y;
+};
 
 struct GatherArgs {
 	const void* src;            // the caller's image: dim_z slices of dim_x * dim_y texels, contiguous
@@ -20,6 +35,11 @@ struct GatherArgs {
 	unsigned int dim_x, dim_y, dim_z;
 	unsigned int blocks_x, blocks_y;
 	unsigned int bx, by, bz;    // footprint; bz = 1 for 2D block sizes, whose block index then counts slice z of a texture array
+	// An image table: staging block i is call block base + i of `images` (whose entries replace src, avg_src's offset and the
+	// dims above). Null: one source image and the index list.
+	const GatherImage* images = nullptr;
+	unsigned int image_count = 0;
+	size_t base = 0;
 };
 
 // Texel t (x fastest, then y, then z) of listed block i: where it comes from in the source image (a texel index, clamped to the
@@ -49,10 +69,26 @@ ASTC_FN GatherTexel gather_texel(const GatherArgs& g, unsigned int i, uint32_t i
 	return r;
 }
 
-// Listed block i, by the lanes of one warp (lane / lanes): the texels word by word, so that consecutive lanes read consecutive
-// words of a footprint row; then the alpha averages (0 for texels outside the image). The host simulation calls it with 0 / 1.
-ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lanes) {
-	const uint32_t index = ASTC_LDG(g.indices + i);
+// The table entry that holds staging block i: the last image whose first block is at or before call block base + i (every image
+// has at least one block, so there is exactly one).
+ASTC_FN unsigned int table_image(const GatherArgs& g, unsigned int i) {
+	const size_t c = g.base + i;
+	unsigned int lo = 0, hi = g.image_count - 1;
+	while (lo < hi) {
+		unsigned int mid = (lo + hi + 1) / 2;
+		if (g.images[mid].first <= c) {
+			lo = mid;
+		} else {
+			hi = mid - 1;
+		}
+	}
+	return lo;
+}
+
+// Block `index` of the source described by g into staging block i, by the lanes of one warp (lane / lanes): the texels word by
+// word, so that consecutive lanes read consecutive words of a footprint row; then the alpha averages (0 for texels outside the
+// image).
+ASTC_FN void gather_footprint(const GatherArgs& g, unsigned int i, uint32_t index, int lane, int lanes) {
 	const unsigned int T = g.bx * g.by * g.bz;
 	const uint32_t* src = static_cast<const uint32_t*>(g.src);
 	uint32_t* dst = static_cast<uint32_t*>(g.dst);
@@ -67,4 +103,31 @@ ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lan
 			g.avg_dst[p.dst] = p.inside ? ASTC_LDG(g.avg_src + p.src) : 0.0f;
 		}
 	}
+}
+
+// Staging block i: listed block i of the one source, or its block of an image table. The host simulation calls it with 0 / 1.
+ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lanes) {
+	if (g.images == nullptr) {
+		gather_footprint(g, i, ASTC_LDG(g.indices + i), lane, lanes);
+		return;
+	}
+	const GatherImage& im = g.images[table_image(g, i)];
+	GatherArgs s = g;
+	s.src = im.data;
+	s.avg_src = g.avg_src != nullptr ? g.avg_src + im.avg_offset : nullptr;
+	s.dim_x = im.dim_x;
+	s.dim_y = im.dim_y;
+	s.dim_z = im.dim_z;
+	s.blocks_x = im.blocks_x;
+	s.blocks_y = im.blocks_y;
+	gather_footprint(s, i, (uint32_t)(g.base + i - im.first), lane, lanes);      // (an image has fewer than 2^32 blocks)
+}
+
+// Where staging block i goes: the payload position of listed block i, or of its block of an image table.
+ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i, uint8_t* payload) {
+	if (g.images == nullptr) {
+		return payload + (size_t)ASTC_LDG(g.indices + i) * 16;
+	}
+	const GatherImage& im = g.images[table_image(g, i)];
+	return im.payload + (g.base + i - im.first) * 16;
 }

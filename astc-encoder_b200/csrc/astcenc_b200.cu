@@ -206,7 +206,7 @@ astc_alpha_average_kernel(const __grid_constant__ DevImage img, unsigned int rad
 	alpha_average_tile(img, radius, tx * ALPHA_TILE, ty * ALPHA_TILE, 0, averages, (int)threadIdx.x, (int)blockDim.x);
 }
 
-// ---- block lists (astc_dev_gather.cuh): one warp per listed block, grid-stride ----
+// ---- block lists and image tables (astc_dev_gather.cuh): one warp per staging block, grid-stride ----
 #define ASTC_GATHER_THREADS 256
 __global__ void __launch_bounds__(ASTC_GATHER_THREADS)
 astc_gather_blocks_kernel(const __grid_constant__ GatherArgs g) {
@@ -216,16 +216,16 @@ astc_gather_blocks_kernel(const __grid_constant__ GatherArgs g) {
 	}
 }
 
-// staging block i -> payload block indices[i] (duplicates write the same bytes); one thread per block
+// staging block i -> its payload position (duplicate list entries write the same bytes); one thread per block
 __global__ void __launch_bounds__(ASTC_GATHER_THREADS)
-astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const uint32_t* __restrict__ indices, unsigned int n, uint8_t* payload, int aligned16) {
+astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_constant__ GatherArgs g, uint8_t* payload) {
 	unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) {
+	if (i >= g.n) {
 		return;
 	}
-	uint8_t* dst = payload + (size_t)__ldg(indices + i) * 16;
+	uint8_t* dst = scatter_target(g, i, payload);
 	uint4 v = __ldg(reinterpret_cast<const uint4*>(staged) + i);
-	if (aligned16) {
+	if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
 		*reinterpret_cast<uint4*>(dst) = v;
 	} else {
 		const uint8_t* b = reinterpret_cast<const uint8_t*>(&v);
@@ -1652,45 +1652,68 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 	return launch_slab(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, 1, *swizzle), block_row0, block_rows, d_out, s);
 }
 
-// Block lists (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk (a staging row is
-// one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks blocks). The
-// whole call is one turn of the context's scratch (launch_mtx, scratch_done), like a launch_slab. `src` is the whole source
-// image, dim_z slices of it.
-static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, const SlabGeometry& geo, const astcenc_swizzle& swizzle,
-                                   const std::vector<uint32_t>& list, unsigned int row_lo, unsigned int row_hi, uint8_t* d_payload, cudaStream_t stream) {
+// What launch_blocks compresses: the listed blocks of one image (`list`), or every block of the images of `table`. `srcs` are
+// the source images as a pass reads them: the list's image, or one per table entry. Their alpha-scale pre-passes cover block
+// rows [row_lo, row_hi] of a list's image and the whole of each table image.
+struct BlockCall {
+	std::vector<DevImage> srcs;
+	std::vector<GatherImage> table;
+	std::vector<uint32_t> list;
+	unsigned int row_lo = 0, row_hi = 0;
+	size_t blocks = 0;                 // staging blocks of the whole call
+	size_t texel_bytes = 0;
+	uint8_t* payload = nullptr;        // (lists) the image's payload
+};
+
+// Block lists and image tables (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk
+// (a staging row is one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most
+// knobs.batch_blocks blocks). A chunk of an image table may span several images. The whole call is one turn of the context's
+// scratch (launch_mtx, scratch_done), like a launch_slab.
+static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
-	const bool volume = geo.volume;
+	const bool volume = bsd.dim_z > 1;
+	const bool table = !call.table.empty();
+	const DevImage& src = call.srcs[0];
 	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
-	const size_t n = list.size();
+	const size_t n = call.blocks;
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
-	const unsigned int words = (unsigned int)(geo.texel_bytes / 4);
+	size_t avg_floats = 0;
+	for (const DevImage& s : call.srcs) {
+		avg_floats += (size_t)s.dim_x * s.dim_y;
+	}
 	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
 	if (ctx->scratch_used) {
 		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
-	astcenc_error st = ensure_buffer(ctx->list, n * sizeof(uint32_t));
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * geo.texel_bytes);
+	const size_t list_bytes = table ? call.table.size() * sizeof(GatherImage) : n * sizeof(uint32_t);
+	astcenc_error st = ensure_buffer(ctx->list, list_bytes);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * call.texel_bytes);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
 	if (st == ASTCENC_SUCCESS && radius != 0) {
-		st = ensure_buffer(ctx->list_alpha, (size_t)src.dim_x * src.dim_y * sizeof(float));
+		st = ensure_buffer(ctx->list_alpha, avg_floats * sizeof(float));
 		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
 	if (st == ASTCENC_SUCCESS) {
-		// (from pageable memory: staged by the driver before the call returns, so `list` may go when this function does)
-		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, list.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+		// (from pageable memory: staged by the driver before the call returns, so the list or table may go when this function does)
+		const void* host = table ? static_cast<const void*>(call.table.data()) : static_cast<const void*>(call.list.data());
+		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, host, list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
-	// The staging pass reads averages gathered from the source's, so it runs no pre-pass of its own: its box filter would reach
-	// across the seams between unrelated blocks. The source's averages cover the listed blocks' rows, at their image positions.
+	// The staging pass reads averages gathered from the sources', so it runs no pre-pass of its own: its box filter would reach
+	// across the seams between unrelated blocks. A source's averages cover the staged blocks' rows, at their image positions, in
+	// the source's region of list_alpha. The threshold depends on the footprint and the radius alone: one value serves every source.
 	float threshold = 0.0f;
-	if (st == ASTCENC_SUCCESS && radius != 0) {
-		st = alpha_prepass(ctx, src, row_lo, row_hi + 1, ctx->list_alpha.as<float>(), stream, threshold);
+	size_t avg_offset = 0;
+	for (size_t k = 0; k < call.srcs.size() && st == ASTCENC_SUCCESS && radius != 0; k++) {
+		const DevImage& s = call.srcs[k];
+		st = alpha_prepass(ctx, s, table ? 0 : call.row_lo, table ? s.blocks_y : call.row_hi + 1, ctx->list_alpha.as<float>() + avg_offset, stream, threshold);
+		avg_offset += (size_t)s.dim_x * s.dim_y;
 	}
 	GatherArgs g;
 	g.src = src.data;
 	g.dst = ctx->list_image.ptr;
 	g.avg_src = radius != 0 ? ctx->list_alpha.as<const float>() : nullptr;
 	g.avg_dst = radius != 0 ? ctx->alpha.as<float>() : nullptr;
-	g.words = words;
+	g.words = (unsigned int)(call.texel_bytes / 4);
 	g.dim_x = src.dim_x;
 	g.dim_y = src.dim_y;
 	g.dim_z = src.dim_z;
@@ -1699,11 +1722,12 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, co
 	g.bx = bsd.dim_x;
 	g.by = bsd.dim_y;
 	g.bz = bsd.dim_z;
-	const int aligned16 = (reinterpret_cast<uintptr_t>(d_payload) & 15) == 0;
+	g.images = table ? ctx->list.as<const GatherImage>() : nullptr;
+	g.image_count = (unsigned int)call.table.size();
 	for (size_t first = 0; first < n && st == ASTCENC_SUCCESS; first += chunk) {
 		const unsigned int m = (unsigned int)(n - first < chunk ? n - first : chunk);
-		const uint32_t* d_idx = ctx->list.as<const uint32_t>() + first;
-		g.indices = d_idx;
+		g.indices = table ? nullptr : ctx->list.as<const uint32_t>() + first;
+		g.base = first;
 		g.n = m;
 		const unsigned int warps = ASTC_GATHER_THREADS / 32;
 		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->plan.grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->plan.grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
@@ -1714,7 +1738,7 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const DevImage& src, co
 		staged.alpha_threshold = threshold;
 		st = launch_slab_locked(ctx, staged, 0, 1, ctx->list_out.ptr, stream, nullptr);
 		if (st == ASTCENC_SUCCESS) {
-			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, d_idx, m, d_payload, aligned16);
+			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g, call.payload);
 			ctx->launches++;
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 		}
@@ -1741,15 +1765,16 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
 		return status;
 	}
 	// the list is checked whole before anything is enqueued, and copied: the caller may free it when the call returns
-	std::vector<uint32_t> list(block_indices, block_indices + block_count);
-	unsigned int row_lo = 0xFFFFFFFFu, row_hi = 0;
-	for (uint32_t b : list) {
+	BlockCall call;
+	call.list.assign(block_indices, block_indices + block_count);
+	call.row_lo = 0xFFFFFFFFu;
+	for (uint32_t b : call.list) {
 		if (b >= geo.blocks) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
 		unsigned int row = (unsigned int)(b / geo.blocks_x);      // (2D images: the block row, for the alpha-scale pre-pass window)
-		row_lo = row < row_lo ? row : row_lo;
-		row_hi = row > row_hi ? row : row_hi;
+		call.row_lo = row < call.row_lo ? row : call.row_lo;
+		call.row_hi = row > call.row_hi ? row : call.row_hi;
 	}
 	if (block_count == 0) {
 		return ASTCENC_SUCCESS;
@@ -1759,7 +1784,159 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_blocks(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, *swizzle), geo, *swizzle, list, row_lo, row_hi, d_payload, s);
+	call.srcs.push_back(pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, *swizzle));
+	call.blocks = block_count;
+	call.texel_bytes = geo.texel_bytes;
+	call.payload = d_payload;
+	return launch_blocks(ctx, call, *swizzle, s);
+}
+
+// The image table of a multi-image call, checked whole before anything is enqueued (the caller has checked the context, the
+// swizzle and the pointers): zero dimensions and the data type (ASTCENC_ERR_BAD_PARAM), a_scale_radius on a texture array
+// (ASTCENC_ERR_NOT_IMPLEMENTED), then the block counts (ASTCENC_ERR_BAD_PARAM when an image's payload does not fit a size_t, an
+// image has 2^32 blocks or more - the gather indexes an image's blocks with 32 bits, as block lists do - or the call's total
+// does not fit a size_t). Fills call.table (data and payload as given), call.srcs, call.blocks and call.texel_bytes.
+static astcenc_error plan_image_table(const astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
+                                      const astcenc_swizzle& swizzle, BlockCall& call) {
+	astcenc_error status = ASTCENC_SUCCESS;
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
+		status = check_texel_count(images[i].dim_x, images[i].dim_y, images[i].dim_z);
+	}
+	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
+		status = check_alpha_scale(ctx, images[i].dim_z);
+	}
+	if (status != ASTCENC_SUCCESS) {
+		return status;
+	}
+	size_t blocks = 0, avg_offset = 0;
+	for (unsigned int i = 0; i < image_count; i++) {
+		const astcenc_b200_device_image& im = images[i];
+		const SlabGeometry geo = slab_geometry(ctx, im.dim_x, im.dim_y, im.dim_z, (int)data_type);
+		if (geo.payload_overflow() || geo.blocks > 0xFFFFFFFFu || geo.blocks > SIZE_MAX - blocks) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		GatherImage e;
+		e.data = im.data;
+		e.payload = im.payload;
+		e.first = blocks;
+		e.avg_offset = avg_offset;
+		e.dim_x = im.dim_x;
+		e.dim_y = im.dim_y;
+		e.dim_z = im.dim_z;
+		e.blocks_x = (unsigned int)geo.blocks_x;
+		e.blocks_y = (unsigned int)geo.blocks_y;
+		call.table.push_back(e);
+		call.srcs.push_back(pass_image(ctx, im.data, (int)data_type, im.dim_x, im.dim_y, im.dim_z, swizzle));
+		blocks += geo.blocks;
+		avg_offset += (size_t)im.dim_x * im.dim_y;
+		call.texel_bytes = geo.texel_bytes;
+	}
+	call.blocks = blocks;
+	return ASTCENC_SUCCESS;
+}
+
+astcenc_error astcenc_b200_compress_device_images(astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
+                                                  const astcenc_swizzle* swizzle, void* cuda_stream) {
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS && image_count != 0 && !images) status = ASTCENC_ERR_BAD_PARAM;
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
+		if (!images[i].data || !images[i].payload) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		}
+	}
+	BlockCall call;
+	if (status == ASTCENC_SUCCESS) status = plan_image_table(ctx, images, image_count, data_type, *swizzle, call);
+	if (status != ASTCENC_SUCCESS || image_count == 0) {
+		return status;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return launch_blocks(ctx, call, *swizzle, s);
+}
+
+// The host-pointer twin: every image goes up into one device buffer (ctx->image), the table is pointed at it and at one payload
+// buffer (ctx->out), one device-image call runs on the context's stream, and each payload comes back into data_out[i].
+astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* const* images, unsigned int image_count, const astcenc_swizzle* swizzle,
+                                           uint8_t* const* data_out, const size_t* data_len) {
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS && image_count != 0 && (!images || !data_out || !data_len)) status = ASTCENC_ERR_BAD_PARAM;
+	std::vector<astcenc_b200_device_image> descs;
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
+		const astcenc_image* im = images[i];
+		if (!im || !im->data || !data_out[i] || im->data_type != images[0]->data_type) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		} else {
+			// (planned with the host pointers; pointed at the device copies below)
+			descs.push_back({im->data, im->dim_x, im->dim_y, im->dim_z, data_out[i]});
+		}
+	}
+	BlockCall call;
+	if (status == ASTCENC_SUCCESS && image_count != 0) {
+		status = plan_image_table(ctx, descs.data(), image_count, images[0]->data_type, *swizzle, call);
+	}
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
+		const size_t end = i + 1 < image_count ? call.table[i + 1].first : call.blocks;
+		if (data_len[i] < (end - call.table[i].first) * 16) {
+			status = ASTCENC_ERR_OUT_OF_MEM;
+		}
+	}
+	if (status != ASTCENC_SUCCESS || image_count == 0) {
+		return status;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	// each image starts 256-byte aligned in the upload buffer
+	std::vector<size_t> in_offset(image_count);
+	size_t in_bytes = 0;
+	for (unsigned int i = 0; i < image_count; i++) {
+		in_offset[i] = in_bytes;
+		in_bytes += ((size_t)images[i]->dim_x * images[i]->dim_y * images[i]->dim_z * call.texel_bytes + 255) & ~(size_t)255;
+	}
+	astcenc_error st = ensure_buffer(ctx->image, in_bytes);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->out, call.blocks * 16);
+	if (st != ASTCENC_SUCCESS) {
+		return st;
+	}
+	ctx->last_h2d = ctx->last_d2h = 0;
+	ctx->last_kernel_ms = 0.0f;
+	for (unsigned int i = 0; i < image_count; i++) {
+		const astcenc_image& im = *images[i];
+		uint8_t* d_data = ctx->image.ptr + in_offset[i];
+		const size_t slice_bytes = (size_t)im.dim_x * im.dim_y * call.texel_bytes;
+		st = upload_slices(d_data, im.data, 0, im.dim_z, slice_bytes, ctx->stream);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
+		ctx->last_h2d += slice_bytes * im.dim_z;
+		call.table[i].data = d_data;
+		call.table[i].payload = ctx->out.ptr + call.table[i].first * 16;
+		call.srcs[i].data = d_data;
+	}
+	CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+	st = launch_blocks(ctx, call, *swizzle, ctx->stream);
+	if (st != ASTCENC_SUCCESS) {
+		return st;
+	}
+	CUDA_TRY(cudaEventRecord(ctx->ev1, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+	for (unsigned int i = 0; i < image_count; i++) {
+		const size_t end = i + 1 < image_count ? call.table[i + 1].first : call.blocks;
+		const size_t bytes = (end - call.table[i].first) * 16;
+		CUDA_TRY(cudaMemcpyAsync(data_out[i], call.table[i].payload, bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		ctx->last_d2h += bytes;
+	}
+	CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+	cudaEventElapsedTime(&ctx->last_kernel_ms, ctx->ev0, ctx->ev1);
+	return ASTCENC_SUCCESS;
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

@@ -236,6 +236,41 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device_blocks(struct ast
                                                                       unsigned int dim_x, unsigned int dim_y, unsigned int dim_z, const struct astcenc_swizzle* swizzle,
                                                                       const uint32_t* block_indices, unsigned int block_count, uint8_t* d_payload, void* cuda_stream);
 
+/* Compress many images - the levels of a mip chain, a set of small textures - in shared pipeline passes: for callers whose
+ * images are small, each of which would otherwise pay the fixed cost of a pass of its own (a few milliseconds, whatever the
+ * image's size).
+ *  - astcenc_b200_compress_device_images: images[i] describes an image ALREADY RESIDENT in device memory (data: dim_z slices
+ *    of dim_x * dim_y texels, contiguous) and its device payload. Every block of every image is written to that image's
+ *    payload, in astcenc_compress_image's order, and the bytes are those astcenc_compress_image writes for the image alone.
+ *    Images may differ in size and take the shapes astcenc_compress_image takes: 2D images, texture arrays (2D block size,
+ *    dim_z > 1) and volumes of 3D block sizes. All share data_type and swizzle. Payloads must not overlap (not checked). The
+ *    descriptor array is copied: the caller may free it when the call returns. Enqueued on `cuda_stream` (0 = the context's
+ *    own stream), without synchronising, in order with every other pass of the context (see above). No progress callback, no
+ *    cancellation.
+ *  - astcenc_b200_compress_images: the host-pointer twin. Every image goes up into one device buffer, the device path runs on
+ *    the context's stream, payload i is copied into data_out[i] (data_len[i] bytes, which must hold it), and the call returns
+ *    when that is done. All images must have the same data_type. astcenc_b200_last_timing() reports its device time and its
+ *    H2D / D2H bytes. It uses the context's host-path buffers: one host-pointer call at a time per context.
+ *  - Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_CONTEXT for a decompress-only
+ *    context; ASTCENC_ERR_BAD_PARAM for a NULL swizzle, then ASTCENC_ERR_BAD_SWIZZLE; ASTCENC_ERR_BAD_PARAM for images == NULL
+ *    with a non-zero count, a NULL data, payload or output pointer, a zero dimension, a bad data type or (host entry) mixed
+ *    data types; ASTCENC_ERR_NOT_IMPLEMENTED for a_scale_radius on a texture array; ASTCENC_ERR_BAD_PARAM when the block count
+ *    of an image (2^32 blocks or more) or of the whole call overflows; (host entry) ASTCENC_ERR_OUT_OF_MEM when a data_len[i]
+ *    is too short. All images are checked before anything is enqueued. image_count == 0 does nothing.
+ * The images' blocks are gathered, in call order, into staging rows of at most ASTCENC_B200_BATCH_BLOCKS blocks, as block lists
+ * are: one ordinary pass per staging row, which may span several images, then a scatter to each image's payload. With
+ * a_scale_radius (2D block sizes) each image gets its own alpha-scale pre-pass over the whole image: one extra launch per image. */
+struct astcenc_b200_device_image {
+	const void* data;              /* device: dim_z slices of dim_x * dim_y texels, contiguous */
+	unsigned int dim_x, dim_y, dim_z;
+	uint8_t* payload;              /* device: the image's whole payload, astcenc_compress_image's block order */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device_images(struct astcenc_context* context, const struct astcenc_b200_device_image* images,
+                                                                      unsigned int image_count, enum astcenc_type data_type, const struct astcenc_swizzle* swizzle,
+                                                                      void* cuda_stream);
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_images(struct astcenc_context* context, struct astcenc_image* const* images, unsigned int image_count,
+                                                               const struct astcenc_swizzle* swizzle, uint8_t* const* data_out, const size_t* data_len);
+
 /**
  * Multi-GPU sharding: one process per GPU, each with its own context; the only exchange is the gather of the compressed
  * payload over NCCL (loaded at run time: "libnccl.so.2"; ASTCENC_ERR_NOT_IMPLEMENTED when it cannot be loaded).
@@ -283,7 +318,7 @@ ASTCENC_PUBLIC unsigned long long astcenc_b200_launch_count(struct astcenc_conte
 ASTCENC_PUBLIC enum astcenc_error astcenc_b200_stage_timing(struct astcenc_context* context, int enable, float stage_ms[4], unsigned int stage_launches[4]);
 
 /* Milliseconds of device time (CUDA events on the launching stream) spent in the compress kernel by the most
- * recent astcenc_compress_image() call on this context, and its H2D / D2H byte counts. */
+ * recent astcenc_compress_image() or astcenc_b200_compress_images() call on this context, and its H2D / D2H byte counts. */
 ASTCENC_PUBLIC enum astcenc_error astcenc_b200_last_timing(struct astcenc_context* context, float* kernel_ms, size_t* h2d_bytes, size_t* d2h_bytes);
 
 /**

@@ -67,6 +67,11 @@ class DeviceImage(C.Structure):
     _fields_ = [("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("payload", C.c_void_p)]
 
 
+class DeviceDecodeImage(C.Structure):
+    """struct astcenc_b200_device_decode_image (include/astcenc.h)."""
+    _fields_ = [("payload", C.c_void_p), ("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint)]
+
+
 class ErrorMetrics(C.Structure):
     """struct astcenc_b200_error_metrics (include/astcenc.h)."""
     _fields_ = [(n, C.c_double) for n in ("psnr", "alpha_psnr", "rgb_psnr", "rgb_peak", "peak_psnr", "mpsnr", "log_rmse",
@@ -124,6 +129,8 @@ def lib():
         l.astcenc_b200_compress_images.argtypes = [C.c_void_p, C.POINTER(C.POINTER(Image)), C.c_uint, C.POINTER(Swizzle), C.POINTER(C.c_void_p),
                                                    C.POINTER(C.c_size_t)]
         l.astcenc_b200_compress_images.restype = C.c_int
+        l.astcenc_b200_decompress_device_images.argtypes = [C.c_void_p, C.POINTER(DeviceDecodeImage), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
+        l.astcenc_b200_decompress_device_images.restype = C.c_int
         l.astcenc_b200_launch_count.argtypes = [C.c_void_p]
         l.astcenc_b200_launch_count.restype = C.c_ulonglong
         l.astcenc_b200_last_timing.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
@@ -313,6 +320,18 @@ class Context:
         if err:
             raise AstcencError(err, "astcenc_b200_compress_images")
         return outs
+
+    def decompress_device_images(self, images, data_type, swizzle=(0, 1, 2, 3), stream=0):
+        """Many device-resident payloads into device images in one launch (astcenc_b200_decompress_device_images). images: a
+        sequence of (d_payload_ptr, d_image_ptr, dim_x, dim_y, dim_z); every image receives the texels decompress_image gives
+        for its payload alone. Enqueued on `stream`, no sync; works on decompress-only contexts."""
+        n = len(images)
+        table = (DeviceDecodeImage * n)(*[DeviceDecodeImage(C.c_void_p(p), C.c_void_p(d), x, y, z) for p, d, x, y, z in images])
+        sw = Swizzle(*swizzle) if swizzle is not None else None
+        err = lib().astcenc_b200_decompress_device_images(self.handle, table if n else None, n, data_type, C.byref(sw) if sw is not None else None,
+                                                          C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_decompress_device_images")
 
     def launch_count(self):
         return int(lib().astcenc_b200_launch_count(self.handle))

@@ -235,7 +235,16 @@ ASTC_FN float decode_component(int v, bool lns) {   // decode_texel :66-87
 	return sf16_to_float((uint16_t)sf);
 }
 
-// store one texel (store_image_block); swz uses astcenc_swz numbering (4 = 0, 5 = 1, 6 = Z)
+// n bytes from src to dst, one at a time (an output that starts at any byte)
+ASTC_FN void store_bytes(uint8_t* dst, const uint8_t* src, int n) {
+	for (int k = 0; k < n; k++) {
+		dst[k] = src[k];
+	}
+}
+
+// store one texel (store_image_block); swz uses astcenc_swz numbering (4 = 0, 5 = 1, 6 = Z). ANY_ALIGN: img.data may start at
+// any byte (decode calls over image tables), and a texel that is not aligned to its components is stored byte by byte.
+template <bool ANY_ALIGN>
 ASTC_FN void store_texel(const DevImage& img, unsigned int x, unsigned int y, unsigned int z, f4 d) {
 	bool needs_swz = img.swz[0] != 0 || img.swz[1] != 1 || img.swz[2] != 2 || img.swz[3] != 3;
 	bool needs_z = img.swz[0] == 6 || img.swz[1] == 6 || img.swz[2] == 6 || img.swz[3] == 6;
@@ -265,7 +274,12 @@ ASTC_FN void store_texel(const DevImage& img, unsigned int x, unsigned int y, un
 			o0 = 0xFF; o1 = 0x00; o2 = 0xFF; o3 = 0xFF;
 		}
 		uint32_t px = (uint32_t)(o0 & 0xFF) | ((uint32_t)(o1 & 0xFF) << 8) | ((uint32_t)(o2 & 0xFF) << 16) | ((uint32_t)(o3 & 0xFF) << 24);
-		*reinterpret_cast<uint32_t*>(static_cast<uint8_t*>(base) + o) = px;
+		uint8_t* dst = static_cast<uint8_t*>(base) + o;
+		if (ANY_ALIGN && (reinterpret_cast<uintptr_t>(dst) & 3) != 0) {
+			store_bytes(dst, reinterpret_cast<const uint8_t*>(&px), 4);
+		} else {
+			*reinterpret_cast<uint32_t*>(dst) = px;
+		}
 		return;
 	}
 	f4 ov = d;
@@ -294,12 +308,22 @@ ASTC_FN void store_texel(const DevImage& img, unsigned int x, unsigned int y, un
 	}
 	if (img.data_type == 1) {
 		uint16_t* p = static_cast<uint16_t*>(base) + o;
+		if (ANY_ALIGN && (reinterpret_cast<uintptr_t>(p) & 1) != 0) {
+			const uint16_t h[4] = {float_to_sf16(ov.x), float_to_sf16(ov.y), float_to_sf16(ov.z), float_to_sf16(ov.w)};
+			store_bytes(reinterpret_cast<uint8_t*>(p), reinterpret_cast<const uint8_t*>(h), 8);
+			return;
+		}
 		p[0] = float_to_sf16(ov.x);
 		p[1] = float_to_sf16(ov.y);
 		p[2] = float_to_sf16(ov.z);
 		p[3] = float_to_sf16(ov.w);
 	} else {
 		float* p = static_cast<float*>(base) + o;
+		if (ANY_ALIGN && (reinterpret_cast<uintptr_t>(p) & 3) != 0) {
+			const float f[4] = {ov.x, ov.y, ov.z, ov.w};
+			store_bytes(reinterpret_cast<uint8_t*>(p), reinterpret_cast<const uint8_t*>(f), 16);
+			return;
+		}
 		p[0] = ov.x;
 		p[1] = ov.y;
 		p[2] = ov.z;
@@ -307,7 +331,8 @@ ASTC_FN void store_texel(const DevImage& img, unsigned int x, unsigned int y, un
 	}
 }
 
-// Decompress block (bx_i, by_i) of the image described by IMG (IMG.data = output image, IMG.out unused).
+// Decompress block (bx_i, by_i) of the image described by IMG (IMG.data = output image, IMG.out unused). ANY_ALIGN: see store_texel.
+template <bool ANY_ALIGN = false>
 ASTC_COOP void decompress_block(int lane, uint32_t slice, const uint8_t* pcb, unsigned int bx_i, unsigned int by_i) {
 	const DevImage& img = IMG;
 	int T = BSD.texel_count;
@@ -358,7 +383,7 @@ ASTC_COOP void decompress_block(int lane, uint32_t slice, const uint8_t* pcb, un
 			unsigned int tyz = (unsigned int)t / bdx, tz = volume ? tyz / BSD.dim_y : 0u;
 			unsigned int x = pos_x + (unsigned int)t % bdx, y = pos_y + tyz - tz * BSD.dim_y, z = pos_z + tz;
 			if (x < img.dim_x && y < img.dim_y && z < lim_z) {
-				store_texel(img, x, y, z, c);
+				store_texel<ANY_ALIGN>(img, x, y, z, c);
 			}
 		}
 		wsync();
@@ -413,7 +438,7 @@ ASTC_COOP void decompress_block(int lane, uint32_t slice, const uint8_t* pcb, un
 		unsigned int tyz = (unsigned int)t / bdx, tz = volume ? tyz / BSD.dim_y : 0u;
 		unsigned int x = pos_x + (unsigned int)t % bdx, y = pos_y + tyz - tz * BSD.dim_y, z = pos_z + tz;
 		if (x < img.dim_x && y < img.dim_y && z < lim_z) {
-			store_texel(img, x, y, z, d);
+			store_texel<ANY_ALIGN>(img, x, y, z, d);
 		}
 	}
 	wsync();

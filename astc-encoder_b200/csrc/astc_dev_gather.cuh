@@ -12,6 +12,9 @@
 // is block c - first[j] of image j, where first[] is the exclusive prefix sum of the images' block counts in call order; the
 // gather and the scatter find j by binary search over first[]. A chunk of the call (GatherArgs::base) may span several images,
 // and an image several chunks.
+//
+// A decode call (astcenc_b200_decompress_device_images) walks the same kind of table: each entry's payload is read and its data
+// written.
 #pragma once
 
 // One image of an image table.
@@ -69,20 +72,24 @@ ASTC_FN GatherTexel gather_texel(const GatherArgs& g, unsigned int i, uint32_t i
 	return r;
 }
 
-// The table entry that holds staging block i: the last image whose first block is at or before call block base + i (every image
-// has at least one block, so there is exactly one).
-ASTC_FN unsigned int table_image(const GatherArgs& g, unsigned int i) {
-	const size_t c = g.base + i;
-	unsigned int lo = 0, hi = g.image_count - 1;
+// The table entry that holds call block c: the last image whose first block is at or before c (every image has at least one
+// block, so there is exactly one).
+ASTC_FN unsigned int find_image(const GatherImage* images, unsigned int image_count, size_t c) {
+	unsigned int lo = 0, hi = image_count - 1;
 	while (lo < hi) {
 		unsigned int mid = (lo + hi + 1) / 2;
-		if (g.images[mid].first <= c) {
+		if (images[mid].first <= c) {
 			lo = mid;
 		} else {
 			hi = mid - 1;
 		}
 	}
 	return lo;
+}
+
+// The table entry that holds staging block i.
+ASTC_FN unsigned int table_image(const GatherArgs& g, unsigned int i) {
+	return find_image(g.images, g.image_count, g.base + i);
 }
 
 // Block `index` of the source described by g into staging block i, by the lanes of one warp (lane / lanes): the texels word by
@@ -130,4 +137,42 @@ ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i, uint8_t* pa
 	}
 	const GatherImage& im = g.images[table_image(g, i)];
 	return im.payload + (g.base + i - im.first) * 16;
+}
+
+// ---- image tables of a decode call (astc_decompress_images_kernel) ----
+// Call block c is block c - first[j] of image j, found by find_image. decompress_block reads its image from the CTA's launch
+// constants (IMG), so a CTA decodes its blocks one plane at a time and restages IMG between planes behind a barrier. A plane is
+// an image of a 3D block size (its blocks count layer * blocks_y + row) or one slice of an image of a 2D block size (a texture
+// array's combined row slice * blocks_y + row, with IMG.data at the slice).
+//
+// Call blocks [c0, c1) by the `warps` warps of one CTA; this is warp `warp` (the host simulation runs warp 0 of 1). On entry IMG
+// holds the call's data type and swizzle; its pointer and dimensions are restaged here.
+ASTC_FN void decode_table_blocks(const GatherImage* images, unsigned int image_count, size_t c0, size_t c1, int warp, int warps, int lane,
+                                 uint32_t slice) {
+	DevImage& img = reinterpret_cast<SmemHdr*>(astc_smem)->img;
+	const unsigned int bz = BSD.dim_z;
+	const size_t texel_bytes = img.data_type == 0 ? 4 : img.data_type == 1 ? 8 : 16;
+	for (size_t c = c0; c < c1;) {
+		const GatherImage& im = images[find_image(images, image_count, c)];
+		const size_t plane_blocks = (size_t)im.blocks_x * im.blocks_y * (bz > 1 ? (im.dim_z + bz - 1) / bz : 1);
+		const size_t plane = (c - im.first) / plane_blocks;
+		const size_t p0 = im.first + plane * plane_blocks;
+		const size_t end = p0 + plane_blocks < c1 ? p0 + plane_blocks : c1;
+		cta_sync();      // every warp is done with the previous plane
+		if (warp == 0 && lane == 0) {
+			img.data = static_cast<const uint8_t*>(im.data) + plane * (size_t)im.dim_x * im.dim_y * texel_bytes;
+			img.dim_x = im.dim_x;
+			img.dim_y = im.dim_y;
+			img.dim_z = bz > 1 ? im.dim_z : 1;
+			img.blocks_x = im.blocks_x;
+			img.blocks_y = im.blocks_y;
+		}
+		cta_sync();
+		for (size_t b = c + (size_t)warp; b < end; b += (size_t)warps) {
+			const unsigned int k = (unsigned int)(b - p0);      // (a plane has fewer than 2^32 blocks)
+			const unsigned int by = k / im.blocks_x;
+			decompress_block<true>(lane, slice, im.payload + (b - im.first) * 16, k - by * im.blocks_x, by);
+		}
+		c = end;
+	}
 }

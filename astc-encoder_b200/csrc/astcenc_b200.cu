@@ -251,6 +251,19 @@ astc_decompress_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant
 	}
 }
 
+// ---- decode calls over image tables (astcenc_b200_decompress_device_images): one warp per block, each CTA over a contiguous
+// share of the call's blocks; img carries the call's data type and swizzle ----
+__global__ void __launch_bounds__(ASTC_DECODE_THREADS, 2)
+astc_decompress_images_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
+                              const GatherImage* __restrict__ images, unsigned int image_count, size_t total) {
+	stage_launch_constants(bsd, cfg, img);
+	const size_t per = (total + gridDim.x - 1) / gridDim.x;
+	const size_t c0 = blockIdx.x * per;
+	const size_t c1 = c0 + per < total ? c0 + per : total;
+	decode_table_blocks(images, image_count, c0, c1, (int)(threadIdx.x >> 5), (int)(blockDim.x >> 5), (int)(threadIdx.x & 31),
+	                    ASTC_SMEM_HDR + (threadIdx.x >> 5) * D_SLICE);
+}
+
 __global__ void __launch_bounds__(32, 1)
 astc_block_info_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
                        unsigned long long lo, unsigned long long hi, DevBlockInfo* out) {
@@ -1936,6 +1949,76 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 	}
 	CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	cudaEventElapsedTime(&ctx->last_kernel_ms, ctx->ev0, ctx->ev1);
+	return ASTCENC_SUCCESS;
+}
+
+// Decode calls: every image is checked before anything is enqueued; the table goes up in one copy and one launch decodes every
+// block of the call. The launch takes the context's table buffer (ctx->list), so it is a turn of the scratch like any pass
+// (launch_mtx, scratch_done).
+astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const astcenc_b200_device_decode_image* images, unsigned int image_count,
+                                                    astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
+	astcenc_error status = swizzle ? validate_decompression_swizzle(*swizzle) : ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS && image_count != 0 && !images) status = ASTCENC_ERR_BAD_PARAM;
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
+		if (!images[i].payload || !images[i].data) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		} else {
+			status = check_texel_count(images[i].dim_x, images[i].dim_y, images[i].dim_z);
+		}
+	}
+	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
+	if (status != ASTCENC_SUCCESS) {
+		return status;
+	}
+	std::vector<GatherImage> table(image_count);
+	size_t blocks = 0;
+	for (unsigned int i = 0; i < image_count; i++) {
+		const astcenc_b200_device_decode_image& im = images[i];
+		const SlabGeometry geo = slab_geometry(ctx, im.dim_x, im.dim_y, im.dim_z, (int)data_type);
+		if (geo.payload_overflow() || geo.blocks > 0xFFFFFFFFu || geo.blocks > SIZE_MAX - blocks) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		GatherImage& e = table[i];
+		e.data = im.data;
+		e.payload = const_cast<uint8_t*>(im.payload);      // (read, never written)
+		e.first = blocks;
+		e.avg_offset = 0;
+		e.dim_x = im.dim_x;
+		e.dim_y = im.dim_y;
+		e.dim_z = im.dim_z;
+		e.blocks_x = (unsigned int)geo.blocks_x;
+		e.blocks_y = (unsigned int)geo.blocks_y;
+		blocks += geo.blocks;
+	}
+	if (image_count == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	int sms = 0;
+	CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device), return ASTCENC_ERR_BAD_CONTEXT);
+	const unsigned int warps = ASTC_DECODE_THREADS / 32;
+	const size_t ctas = (blocks + warps - 1) / warps;
+	const unsigned int grid = ctas < (size_t)sms * 8 ? (unsigned int)ctas : (unsigned int)sms * 8;
+	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
+	if (ctx->scratch_used) {
+		CUDA_TRY(cudaStreamWaitEvent(s, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
+	}
+	astcenc_error st = ensure_buffer(ctx->list, table.size() * sizeof(GatherImage));
+	if (st != ASTCENC_SUCCESS) {
+		return st;
+	}
+	// (from pageable memory: staged by the driver before the call returns)
+	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, table.data(), table.size() * sizeof(GatherImage), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+	astc_decompress_images_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, s>>>(
+	    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, (int)data_type, 0, 0, 0, *swizzle), ctx->list.as<const GatherImage>(), image_count, blocks);
+	ctx->launches++;
+	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+	CUDA_TRY(cudaEventRecord(ctx->scratch_done, s), return ASTCENC_ERR_BAD_CONTEXT);
+	ctx->scratch_used = true;
 	return ASTCENC_SUCCESS;
 }
 

@@ -272,6 +272,32 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_images(struct astcenc_co
                                                                const struct astcenc_swizzle* swizzle, uint8_t* const* data_out, const size_t* data_len);
 
 /**
+ * Device-resident decompression of many images in one launch, such as the levels of a mip chain or a set of textures.
+ * images[i] describes a payload ALREADY RESIDENT in device memory (astcenc_compress_image's block order, 16 bytes per block) and
+ * the device image it decodes into (dim_z slices of dim_x * dim_y texels of data_type, contiguous). Image i's data receives
+ * exactly the texels astcenc_decompress_image writes for payload i alone, with the same data_type and swizzle: Z
+ * reconstruction, the error colour of illegal blocks and the F16 void-extent behaviour included. Images may differ in size and
+ * take the shapes astcenc_decompress_image takes: 2D images, texture arrays (2D block size, dim_z > 1) and volumes of 3D block
+ * sizes. Outputs must not overlap each other or any payload (not checked); they need no alignment. The descriptor array is
+ * copied: the caller may free it when the call returns. Enqueued on `cuda_stream` (0 = the context's own stream), without
+ * synchronising, in order with every other pass of the context. Works on decompress-only contexts. No progress callback, no
+ * cancellation. A single image is a call with image_count == 1.
+ * Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_PARAM for a NULL swizzle, then
+ * ASTCENC_ERR_BAD_SWIZZLE (r, g, b, a, 0, 1 and Z are allowed); ASTCENC_ERR_BAD_PARAM for images == NULL with a non-zero count, a
+ * NULL payload or data pointer, a zero dimension or a bad data type; ASTCENC_ERR_BAD_PARAM when the block count of an image
+ * (2^32 blocks or more) or of the whole call overflows. All images are checked before anything is enqueued. image_count == 0
+ * does nothing. The call's table goes up in one small copy and every block of the call is decoded by one kernel launch.
+ */
+struct astcenc_b200_device_decode_image {
+	const uint8_t* payload;        /* device: the image's whole payload, astcenc_compress_image's block order */
+	void* data;                    /* device: dim_z slices of dim_x * dim_y texels of data_type, contiguous */
+	unsigned int dim_x, dim_y, dim_z;
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_decompress_device_images(struct astcenc_context* context, const struct astcenc_b200_device_decode_image* images,
+                                                                        unsigned int image_count, enum astcenc_type data_type,
+                                                                        const struct astcenc_swizzle* swizzle, void* cuda_stream);
+
+/**
  * Multi-GPU sharding: one process per GPU, each with its own context; the only exchange is the gather of the compressed
  * payload over NCCL (loaded at run time: "libnccl.so.2"; ASTCENC_ERR_NOT_IMPLEMENTED when it cannot be loaded).
  * The reference has no counterpart - its unit of distribution is the block ticket of one process

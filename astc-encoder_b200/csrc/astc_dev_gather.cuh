@@ -171,7 +171,7 @@ ASTC_FN void decode_table_blocks(const GatherImage* images, unsigned int image_c
 		for (size_t b = c + (size_t)warp; b < end; b += (size_t)warps) {
 			const unsigned int k = (unsigned int)(b - p0);      // (a plane has fewer than 2^32 blocks)
 			const unsigned int by = k / im.blocks_x;
-			decompress_block<true>(lane, slice, im.payload + (b - im.first) * 16, k - by * im.blocks_x, by);
+			decompress_block(lane, slice, im.payload + (b - im.first) * 16, k - by * im.blocks_x, by);
 		}
 		c = end;
 	}

@@ -235,24 +235,9 @@ astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_cons
 	}
 }
 
-// ---- decompression (SURVEY.md section 8f): one warp per block, grid-stride ----
+// ---- decompression (SURVEY.md section 8f) over image tables (astcenc_decompress_image, astcenc_b200_decompress_device_images):
+// one warp per block, each CTA over a contiguous share of the call's blocks; img carries the call's data type and swizzle ----
 #define ASTC_DECODE_THREADS 256
-__global__ void __launch_bounds__(ASTC_DECODE_THREADS, 2)
-astc_decompress_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
-                       const uint8_t* __restrict__ blocks, unsigned int block_count) {
-	stage_launch_constants(bsd, cfg, img);
-	const int lane = threadIdx.x & 31;
-	const unsigned int warps_per_cta = blockDim.x >> 5;
-	const uint32_t slice = ASTC_SMEM_HDR + (threadIdx.x >> 5) * D_SLICE;
-	for (unsigned int b = blockIdx.x * warps_per_cta + (threadIdx.x >> 5); b < block_count; b += gridDim.x * warps_per_cta) {
-		unsigned int by = b / img.blocks_x;
-		unsigned int bx = b - by * img.blocks_x;
-		decompress_block(lane, slice, blocks + (size_t)b * 16, bx, by);
-	}
-}
-
-// ---- decode calls over image tables (astcenc_b200_decompress_device_images): one warp per block, each CTA over a contiguous
-// share of the call's blocks; img carries the call's data type and swizzle ----
 __global__ void __launch_bounds__(ASTC_DECODE_THREADS, 2)
 astc_decompress_images_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
                               const GatherImage* __restrict__ images, unsigned int image_count, size_t total) {
@@ -425,11 +410,13 @@ struct astcenc_context {
 	// block lists (astcenc_b200_compress_device_blocks), grown on demand: the list, the staging image and payload of one chunk,
 	// the pre-pass averages of the source image
 	DevBuffer list, list_image, list_out, list_alpha;
-	// The per-context scratch (records, queues, counters, alpha averages) serves ONE pipeline pass at a time: launch_mtx
-	// serialises the host side, scratch_done orders a pass on one stream behind the previous pass on another.
+	// The per-context scratch (records, queues, counters, alpha averages, table and staging buffers) serves ONE pass at a time
+	// (scratch_turn): launch_mtx serialises the host side, scratch_done orders a pass on one stream behind the previous pass on
+	// another.
 	std::mutex launch_mtx;
 	cudaEvent_t scratch_done = nullptr;
 	bool scratch_used = false;
+	int sm_count = 0;            // the device's SMs (grids of the decode and pipeline launches)
 	// host-pointer path: uploads run on copy_stream, band by band, under the set-up of the previous band
 	cudaStream_t copy_stream = nullptr;
 	cudaEvent_t band_ready[ASTC_MAX_BANDS] = {};
@@ -479,6 +466,29 @@ static astcenc_error run_once(astcenc_context* ctx, CallerGate& gate, F work) {
 	}
 	ctx->cv.wait(lk, [&gate] { return gate.state == 2; });
 	return gate.result;
+}
+
+// Orders `stream` behind the last turn of the scratch (a no-op when that ran on the same stream). Under launch_mtx.
+static astcenc_error wait_for_scratch(astcenc_context* ctx, cudaStream_t stream) {
+	if (ctx->scratch_used) {
+		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
+	}
+	return ASTCENC_SUCCESS;
+}
+
+// One turn of the context's scratch: `work` enqueues a pass on `stream`. Calls may come from several host threads and on
+// different streams: launch_mtx serialises the enqueueing, the pass starts behind the event that closed the previous turn, and
+// every exit records that event behind this one. Returns the first error.
+template <typename F>
+static astcenc_error scratch_turn(astcenc_context* ctx, cudaStream_t stream, F work) {
+	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
+	astcenc_error st = wait_for_scratch(ctx, stream);
+	if (st == ASTCENC_SUCCESS) {
+		st = work();
+	}
+	CUDA_TRY(cudaEventRecord(ctx->scratch_done, stream), return st != ASTCENC_SUCCESS ? st : ASTCENC_ERR_BAD_CONTEXT);
+	ctx->scratch_used = true;
+	return st;
 }
 
 static std::mutex g_const_mtx;
@@ -574,11 +584,12 @@ astcenc_error astcenc_context_alloc(const astcenc_config* configp, unsigned int 
 		t->bsd_1p = pk.bsd_1p;
 	}
 	astc_host::make_device_config(cfg, ctx->dcfg);
+	CUDA_TRY(cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
 
 	if (!(cfg.flags & ASTCENC_FLG_DECOMPRESS_ONLY)) {
 		cudaDeviceProp prop;
 		CUDA_TRY(cudaGetDeviceProperties(&prop, device), ALLOC_FAIL(ASTCENC_ERR_BAD_CONTEXT));
-		status = plan_kernels(ctx->tables->bsd, ctx->tables->bsd_1p, cfg, prop.sharedMemPerBlockOptin, prop.multiProcessorCount, ctx->knobs, ctx->plan);
+		status = plan_kernels(ctx->tables->bsd, ctx->tables->bsd_1p, cfg, prop.sharedMemPerBlockOptin, ctx->sm_count, ctx->knobs, ctx->plan);
 		if (status != ASTCENC_SUCCESS) {
 			ALLOC_FAIL(status);
 		}
@@ -675,10 +686,12 @@ void astcenc_context_free(astcenc_context* ctx) {
 	delete ctx;
 }
 
-static astcenc_error validate_compression_swizzle(const astcenc_swizzle& s) {
+// Every component a selector from ASTCENC_SWZ_R to `highest`: ASTCENC_SWZ_1 for compression, ASTCENC_SWZ_Z for decompression
+// (astcenc_entry.cpp:279-300).
+static astcenc_error check_swizzle(const astcenc_swizzle& s, astcenc_swz highest) {
 	const int v[4] = {(int)s.r, (int)s.g, (int)s.b, (int)s.a};
 	for (int i = 0; i < 4; i++) {
-		if (v[i] < ASTCENC_SWZ_R || v[i] > ASTCENC_SWZ_1) {
+		if (v[i] < ASTCENC_SWZ_R || v[i] > (int)highest) {
 			return ASTCENC_ERR_BAD_SWIZZLE;
 		}
 	}
@@ -689,6 +702,10 @@ static size_t mul_safe(size_t a, size_t b, bool& overflow) {
 	size_t r = a * b;
 	overflow = overflow || ((b != 0) && ((r / b) != a));
 	return r;
+}
+
+static size_t texel_bytes(int data_type) {
+	return data_type == ASTCENC_TYPE_U8 ? 4 : data_type == ASTCENC_TYPE_F16 ? 8 : 16;
 }
 
 static size_t block_count_axis(size_t dim, size_t blk) {
@@ -730,7 +747,7 @@ static SlabGeometry slab_geometry(const astcenc_context* ctx, unsigned int dim_x
 	g.overflow = false;
 	g.blocks = mul_safe(mul_safe(g.blocks_x, g.blocks_y, g.overflow), g.layers, g.overflow);
 	g.row_out = g.blocks_x * 16;
-	g.texel_bytes = data_type == ASTCENC_TYPE_U8 ? 4 : data_type == ASTCENC_TYPE_F16 ? 8 : 16;
+	g.texel_bytes = texel_bytes(data_type);
 	g.slice_bytes = (size_t)dim_x * dim_y * g.texel_bytes;
 	return g;
 }
@@ -1093,9 +1110,12 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const DevImage& sr
 	                 blocks_x * block_rows >= (size_t)pipes * 8192;
 	// banded uploads need the whole slab in one batch on the wave pipeline, and no pre-pass that reads the window first
 	bool banded = up != nullptr && radius == 0 && ctx->plan.driver == 0 && single_batch && (use_pipes || (up->bands > 1 && block_rows >= (unsigned int)up->bands * 4));
-	if (up != nullptr && ctx->scratch_used) {
+	if (up != nullptr) {
 		// the upload streams on the copy stream; it must not overtake a pass that still reads the image buffer
-		CUDA_TRY(cudaStreamWaitEvent(ctx->copy_stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
+		astcenc_error st = wait_for_scratch(ctx, ctx->copy_stream);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
 	}
 	if (up != nullptr && !banded) {
 		size_t y0, y1;
@@ -1141,19 +1161,9 @@ static astcenc_error launch_slab_locked(astcenc_context* ctx, const DevImage& sr
 	return ASTCENC_SUCCESS;
 }
 
-// The context's scratch buffers serve one pass at a time. Calls may come from several host threads and on different
-// streams: launch_mtx serialises the enqueueing, and every pass starts by making its stream wait for the event that
-// closes the previous pass (a no-op when both ran on the same stream).
 static astcenc_error launch_slab(astcenc_context* ctx, const DevImage& src, unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, cudaStream_t stream,
                                  const UploadPlan* up = nullptr) {
-	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
-	if (ctx->scratch_used) {
-		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
-	}
-	astcenc_error st = launch_slab_locked(ctx, src, block_row0, block_rows, d_out, stream, up);
-	CUDA_TRY(cudaEventRecord(ctx->scratch_done, stream), return ASTCENC_ERR_BAD_CONTEXT);
-	ctx->scratch_used = true;
-	return st;
+	return scratch_turn(ctx, stream, [&] { return launch_slab_locked(ctx, src, block_row0, block_rows, d_out, stream, up); });
 }
 
 // Progress of one astcenc_compress_image call, reported like the reference's task pool (astcenc_internal_entry.h:199-295):
@@ -1280,7 +1290,7 @@ astcenc_error astcenc_compress_reset(astcenc_context* ctx);
 astcenc_error astcenc_compress_image(astcenc_context* ctx, astcenc_image* imagep, const astcenc_swizzle* swizzle, uint8_t* data_out, size_t data_len,
                                      unsigned int thread_index) {
 	astcenc_error status = check_compress_context(ctx);
-	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
 	if (status == ASTCENC_SUCCESS && thread_index >= ctx->thread_count) status = ASTCENC_ERR_BAD_PARAM;
 	if (status != ASTCENC_SUCCESS) {
 		return status;
@@ -1334,66 +1344,80 @@ astcenc_error astcenc_compress_cancel(astcenc_context* ctx) {
 	return ASTCENC_SUCCESS;
 }
 
-static astcenc_error validate_decompression_swizzle(const astcenc_swizzle& s) {   // astcenc_entry.cpp:279-300: r,g,b,a,0,1 and Z
-	const int v[4] = {(int)s.r, (int)s.g, (int)s.b, (int)s.a};
-	for (int i = 0; i < 4; i++) {
-		if (v[i] < ASTCENC_SWZ_R || v[i] > ASTCENC_SWZ_Z) {
-			return ASTCENC_ERR_BAD_SWIZZLE;
-		}
+// Entry e of an image table: dim_z slices of dim_x * dim_y texels of `data_type` at `data`, its payload at `payload`, call blocks
+// [first, first + its blocks). Advances `first`. ASTCENC_ERR_BAD_PARAM when the image's payload does not fit a size_t, the image
+// has 2^32 blocks or more (the table walks index an image's blocks with 32 bits, as block lists do) or the call's total does
+// not fit a size_t.
+static astcenc_error table_entry(const astcenc_context* ctx, int data_type, unsigned int dim_x, unsigned int dim_y, unsigned int dim_z, const void* data,
+                                 uint8_t* payload, size_t& first, GatherImage& e) {
+	const SlabGeometry geo = slab_geometry(ctx, dim_x, dim_y, dim_z, data_type);
+	if (geo.payload_overflow() || geo.blocks > 0xFFFFFFFFu || geo.blocks > SIZE_MAX - first) {
+		return ASTCENC_ERR_BAD_PARAM;
 	}
+	e.data = data;
+	e.payload = payload;
+	e.first = first;
+	e.avg_offset = 0;
+	e.dim_x = dim_x;
+	e.dim_y = dim_y;
+	e.dim_z = dim_z;
+	e.blocks_x = (unsigned int)geo.blocks_x;
+	e.blocks_y = (unsigned int)geo.blocks_y;
+	first += geo.blocks;
 	return ASTCENC_SUCCESS;
 }
 
+// One launch decodes the `blocks` call blocks of an image table on `stream` (inside a scratch turn: the table goes up into the
+// context's table buffer, ctx->list).
+static astcenc_error launch_decode(astcenc_context* ctx, const GatherImage* table, unsigned int image_count, size_t blocks, int data_type,
+                                   const astcenc_swizzle& swizzle, cudaStream_t stream) {
+	astcenc_error st = ensure_buffer(ctx->list, image_count * sizeof(GatherImage));
+	if (st != ASTCENC_SUCCESS) {
+		return st;
+	}
+	// (from pageable memory: staged by the driver before the call returns)
+	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, table, image_count * sizeof(GatherImage), cudaMemcpyHostToDevice, stream), return ASTCENC_ERR_BAD_CONTEXT);
+	const unsigned int warps = ASTC_DECODE_THREADS / 32;
+	const size_t ctas = (blocks + warps - 1) / warps;
+	const unsigned int grid = ctas < (size_t)ctx->sm_count * 8 ? (unsigned int)ctas : (unsigned int)ctx->sm_count * 8;
+	astc_decompress_images_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, stream>>>(
+	    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, data_type, 0, 0, 0, swizzle), ctx->list.as<const GatherImage>(), image_count, blocks);
+	ctx->launches++;
+	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+	return ASTCENC_SUCCESS;
+}
+
+// The host-pointer twin of astcenc_b200_decompress_device_images: the whole payload goes up into ctx->out, a one-entry table
+// points it at ctx->image (the image's dim_z slices: an array, or the volume of a 3D block size), one launch decodes it and each
+// slice comes back into image.data[z]. The buffers are shared with the compression path: everything up to the copies back is
+// one scratch turn, and the call waits for them outside it.
 static astcenc_error decompress_image_gpu(astcenc_context* ctx, const uint8_t* data, astcenc_image& image, const SlabGeometry& geo, const astcenc_swizzle& swizzle) {
-	const DevBsd& bsd = ctx->tables->bsd;
 	DeviceGuard guard(ctx->device);
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	std::lock_guard<std::mutex> launch_lock(ctx->launch_mtx);      // (shares image / out with the compression path)
-	if (ctx->scratch_used) {
-		CUDA_TRY(cudaStreamWaitEvent(ctx->stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
-	}
-	// 3D block sizes decode the volume in one pass (blocks in z, y, x order); 2D block sizes take it slice by slice
-	const size_t slice_bytes = geo.slice_bytes;
-	const size_t in_bytes = geo.pass_out_bytes();
-	astcenc_error st = ensure_buffer(ctx->image, slice_bytes * geo.pass_slices());
-	if (st == ASTCENC_SUCCESS) {
-		st = ensure_buffer(ctx->out, in_bytes);
-	}
+	astcenc_error st = scratch_turn(ctx, ctx->stream, [&]() -> astcenc_error {
+		const size_t slice_bytes = geo.slice_bytes;
+		astcenc_error r = ensure_buffer(ctx->image, slice_bytes * image.dim_z);
+		if (r == ASTCENC_SUCCESS) r = ensure_buffer(ctx->out, geo.out_bytes());
+		GatherImage e;
+		size_t blocks = 0;
+		if (r == ASTCENC_SUCCESS) r = table_entry(ctx, (int)image.data_type, image.dim_x, image.dim_y, image.dim_z, ctx->image.ptr, ctx->out.ptr, blocks, e);
+		if (r != ASTCENC_SUCCESS) {
+			return r;
+		}
+		CUDA_TRY(cudaMemcpyAsync(ctx->out.ptr, data, geo.out_bytes(), cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+		r = launch_decode(ctx, &e, 1, blocks, (int)image.data_type, swizzle, ctx->stream);
+		for (unsigned int z = 0; z < image.dim_z && r == ASTCENC_SUCCESS; z++) {
+			CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->image.ptr + (size_t)z * slice_bytes, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream),
+			         return ASTCENC_ERR_BAD_CONTEXT);
+		}
+		return r;
+	});
 	if (st != ASTCENC_SUCCESS) {
 		return st;
 	}
-	DevImage img = pass_image(ctx, ctx->image.ptr, (int)image.data_type, image.dim_x, image.dim_y, geo.pass_slices(), swizzle);
-	img.block_rows = geo.pass_rows();
-	cudaDeviceProp prop;
-	CUDA_TRY(cudaGetDeviceProperties(&prop, ctx->device), return ASTCENC_ERR_BAD_CONTEXT);
-	unsigned int nblocks = (unsigned int)(geo.blocks_x * geo.pass_rows());
-	int warps = ASTC_DECODE_THREADS / 32;
-	int grid = (int)((nblocks + warps - 1) / warps);
-	if (grid > prop.multiProcessorCount * 8) {
-		grid = prop.multiProcessorCount * 8;
-	}
-	if (geo.volume) {
-		CUDA_TRY(cudaMemcpyAsync(ctx->out.ptr, data, in_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		astc_decompress_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, ctx->stream>>>(bsd, ctx->dcfg, img, ctx->out.ptr, nblocks);
-		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
-		ctx->launches++;
-		for (unsigned int z = 0; z < image.dim_z; z++) {
-			CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->image.ptr + (size_t)z * slice_bytes, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		}
-		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		return ASTCENC_SUCCESS;
-	}
-	// 3D images with 2D blocks are an array of independent 2D slices; blocks of slice z follow those of slice z - 1
-	for (unsigned int z = 0; z < image.dim_z; z++) {
-		CUDA_TRY(cudaMemcpyAsync(ctx->out.ptr, data + (size_t)z * in_bytes, in_bytes, cudaMemcpyHostToDevice, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		astc_decompress_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, ctx->stream>>>(bsd, ctx->dcfg, img, ctx->out.ptr, nblocks);
-		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
-		ctx->launches++;
-		CUDA_TRY(cudaMemcpyAsync(image.data[z], ctx->image.ptr, slice_bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-		CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
-	}
+	CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	return ASTCENC_SUCCESS;
 }
 
@@ -1403,7 +1427,7 @@ astcenc_error astcenc_decompress_image(astcenc_context* ctx, const uint8_t* data
 	if (thread_index >= ctx->thread_count) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
-	astcenc_error status = validate_decompression_swizzle(*swizzle);
+	astcenc_error status = check_swizzle(*swizzle, ASTCENC_SWZ_Z);
 	if (status != ASTCENC_SUCCESS) {
 		return status;
 	}
@@ -1640,7 +1664,7 @@ const char* astcenc_get_error_string(astcenc_error status) {
 astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_pixels, astcenc_type data_type, unsigned int dim_x, unsigned int dim_y,
                                            const astcenc_swizzle* swizzle, unsigned int block_row0, unsigned int block_rows, uint8_t* d_out, void* cuda_stream) {
 	astcenc_error status = check_compress_context(ctx);
-	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
 	if (status != ASTCENC_SUCCESS) {
 		return status;
 	}
@@ -1680,9 +1704,9 @@ struct BlockCall {
 
 // Block lists and image tables (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk
 // (a staging row is one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most
-// knobs.batch_blocks blocks). A chunk of an image table may span several images. The whole call is one turn of the context's
-// scratch (launch_mtx, scratch_done), like a launch_slab.
-static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
+// knobs.batch_blocks blocks). A chunk of an image table may span several images. The whole call is one scratch turn
+// (launch_blocks), like a launch_slab.
+static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	const bool volume = bsd.dim_z > 1;
 	const bool table = !call.table.empty();
@@ -1693,10 +1717,6 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, 
 	size_t avg_floats = 0;
 	for (const DevImage& s : call.srcs) {
 		avg_floats += (size_t)s.dim_x * s.dim_y;
-	}
-	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
-	if (ctx->scratch_used) {
-		CUDA_TRY(cudaStreamWaitEvent(stream, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
 	}
 	const size_t list_bytes = table ? call.table.size() * sizeof(GatherImage) : n * sizeof(uint32_t);
 	astcenc_error st = ensure_buffer(ctx->list, list_bytes);
@@ -1756,9 +1776,11 @@ static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, 
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 		}
 	}
-	CUDA_TRY(cudaEventRecord(ctx->scratch_done, stream), return ASTCENC_ERR_BAD_CONTEXT);
-	ctx->scratch_used = true;
 	return st;
+}
+
+static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
+	return scratch_turn(ctx, stream, [&] { return launch_blocks_locked(ctx, call, swizzle, stream); });
 }
 
 astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const void* d_pixels, astcenc_type data_type, unsigned int dim_x, unsigned int dim_y,
@@ -1766,7 +1788,7 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
                                                   uint8_t* d_payload, void* cuda_stream) {
 	astcenc_error status = check_compress_context(ctx);
 	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
-	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
 	if (status == ASTCENC_SUCCESS && (dim_x == 0 || dim_y == 0 || dim_z == 0 || !d_pixels || !d_payload || (block_count != 0 && !block_indices))) {
 		status = ASTCENC_ERR_BAD_PARAM;
 	}
@@ -1806,9 +1828,8 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
 
 // The image table of a multi-image call, checked whole before anything is enqueued (the caller has checked the context, the
 // swizzle and the pointers): zero dimensions and the data type (ASTCENC_ERR_BAD_PARAM), a_scale_radius on a texture array
-// (ASTCENC_ERR_NOT_IMPLEMENTED), then the block counts (ASTCENC_ERR_BAD_PARAM when an image's payload does not fit a size_t, an
-// image has 2^32 blocks or more - the gather indexes an image's blocks with 32 bits, as block lists do - or the call's total
-// does not fit a size_t). Fills call.table (data and payload as given), call.srcs, call.blocks and call.texel_bytes.
+// (ASTCENC_ERR_NOT_IMPLEMENTED), then the block counts (table_entry). Fills call.table (data and payload as given), call.srcs,
+// call.blocks and call.texel_bytes.
 static astcenc_error plan_image_table(const astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
                                       const astcenc_swizzle& swizzle, BlockCall& call) {
 	astcenc_error status = ASTCENC_SUCCESS;
@@ -1819,41 +1840,30 @@ static astcenc_error plan_image_table(const astcenc_context* ctx, const astcenc_
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		status = check_alpha_scale(ctx, images[i].dim_z);
 	}
-	if (status != ASTCENC_SUCCESS) {
-		return status;
-	}
-	size_t blocks = 0, avg_offset = 0;
-	for (unsigned int i = 0; i < image_count; i++) {
+	call.table.resize(image_count);
+	size_t avg_offset = 0;
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_image& im = images[i];
-		const SlabGeometry geo = slab_geometry(ctx, im.dim_x, im.dim_y, im.dim_z, (int)data_type);
-		if (geo.payload_overflow() || geo.blocks > 0xFFFFFFFFu || geo.blocks > SIZE_MAX - blocks) {
-			return ASTCENC_ERR_BAD_PARAM;
-		}
-		GatherImage e;
-		e.data = im.data;
-		e.payload = im.payload;
-		e.first = blocks;
-		e.avg_offset = avg_offset;
-		e.dim_x = im.dim_x;
-		e.dim_y = im.dim_y;
-		e.dim_z = im.dim_z;
-		e.blocks_x = (unsigned int)geo.blocks_x;
-		e.blocks_y = (unsigned int)geo.blocks_y;
-		call.table.push_back(e);
+		status = table_entry(ctx, (int)data_type, im.dim_x, im.dim_y, im.dim_z, im.data, im.payload, call.blocks, call.table[i]);
+		call.table[i].avg_offset = avg_offset;
 		call.srcs.push_back(pass_image(ctx, im.data, (int)data_type, im.dim_x, im.dim_y, im.dim_z, swizzle));
-		blocks += geo.blocks;
 		avg_offset += (size_t)im.dim_x * im.dim_y;
-		call.texel_bytes = geo.texel_bytes;
 	}
-	call.blocks = blocks;
-	return ASTCENC_SUCCESS;
+	call.texel_bytes = texel_bytes(data_type);
+	return status;
+}
+
+// Payload bytes of image i of an image-table call.
+static size_t payload_bytes(const BlockCall& call, size_t i) {
+	const size_t end = i + 1 < call.table.size() ? call.table[i + 1].first : call.blocks;
+	return (end - call.table[i].first) * 16;
 }
 
 astcenc_error astcenc_b200_compress_device_images(astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
                                                   const astcenc_swizzle* swizzle, void* cuda_stream) {
 	astcenc_error status = check_compress_context(ctx);
 	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
-	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
 	if (status == ASTCENC_SUCCESS && image_count != 0 && !images) status = ASTCENC_ERR_BAD_PARAM;
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		if (!images[i].data || !images[i].payload) {
@@ -1879,7 +1889,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
                                            uint8_t* const* data_out, const size_t* data_len) {
 	astcenc_error status = check_compress_context(ctx);
 	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
-	if (status == ASTCENC_SUCCESS) status = validate_compression_swizzle(*swizzle);
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
 	if (status == ASTCENC_SUCCESS && image_count != 0 && (!images || !data_out || !data_len)) status = ASTCENC_ERR_BAD_PARAM;
 	std::vector<astcenc_b200_device_image> descs;
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
@@ -1896,8 +1906,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 		status = plan_image_table(ctx, descs.data(), image_count, images[0]->data_type, *swizzle, call);
 	}
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
-		const size_t end = i + 1 < image_count ? call.table[i + 1].first : call.blocks;
-		if (data_len[i] < (end - call.table[i].first) * 16) {
+		if (data_len[i] < payload_bytes(call, i)) {
 			status = ASTCENC_ERR_OUT_OF_MEM;
 		}
 	}
@@ -1942,8 +1951,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 	}
 	CUDA_TRY(cudaEventRecord(ctx->ev1, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	for (unsigned int i = 0; i < image_count; i++) {
-		const size_t end = i + 1 < image_count ? call.table[i + 1].first : call.blocks;
-		const size_t bytes = (end - call.table[i].first) * 16;
+		const size_t bytes = payload_bytes(call, i);
 		CUDA_TRY(cudaMemcpyAsync(data_out[i], call.table[i].payload, bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		ctx->last_d2h += bytes;
 	}
@@ -1953,11 +1961,10 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 }
 
 // Decode calls: every image is checked before anything is enqueued; the table goes up in one copy and one launch decodes every
-// block of the call. The launch takes the context's table buffer (ctx->list), so it is a turn of the scratch like any pass
-// (launch_mtx, scratch_done).
+// block of the call, in one scratch turn (the launch takes the context's table buffer, ctx->list).
 astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const astcenc_b200_device_decode_image* images, unsigned int image_count,
                                                     astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
-	astcenc_error status = swizzle ? validate_decompression_swizzle(*swizzle) : ASTCENC_ERR_BAD_PARAM;
+	astcenc_error status = swizzle ? check_swizzle(*swizzle, ASTCENC_SWZ_Z) : ASTCENC_ERR_BAD_PARAM;
 	if (status == ASTCENC_SUCCESS && image_count != 0 && !images) status = ASTCENC_ERR_BAD_PARAM;
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		if (!images[i].payload || !images[i].data) {
@@ -1967,59 +1974,22 @@ astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const 
 		}
 	}
 	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
-	if (status != ASTCENC_SUCCESS) {
-		return status;
-	}
 	std::vector<GatherImage> table(image_count);
 	size_t blocks = 0;
-	for (unsigned int i = 0; i < image_count; i++) {
+	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_decode_image& im = images[i];
-		const SlabGeometry geo = slab_geometry(ctx, im.dim_x, im.dim_y, im.dim_z, (int)data_type);
-		if (geo.payload_overflow() || geo.blocks > 0xFFFFFFFFu || geo.blocks > SIZE_MAX - blocks) {
-			return ASTCENC_ERR_BAD_PARAM;
-		}
-		GatherImage& e = table[i];
-		e.data = im.data;
-		e.payload = const_cast<uint8_t*>(im.payload);      // (read, never written)
-		e.first = blocks;
-		e.avg_offset = 0;
-		e.dim_x = im.dim_x;
-		e.dim_y = im.dim_y;
-		e.dim_z = im.dim_z;
-		e.blocks_x = (unsigned int)geo.blocks_x;
-		e.blocks_y = (unsigned int)geo.blocks_y;
-		blocks += geo.blocks;
+		// (the payload is read, never written)
+		status = table_entry(ctx, (int)data_type, im.dim_x, im.dim_y, im.dim_z, im.data, const_cast<uint8_t*>(im.payload), blocks, table[i]);
 	}
-	if (image_count == 0) {
-		return ASTCENC_SUCCESS;
+	if (status != ASTCENC_SUCCESS || image_count == 0) {
+		return status;
 	}
 	DeviceGuard guard(ctx->device);
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	int sms = 0;
-	CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device), return ASTCENC_ERR_BAD_CONTEXT);
-	const unsigned int warps = ASTC_DECODE_THREADS / 32;
-	const size_t ctas = (blocks + warps - 1) / warps;
-	const unsigned int grid = ctas < (size_t)sms * 8 ? (unsigned int)ctas : (unsigned int)sms * 8;
-	std::lock_guard<std::mutex> lk(ctx->launch_mtx);
-	if (ctx->scratch_used) {
-		CUDA_TRY(cudaStreamWaitEvent(s, ctx->scratch_done, 0), return ASTCENC_ERR_BAD_CONTEXT);
-	}
-	astcenc_error st = ensure_buffer(ctx->list, table.size() * sizeof(GatherImage));
-	if (st != ASTCENC_SUCCESS) {
-		return st;
-	}
-	// (from pageable memory: staged by the driver before the call returns)
-	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, table.data(), table.size() * sizeof(GatherImage), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
-	astc_decompress_images_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, s>>>(
-	    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, (int)data_type, 0, 0, 0, *swizzle), ctx->list.as<const GatherImage>(), image_count, blocks);
-	ctx->launches++;
-	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
-	CUDA_TRY(cudaEventRecord(ctx->scratch_done, s), return ASTCENC_ERR_BAD_CONTEXT);
-	ctx->scratch_used = true;
-	return ASTCENC_SUCCESS;
+	return scratch_turn(ctx, s, [&] { return launch_decode(ctx, table.data(), image_count, blocks, (int)data_type, *swizzle, s); });
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

@@ -10,6 +10,7 @@
 #include "simt_emul.h"
 #endif
 #include "../../astc-encoder_b200/csrc/astc_dev_search.cuh"
+#include "../../astc-encoder_b200/csrc/astc_dev_gather.cuh"
 #include "../../astc-encoder_b200/csrc/astc_host_pack.h"
 #include "../../astc-encoder_b200/csrc/astc_host_config.h"
 #include "../../astc-encoder_b200/csrc/astc_host_launch.h"
@@ -193,7 +194,8 @@ extern "C" int hostsim_compress_image(int profile, unsigned int bx, unsigned int
 	return hostsim_compress_volume(profile, bx, by, 1, quality, flags, data, data_type, dim_x, dim_y, 1, swz, out);
 }
 
-// decompression through the device source (one simulated lane). swz uses astcenc_swz numbering.
+// decompression through the device source (one simulated lane): the table walk of astc_decompress_images_kernel over a one-entry
+// table, as astcenc_decompress_image builds it. swz uses astcenc_swz numbering.
 extern "C" int hostsim_decompress_volume(int profile, unsigned int bx, unsigned int by, unsigned int bz, unsigned int flags, const uint8_t* blocks, void* out, int data_type,
                                          unsigned int dim_x, unsigned int dim_y, unsigned int dim_z, const int* swz) {
 	astcenc_config cfg;
@@ -209,20 +211,21 @@ extern "C" int hostsim_decompress_volume(int profile, unsigned int bx, unsigned 
 	astc_host::make_device_config(cfg, dcfg);
 	std::vector<uint8_t> window(ASTC_SMEM_HDR + D_SLICE + 64, 0xCD);
 	astc_smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(window.data()) + 15) & ~(uintptr_t)15);
-	DevImage img;
-	img.data = out;
+	GatherImage e;
+	e.data = out;
+	e.payload = const_cast<uint8_t*>(blocks);
+	e.first = 0;
+	e.avg_offset = 0;
+	e.dim_x = dim_x;
+	e.dim_y = dim_y;
+	e.dim_z = dim_z;
+	e.blocks_x = (dim_x + bx - 1) / bx;
+	e.blocks_y = (dim_y + by - 1) / by;
+	const size_t total = (size_t)e.blocks_x * e.blocks_y * (bz > 1 ? (dim_z + bz - 1) / bz : 1);
+	// the launch's DevImage: the call's data type and swizzle, nothing else
+	DevImage img{};
 	img.data_type = data_type;
-	img.dim_x = dim_x;
-	img.dim_y = dim_y;
-	img.dim_z = dim_z;
-	img.blocks_x = (dim_x + bx - 1) / bx;
-	img.blocks_y = (dim_y + by - 1) / by;
-	img.block_row0 = 0;
-	img.block_rows = img.blocks_y * (bz > 1 ? (dim_z + bz - 1) / bz : 1);
 	for (int i = 0; i < 4; i++) img.swz[i] = swz ? swz[i] : i;
-	img.out = nullptr;
-	img.alpha_avg = nullptr;
-	img.alpha_threshold = 0.0f;
 	SmemHdr* hdr = reinterpret_cast<SmemHdr*>(astc_smem);
 	hdr->bsd = pk.bsd;
 	hdr->cfg = dcfg;
@@ -230,11 +233,7 @@ extern "C" int hostsim_decompress_volume(int profile, unsigned int bx, unsigned 
 	hdr->dec_smem_off = 0;
 	hdr->cq_smem_off = 0;
 	run_lanes([&](int lane) {
-		for (unsigned int y = 0; y < img.block_rows; y++) {
-			for (unsigned int x = 0; x < img.blocks_x; x++) {
-				decompress_block(lane, ASTC_SMEM_HDR, blocks + ((size_t)y * img.blocks_x + x) * 16, x, y);
-			}
-		}
+		decode_table_blocks(&e, 1, 0, total, 0, 1, lane, ASTC_SMEM_HDR);
 	});
 	astc_host::free_block_size_tables(t);
 	return 0;

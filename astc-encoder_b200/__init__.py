@@ -72,6 +72,12 @@ class DeviceDecodeImage(C.Structure):
     _fields_ = [("payload", C.c_void_p), ("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint)]
 
 
+class DeviceMetricsImage(C.Structure):
+    """struct astcenc_b200_device_metrics_image (include/astcenc.h)."""
+    _fields_ = [("original", C.c_void_p), ("decoded", C.c_void_p), ("original_type", C.c_int), ("decoded_type", C.c_int), ("dim_x", C.c_uint),
+                ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("metrics", C.c_void_p), ("block_error", C.c_void_p)]
+
+
 class ErrorMetrics(C.Structure):
     """struct astcenc_b200_error_metrics (include/astcenc.h)."""
     _fields_ = [(n, C.c_double) for n in ("psnr", "alpha_psnr", "rgb_psnr", "rgb_peak", "peak_psnr", "mpsnr", "log_rmse",
@@ -140,6 +146,9 @@ def lib():
         l.astcenc_b200_compute_error_metrics.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(Image), C.POINTER(Image), C.c_int, C.c_int,
                                                          C.POINTER(ErrorMetrics)]
         l.astcenc_b200_compute_error_metrics.restype = C.c_int
+        l.astcenc_b200_compute_error_metrics_device_images.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(DeviceMetricsImage), C.c_uint,
+                                                                       C.c_int, C.c_int, C.c_void_p]
+        l.astcenc_b200_compute_error_metrics_device_images.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -433,6 +442,20 @@ class Context:
         d = {n: getattr(out, n) for n, _ in ErrorMetrics._fields_[:9]}
         d["sum_squared_error"] = list(out.sum_squared_error)
         return d
+
+    def compute_error_metrics_device_images(self, images, hdr=False, normal=False, input_components=4, fstop_lo=-10, fstop_hi=10, stream=0):
+        """Error metrics of many device-resident image pairs in one call (astcenc_b200_compute_error_metrics_device_images).
+        images: a sequence of (d_original_ptr, d_decoded_ptr, original_type, decoded_type, dim_x, dim_y, dim_z, d_metrics_ptr,
+        d_block_error_ptr or 0); every metrics pointer receives an ErrorMetrics, the figures compute_error_metrics gives for that
+        pair alone, and every block_error pointer one float per block of the context's footprint. Enqueued on `stream`, no sync;
+        works on decompress-only contexts. ErrorMetrics.from_buffer_copy reads a struct back."""
+        n = len(images)
+        table = (DeviceMetricsImage * n)(*[DeviceMetricsImage(C.c_void_p(o), C.c_void_p(d), ot, dt, x, y, z, C.c_void_p(m), C.c_void_p(b or None))
+                                           for o, d, ot, dt, x, y, z, m, b in images])
+        err = lib().astcenc_b200_compute_error_metrics_device_images(self.handle, int(hdr), int(normal), input_components, table if n else None, n,
+                                                                     fstop_lo, fstop_hi, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compute_error_metrics_device_images")
 
     def last_timing(self):
         ms = C.c_float(); a = C.c_size_t(); b = C.c_size_t()

@@ -53,15 +53,23 @@ struct GatherTexel {
 	bool inside;
 };
 
+// Texel t (x fastest, then y, then z) of the footprint of block `index` of an image of blocks_x x blocks_y blocks per layer:
+// its place (tx, ty, tz) in the footprint and its image coordinates (x, y, z), unclamped: they may lie beyond the image's edges.
+ASTC_FN void footprint_texel(unsigned int blocks_x, unsigned int blocks_y, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index,
+                             unsigned int t, unsigned int& tx, unsigned int& ty, unsigned int& tz, unsigned int& x, unsigned int& y, unsigned int& z) {
+	unsigned int col = index % blocks_x;
+	unsigned int rest = index / blocks_x;
+	unsigned int row = rest % blocks_y;
+	unsigned int layer = rest / blocks_y;
+	tx = t % bx;
+	ty = (t / bx) % by;
+	tz = t / (bx * by);
+	x = col * bx + tx, y = row * by + ty, z = layer * bz + tz;
+}
+
 ASTC_FN GatherTexel gather_texel(const GatherArgs& g, unsigned int i, uint32_t index, unsigned int t) {
-	unsigned int col = index % g.blocks_x;
-	unsigned int rest = index / g.blocks_x;
-	unsigned int row = rest % g.blocks_y;
-	unsigned int layer = rest / g.blocks_y;
-	unsigned int tx = t % g.bx;
-	unsigned int ty = (t / g.bx) % g.by;
-	unsigned int tz = t / (g.bx * g.by);
-	unsigned int x = col * g.bx + tx, y = row * g.by + ty, z = layer * g.bz + tz;
+	unsigned int tx, ty, tz, x, y, z;
+	footprint_texel(g.blocks_x, g.blocks_y, g.bx, g.by, g.bz, index, t, tx, ty, tz, x, y, z);
 	unsigned int xi = x < g.dim_x - 1 ? x : g.dim_x - 1;
 	unsigned int yi = y < g.dim_y - 1 ? y : g.dim_y - 1;
 	unsigned int zi = z < g.dim_z - 1 ? z : g.dim_z - 1;
@@ -72,9 +80,11 @@ ASTC_FN GatherTexel gather_texel(const GatherArgs& g, unsigned int i, uint32_t i
 	return r;
 }
 
-// The table entry that holds call block c: the last image whose first block is at or before c (every image has at least one
-// block, so there is exactly one).
-ASTC_FN unsigned int find_image(const GatherImage* images, unsigned int image_count, size_t c) {
+// The table entry that holds item c of a call: the last entry whose first item is at or before c (every entry has at least one
+// item, so there is exactly one). The entries are images of an image table (items: call blocks), pairs of a metrics call
+// (virtual CTAs) or the mapped pairs of one (map blocks).
+template <typename E>
+ASTC_FN unsigned int find_image(const E* images, unsigned int image_count, size_t c) {
 	unsigned int lo = 0, hi = image_count - 1;
 	while (lo < hi) {
 		unsigned int mid = (lo + hi + 1) / 2;

@@ -5,44 +5,148 @@
 // and for HDR images log2 / multi-exposure (mPSNR) differences, for normal maps the angular error. Per-texel values
 // use the reference's float arithmetic (its polynomial log2, astcenc_vecmathlib.h:416-441; DPPS-ordered dot products);
 // the sums are double accumulators there (:31-58) - here the image is reduced in parallel (thread -> warp -> CTA ->
-// a second single-CTA pass in fixed order), so results are deterministic but differ from the reference's raster-order
+// a second pass in fixed order), so results are deterministic but differ from the reference's raster-order
 // double sums in the last bits (tests/test_metrics.py states the tolerance).
+//
+// A call measures a table of image pairs (MetricEntry). Each slice of an entry owns a fixed number of virtual CTAs
+// (metric_ctas: a function of the slice's texel count only, never of the GPU), so an entry's sums do not depend on the
+// device, on the other entries of the call or on their order. A CTA of the launch finds its entry by binary search over
+// the prefix of the entries' virtual-CTA counts (find_image) and runs the grid-stride loop over its slice as virtual CTA
+// v of `ctas`. Partials go out [slice][virtual CTA] per entry, and the finish kernel walks them in that order.
+//
+// The per-block error map (block_error_sum) is one warp per block of the context's footprint, in astcenc_compress_image's
+// block order; it compiles for the host simulation too (tests/hostsim/hostsim_metrics.cpp).
 #pragma once
+#include <vector>
+#include "../../include/astcenc.h"
 
 #define ASTC_METRIC_SUMS 17
 // [0..3] squared error r,g,b,a; [4..7] alpha-scaled; [8..10] log2 error r,g,b; [11..13] mPSNR error r,g,b;
 // [14] sum of angular error / pixel count; [15] worst angular error (max); [16] rgb peak of image 1 (max)
 enum { MS_ERR = 0, MS_AERR = 4, MS_LOG = 8, MS_MPSNR = 11, MS_ANG_MEAN = 14, MS_ANG_WORST = 15, MS_PEAK = 16 };
 
-struct MetricImage {
-	const void* data;
-	int type;                // ASTCENC_TYPE_*
-	unsigned int dim_x;      // row pitch in texels
+#define ASTC_METRIC_THREADS 256
+#define ASTC_METRIC_MAX_CTAS 592            // virtual CTAs per slice at most
+#define ASTC_METRIC_FINISH_GROUPS 8         // finish kernel: entries per CTA, ASTC_METRIC_SUMS threads each
+#define ASTC_METRIC_MAP_WARPS 8             // map kernel: blocks per CTA, one warp each
+
+#if defined(ASTC_HOSTSIM)
+	#define ASTC_HD static inline
+#else
+	#define ASTC_HD static __host__ __device__ inline
+#endif
+
+// One image pair of a metrics call: the dim_x x dim_y x dim_z intersection of two images, each with its own row pitch and slice
+// stride (in texels), so that a one-entry table compares two images of different sizes as the host entry does.
+struct MetricEntry {
+	const void* img1;                 // the original: slices of texels of type1 (ASTCENC_TYPE_*)
+	const void* img2;                 // the decoded image
+	int type1, type2;
+	unsigned int pitch1, pitch2;
+	size_t stride1, stride2;
+	unsigned int dim_x, dim_y, dim_z;
+	// filled in by plan_metrics
+	unsigned int ctas;                // virtual CTAs per slice
+	size_t first;                     // the entry's first virtual CTA in the call; its partials start there too
+	double inv_pixels;                // 1 / (dim_x * dim_y * dim_z), the product in unsigned arithmetic like the reference's :281
+	unsigned int blocks_x, blocks_y;  // block grid of the map footprint
+	astcenc_b200_error_metrics* metrics;   // receives the figures (device), or null: the sums are read back instead
+	float* block_error;               // the per-block map (device), or null
+};
+
+// A mapped entry of a call: map warps [first, first + its block count) belong to table entry `entry`.
+struct MetricMap {
+	size_t first;
+	unsigned int entry;
 };
 
 struct MetricArgs {
-	MetricImage img1, img2;
-	unsigned int dim_x, dim_y;     // the compared intersection
-	int hdr, normal;
+	const MetricEntry* entries;
+	unsigned int count;
+	const MetricMap* maps;
+	unsigned int map_count;
+	size_t map_blocks;                // blocks of every mapped entry
+	unsigned int bx, by, bz;          // the map footprint
+	int hdr, normal, components;
 	int fstop_lo, fstop_hi;
-	double inv_pixels;
-	double* partials;              // [gridDim.x][ASTC_METRIC_SUMS]
+	size_t ctas;                      // virtual CTAs of the call
+	double* partials;                 // [virtual CTA][ASTC_METRIC_SUMS], then the sums [entry][ASTC_METRIC_SUMS]
 };
 
-static __device__ __forceinline__ float4 metric_load(const MetricImage& im, unsigned int x, unsigned int y) {
-	size_t i = 4 * ((size_t)im.dim_x * y + x);
-	float4 c;
-	if (im.type == 0) {
-		uchar4 v = *reinterpret_cast<const uchar4*>(static_cast<const uint8_t*>(im.data) + i);
-		c = make_float4((float)v.x / 255.0f, (float)v.y / 255.0f, (float)v.z / 255.0f, (float)v.w / 255.0f);
-	} else if (im.type == 1) {
-		ushort4 v = *reinterpret_cast<const ushort4*>(static_cast<const uint16_t*>(im.data) + i);
-		c = make_float4(sf16_to_float(v.x), sf16_to_float(v.y), sf16_to_float(v.z), sf16_to_float(v.w));
-	} else {
-		c = *reinterpret_cast<const float4*>(static_cast<const float*>(im.data) + i);
+// ---- host planning (no CUDA calls: the host tests run it) ----
+
+// Virtual CTAs of one slice of texels texels: the partition the sums are defined by.
+static inline unsigned int metric_ctas(size_t texels) {
+	size_t ctas = (texels + ASTC_METRIC_THREADS - 1) / ASTC_METRIC_THREADS;
+	return (unsigned int)(ctas < ASTC_METRIC_MAX_CTAS ? ctas : ASTC_METRIC_MAX_CTAS);
+}
+
+struct MetricPlan {
+	std::vector<MetricMap> maps;
+	size_t ctas = 0;                  // grid of the metrics kernel
+	size_t map_blocks = 0;            // warps of the map kernel
+	size_t partial_doubles = 0;       // the partials and the per-entry sums
+	unsigned int finish_grid = 0;     // CTAs of the finish kernel
+	unsigned int map_grid = 0;        // CTAs of the map kernel (0: no map asked for)
+};
+
+// Fills in the planned fields of `table` (its images, types, pitches, strides, dims and outputs set) for the footprint
+// bx x by x bz. false: the call does not fit a launch (an entry with a map has 2^32 blocks or more, or a grid exceeds 2^31 - 1).
+static inline bool plan_metrics(std::vector<MetricEntry>& table, unsigned int bx, unsigned int by, unsigned int bz, MetricPlan& p) {
+	const size_t grid_max = 0x7FFFFFFF;
+	p = MetricPlan();
+	for (size_t i = 0; i < table.size(); i++) {
+		MetricEntry& e = table[i];
+		e.ctas = metric_ctas((size_t)e.dim_x * e.dim_y);
+		e.first = p.ctas;
+		e.inv_pixels = 1.0 / (double)(e.dim_x * e.dim_y * e.dim_z);
+		e.blocks_x = (e.dim_x + bx - 1) / bx;
+		e.blocks_y = (e.dim_y + by - 1) / by;
+		p.ctas += (size_t)e.ctas * e.dim_z;
+		if (p.ctas > grid_max) {
+			return false;
+		}
+		if (e.block_error != nullptr) {
+			const size_t blocks = (size_t)e.blocks_x * e.blocks_y * ((e.dim_z + bz - 1) / bz);
+			if (blocks > 0xFFFFFFFFu) {
+				return false;
+			}
+			p.maps.push_back({p.map_blocks, (unsigned int)i});
+			p.map_blocks += blocks;
+		}
 	}
-	if (im.type != 0) {
-		// clamp(0, 65504, c) = min(max(c, 0), 65504) (:187, :200)
+	const size_t map_grid = (p.map_blocks + ASTC_METRIC_MAP_WARPS - 1) / ASTC_METRIC_MAP_WARPS;
+	if (map_grid > grid_max) {
+		return false;
+	}
+	p.map_grid = (unsigned int)map_grid;
+	p.finish_grid = (unsigned int)((table.size() + ASTC_METRIC_FINISH_GROUPS - 1) / ASTC_METRIC_FINISH_GROUPS);
+	p.partial_doubles = (p.ctas + table.size()) * ASTC_METRIC_SUMS;
+	return true;
+}
+
+// ---- per-texel values ----
+
+// Texel t (index in texels) of an image of `type`: U8 scaled to 0..1, F16 / F32 clamped to [0, 65504] (:187, :200). One vector
+// load per texel: the data is aligned to its texel (4, 8 or 16 bytes).
+ASTC_FN f4 metric_texel(const void* data, int type, size_t t) {
+	f4 c;
+	if (type == 0) {
+		const uint32_t v = ASTC_LDG(static_cast<const uint32_t*>(data) + t);
+		c = mk4((float)(v & 0xFF) / 255.0f, (float)((v >> 8) & 0xFF) / 255.0f, (float)((v >> 16) & 0xFF) / 255.0f, (float)(v >> 24) / 255.0f);
+	} else if (type == 1) {
+		const unsigned long long v = ASTC_LDG(static_cast<const unsigned long long*>(data) + t);
+		c = mk4(sf16_to_float((uint16_t)v), sf16_to_float((uint16_t)(v >> 16)), sf16_to_float((uint16_t)(v >> 32)), sf16_to_float((uint16_t)(v >> 48)));
+	} else {
+#if defined(ASTC_HOSTSIM)
+		const float* p = static_cast<const float*>(data) + 4 * t;
+		c = mk4(p[0], p[1], p[2], p[3]);
+#else
+		const float4 v = __ldg(static_cast<const float4*>(data) + t);
+		c = mk4(v.x, v.y, v.z, v.w);
+#endif
+	}
+	if (type != 0) {
 		c.x = fminf(fmaxf(c.x, 0.0f), 65504.0f);
 		c.y = fminf(fmaxf(c.y, 0.0f), 65504.0f);
 		c.z = fminf(fmaxf(c.z, 0.0f), 65504.0f);
@@ -51,6 +155,91 @@ static __device__ __forceinline__ float4 metric_load(const MetricImage& im, unsi
 	return c;
 }
 
+// The channels input_components counts (compute_error_metrics :283-284): 1 RGB, 2 BA, 3 RGB, 4 RGBA.
+ASTC_HD int metric_component_mask(int input_components) {
+	return input_components == 2 ? 0x0C : input_components == 4 ? 0x0F : 0x07;
+}
+
+// ---- the per-block error map ----
+
+// Map block `index` of entry e (astcenc_compress_image's block order for the footprint bx x by x bz; a 2D footprint's index
+// counts the slices of a texture array), by `lanes` lanes of one warp: the sum, over the block's texels inside the image, of
+// the squared differences of the channels in `mask`, each the float square of a float difference as in the sums, added in
+// double. Lane l takes texels l, l + lanes, ... in footprint order, then the lanes are summed in a fixed xor-shuffle order.
+// Every lane returns the sum.
+ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index, int mask, int lane, int lanes) {
+	double acc = 0.0;
+	for (unsigned int t = (unsigned int)lane; t < bx * by * bz; t += (unsigned int)lanes) {
+		unsigned int tx, ty, tz, x, y, z;
+		footprint_texel(e.blocks_x, e.blocks_y, bx, by, bz, index, t, tx, ty, tz, x, y, z);
+		if (x >= e.dim_x || y >= e.dim_y || z >= e.dim_z) {
+			continue;
+		}
+		const f4 c1 = metric_texel(e.img1, e.type1, z * e.stride1 + (size_t)e.pitch1 * y + x);
+		const f4 c2 = metric_texel(e.img2, e.type2, z * e.stride2 + (size_t)e.pitch2 * y + x);
+		const float d[4] = {c1.x - c2.x, c1.y - c2.y, c1.z - c2.z, c1.w - c2.w};
+		for (int k = 0; k < 4; k++) {
+			if (mask & (1 << k)) {
+				acc += (double)(d[k] * d[k]);
+			}
+		}
+	}
+#if !defined(ASTC_ONE_LANE)
+	for (int o = lanes / 2; o > 0; o >>= 1) {
+		acc += __shfl_xor_sync(0xffffffffu, acc, o);
+	}
+#endif
+	return acc;
+}
+
+// ---- the closing arithmetic of compute_error_metrics (:285-411) ----
+
+// The figures of one entry from its 17 sums; `pixels` = (double)(dim_x * dim_y * dim_z), the product in unsigned arithmetic.
+// Runs on the device (the finish kernel) and on the host (astcenc_b200_compute_error_metrics).
+ASTC_HD void metric_close(const double* sums, int hdr, int normal, int input_components, int fstop_lo, int fstop_hi, double pixels,
+                          astcenc_b200_error_metrics* out) {
+	const int mask = metric_component_mask(input_components);
+	double samples = 0.0, num = 0.0, alpha_num = 0.0, log_num = 0.0, mpsnr_num = 0.0;
+	for (int c = 0; c < 4; c++) {
+		if (mask & (1 << c)) {
+			num += sums[MS_ERR + c];
+			alpha_num += sums[MS_AERR + c];
+			if (c < 3) {
+				log_num += sums[MS_LOG + c];
+				mpsnr_num += sums[MS_MPSNR + c];
+			}
+			samples += pixels;
+		}
+	}
+	double stopcount = (double)(fstop_hi - fstop_lo + 1);
+	double mpsnr_denom = pixels * 3.0 * stopcount * 255.0 * 255.0;
+	double psnr = num == 0.0 ? 999.0 : 10.0 * log10(samples / num);
+	double rgb_psnr = psnr;
+	memset(out, 0, sizeof(*out));
+	out->psnr = psnr;
+	out->alpha_psnr = psnr;
+	if (mask & 8) {
+		out->alpha_psnr = alpha_num == 0.0 ? 999.0 : 10.0 * log10(samples / alpha_num);
+		double rgb_num = sums[MS_ERR + 0] + sums[MS_ERR + 1] + sums[MS_ERR + 2];
+		rgb_psnr = rgb_num == 0.0 ? 999.0 : 10.0 * log10(pixels * 3.0 / rgb_num);
+	}
+	out->rgb_psnr = rgb_psnr;
+	out->rgb_peak = sums[MS_PEAK];
+	if (hdr) {
+		out->peak_psnr = rgb_psnr + 20.0 * log10(sums[MS_PEAK]);
+		out->mpsnr = mpsnr_num == 0.0 ? 999.0 : 10.0 * log10(mpsnr_denom / mpsnr_num);
+		out->log_rmse = sqrt(log_num / pixels);
+	}
+	if (normal) {
+		out->mean_angular_error = sums[MS_ANG_MEAN];
+		out->worst_angular_error = sums[MS_ANG_WORST];
+	}
+	for (int c = 0; c < 4; c++) {
+		out->sum_squared_error[c] = sums[MS_ERR + c];
+	}
+}
+
+#if !defined(ASTC_HOSTSIM)
 // the reference's approximate log2 (astcenc_vecmathlib.h:416-441), unfused
 static __device__ __forceinline__ float metric_log2(float x) {
 	int i = __float_as_int(x);
@@ -81,7 +270,7 @@ static __device__ __forceinline__ float metric_mpsnr_sumdiff(float v1, float v2,
 }
 
 // (c - 0.5) * 2, normalize_safe(xyz, unit3) (:269-275; astcenc_vecmathlib.h:362-371), dot in DPPS order
-static __device__ __forceinline__ float3 metric_normal(float4 c) {
+static __device__ __forceinline__ float3 metric_normal(f4 c) {
 	float x = (c.x - 0.5f) * 2.0f, y = (c.y - 0.5f) * 2.0f, z = (c.z - 0.5f) * 2.0f;
 	float len = (x * x + y * y) + (z * z + 0.0f);
 	if (len != 0.0f) {
@@ -92,18 +281,29 @@ static __device__ __forceinline__ float3 metric_normal(float4 c) {
 	return make_float3(u, u, u);
 }
 
-__global__ void __launch_bounds__(256)
+// CTA b of the launch is virtual CTA b - first of its entry: slice z, CTA v of that slice's `ctas`.
+__global__ void __launch_bounds__(ASTC_METRIC_THREADS)
 astc_error_metrics_kernel(const __grid_constant__ MetricArgs a) {
+	const MetricEntry& e = a.entries[find_image(a.entries, a.count, blockIdx.x)];
+	const unsigned int ctas = e.ctas;
+	const unsigned int vz = (unsigned int)(blockIdx.x - e.first);
+	const unsigned int z = vz / ctas, v = vz - z * ctas;
+	const unsigned int dim_x = e.dim_x, pitch1 = e.pitch1, pitch2 = e.pitch2;
+	const int type1 = e.type1, type2 = e.type2;
+	// the slice: 4 << type bytes per texel
+	const void* img1 = static_cast<const uint8_t*>(e.img1) + ((z * e.stride1) << (2 + type1));
+	const void* img2 = static_cast<const uint8_t*>(e.img2) + ((z * e.stride2) << (2 + type2));
+	const double inv_pixels = e.inv_pixels;
 	double acc[ASTC_METRIC_SUMS];
 	for (int k = 0; k < ASTC_METRIC_SUMS; k++) {
 		acc[k] = 0.0;
 	}
-	size_t n = (size_t)a.dim_x * a.dim_y;
-	for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += (size_t)gridDim.x * blockDim.x) {
-		unsigned int y = (unsigned int)(p / a.dim_x);
-		unsigned int x = (unsigned int)(p - (size_t)y * a.dim_x);
-		float4 c1 = metric_load(a.img1, x, y);
-		float4 c2 = metric_load(a.img2, x, y);
+	size_t n = (size_t)dim_x * e.dim_y;
+	for (size_t p = (size_t)v * blockDim.x + threadIdx.x; p < n; p += (size_t)ctas * blockDim.x) {
+		unsigned int y = (unsigned int)(p / dim_x);
+		unsigned int x = (unsigned int)(p - (size_t)y * dim_x);
+		f4 c1 = metric_texel(img1, type1, (size_t)pitch1 * y + x);
+		f4 c2 = metric_texel(img2, type2, (size_t)pitch2 * y + x);
 		acc[MS_PEAK] = fmax(fmax(fmax((double)c1.x, (double)c1.y), (double)c1.z), acc[MS_PEAK]);
 		float dx = c1.x - c2.x, dy = c1.y - c2.y, dz = c1.z - c2.z, dw = c1.w - c2.w;
 		acc[MS_ERR + 0] += (double)(dx * dx);
@@ -133,12 +333,12 @@ astc_error_metrics_kernel(const __grid_constant__ MetricArgs a) {
 			d = fminf(fmaxf(d, -1.0f), 1.0f);
 			float rad_to_degrees = 180.0f / 3.14159265358979323846f;
 			double deg = acos((double)d) * (double)rad_to_degrees;
-			acc[MS_ANG_MEAN] += deg * a.inv_pixels;
+			acc[MS_ANG_MEAN] += deg * inv_pixels;
 			acc[MS_ANG_WORST] = fmax(acc[MS_ANG_WORST], deg);
 		}
 	}
 	// thread -> warp -> CTA, fixed order
-	__shared__ double red[8][ASTC_METRIC_SUMS];
+	__shared__ double red[ASTC_METRIC_THREADS / 32][ASTC_METRIC_SUMS];
 	for (int k = 0; k < ASTC_METRIC_SUMS; k++) {
 		double v = acc[k];
 		bool is_max = k >= MS_ANG_WORST;
@@ -162,16 +362,48 @@ astc_error_metrics_kernel(const __grid_constant__ MetricArgs a) {
 	}
 }
 
-// second pass: one thread per sum walks the CTA partials in order
-__global__ void astc_error_metrics_finish_kernel(const double* partials, int ctas, double* out) {
-	int k = threadIdx.x;
-	if (k < ASTC_METRIC_SUMS) {
+// Second pass: one group of ASTC_METRIC_SUMS threads per entry; thread k walks the entry's partials of sum k in order
+// ([slice][virtual CTA]) into the entry's sums, and the group's first thread closes them into the entry's figures.
+__global__ void __launch_bounds__(ASTC_METRIC_FINISH_GROUPS * ASTC_METRIC_SUMS)
+astc_error_metrics_finish_kernel(const __grid_constant__ MetricArgs a) {
+	__shared__ double sums[ASTC_METRIC_FINISH_GROUPS][ASTC_METRIC_SUMS];
+	const unsigned int g = threadIdx.x / ASTC_METRIC_SUMS, k = threadIdx.x - g * ASTC_METRIC_SUMS;
+	const unsigned int j = blockIdx.x * ASTC_METRIC_FINISH_GROUPS + g;
+	if (j < a.count) {
+		const MetricEntry& e = a.entries[j];
+		const size_t n = (size_t)e.ctas * e.dim_z;
+		const double* p = a.partials + e.first * ASTC_METRIC_SUMS + k;
 		bool is_max = k >= MS_ANG_WORST;
-		double v = partials[k];
-		for (int c = 1; c < ctas; c++) {
-			double t = partials[(size_t)c * ASTC_METRIC_SUMS + k];
+		double v = p[0];
+		for (size_t c = 1; c < n; c++) {
+			double t = p[c * ASTC_METRIC_SUMS];
 			v = is_max ? fmax(v, t) : v + t;
 		}
-		out[k] = v;
+		sums[g][k] = v;
+		a.partials[(a.ctas + j) * ASTC_METRIC_SUMS + k] = v;
+	}
+	__syncthreads();
+	if (j < a.count && k == 0 && a.entries[j].metrics != nullptr) {
+		const MetricEntry& e = a.entries[j];
+		astcenc_b200_error_metrics m;
+		metric_close(sums[g], a.hdr, a.normal, a.components, a.fstop_lo, a.fstop_hi, (double)(e.dim_x * e.dim_y * e.dim_z), &m);
+		*e.metrics = m;
 	}
 }
+
+// The map: warp w of the launch is block w - first of its mapped entry.
+__global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
+astc_block_error_kernel(const __grid_constant__ MetricArgs a) {
+	const size_t w = (size_t)blockIdx.x * ASTC_METRIC_MAP_WARPS + (threadIdx.x >> 5);
+	if (w >= a.map_blocks) {
+		return;      // (the whole warp)
+	}
+	const MetricMap& m = a.maps[find_image(a.maps, a.map_count, w)];
+	const MetricEntry& e = a.entries[m.entry];
+	const uint32_t index = (uint32_t)(w - m.first);      // (a mapped entry has fewer than 2^32 blocks)
+	const double s = block_error_sum(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), threadIdx.x & 31, ASTC_WARP);
+	if ((threadIdx.x & 31) == 0) {
+		e.block_error[index] = (float)s;
+	}
+}
+#endif

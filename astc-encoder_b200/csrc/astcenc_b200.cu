@@ -21,8 +21,8 @@
 #include <chrono>
 
 #include "astc_dev_search.cuh"
-#include "astc_dev_metrics.cuh"
 #include "astc_dev_gather.cuh"
+#include "astc_dev_metrics.cuh"
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
 #include "astc_host_slab.h"
@@ -410,6 +410,8 @@ struct astcenc_context {
 	// block lists (astcenc_b200_compress_device_blocks), grown on demand: the list, the staging image and payload of one chunk,
 	// the pre-pass averages of the source image
 	DevBuffer list, list_image, list_out, list_alpha;
+	// metrics calls: the partial sums of every virtual CTA and the sums of every pair, grown on demand
+	DevBuffer metric_partials;
 	// The per-context scratch (records, queues, counters, alpha averages, table and staging buffers) serves ONE pass at a time
 	// (scratch_turn): launch_mtx serialises the host side, scratch_done orders a pass on one stream behind the previous pass on
 	// another.
@@ -651,7 +653,7 @@ void astcenc_context_free(astcenc_context* ctx) {
 	cudaFree(ctx->d_ticket);
 	cudaFree(ctx->d_counters);
 	for (DevBuffer* b : {&ctx->records, &ctx->queues, &ctx->alpha, &ctx->image, &ctx->image2, &ctx->out, &ctx->list, &ctx->list_image, &ctx->list_out,
-	                     &ctx->list_alpha}) {
+	                     &ctx->list_alpha, &ctx->metric_partials}) {
 		cudaFree(b->ptr);
 	}
 	for (cudaEvent_t e : ctx->stage_events) {
@@ -1514,8 +1516,57 @@ astcenc_error astcenc_get_block_info(astcenc_context* ctx, const uint8_t data[16
 	return ASTCENC_SUCCESS;
 }
 
+// One metrics call of a planned table (plan_metrics) on `stream`, inside a scratch turn: the table and the map list go up into
+// the context's table buffer (ctx->list) in one copy, the metrics kernel and the finish kernel run, then the map kernel when
+// an entry asks for a map. The sums of entry j are left at ctx->metric_partials + (plan.ctas + j) * ASTC_METRIC_SUMS doubles.
+static astcenc_error launch_metrics(astcenc_context* ctx, const std::vector<MetricEntry>& table, const MetricPlan& plan, int hdr, int normal,
+                                    int input_components, int fstop_lo, int fstop_hi, cudaStream_t stream) {
+	const size_t table_bytes = table.size() * sizeof(MetricEntry);
+	const size_t map_bytes = plan.maps.size() * sizeof(MetricMap);
+	std::vector<uint8_t> up(table_bytes + map_bytes);
+	memcpy(up.data(), table.data(), table_bytes);
+	if (map_bytes != 0) {
+		memcpy(up.data() + table_bytes, plan.maps.data(), map_bytes);
+	}
+	astcenc_error st = ensure_buffer(ctx->list, up.size());
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->metric_partials, plan.partial_doubles * sizeof(double));
+	if (st != ASTCENC_SUCCESS) {
+		return st;
+	}
+	// (from pageable memory: staged by the driver before the call returns)
+	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, stream), return ASTCENC_ERR_BAD_CONTEXT);
+	MetricArgs a;
+	a.entries = ctx->list.as<const MetricEntry>();
+	a.count = (unsigned int)table.size();
+	a.maps = reinterpret_cast<const MetricMap*>(ctx->list.ptr + table_bytes);
+	a.map_count = (unsigned int)plan.maps.size();
+	a.map_blocks = plan.map_blocks;
+	a.bx = ctx->config.block_x;
+	a.by = ctx->config.block_y;
+	a.bz = ctx->config.block_z > 1 ? ctx->config.block_z : 1;
+	a.hdr = hdr != 0;
+	a.normal = normal != 0;
+	a.components = input_components;
+	a.fstop_lo = fstop_lo;
+	a.fstop_hi = fstop_hi;
+	a.ctas = plan.ctas;
+	a.partials = ctx->metric_partials.as<double>();
+	astc_error_metrics_kernel<<<(unsigned int)plan.ctas, ASTC_METRIC_THREADS, 0, stream>>>(a);
+	ctx->launches++;
+	astc_error_metrics_finish_kernel<<<plan.finish_grid, ASTC_METRIC_FINISH_GROUPS * ASTC_METRIC_SUMS, 0, stream>>>(a);
+	ctx->launches++;
+	if (plan.map_grid != 0) {
+		astc_block_error_kernel<<<plan.map_grid, ASTC_METRIC_MAP_WARPS * 32, 0, stream>>>(a);
+		ctx->launches++;
+	}
+	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+	return ASTCENC_SUCCESS;
+}
+
 // astcenc_b200_compute_error_metrics: the CLI's compute_error_metrics (astcenccli_error_metrics.cpp:109-413) with the
 // per-texel work and the reductions on the device; the final dB figures are computed here exactly as the CLI prints them.
+// A one-entry metrics call: both images' slices go up into ctx->image and ctx->image2, the table compares their intersection,
+// and the 17 sums come back.
 astcenc_error astcenc_b200_compute_error_metrics(astcenc_context* ctx, int compute_hdr_metrics, int compute_normal_metrics, int input_components,
                                                  const astcenc_image* img1, const astcenc_image* img2, int fstop_lo, int fstop_hi,
                                                  astcenc_b200_error_metrics* out) {
@@ -1539,106 +1590,48 @@ astcenc_error astcenc_b200_compute_error_metrics(astcenc_context* ctx, int compu
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	static const size_t comp_bytes[3] = {1, 2, 4};
-	size_t slice1 = (size_t)img1->dim_x * img1->dim_y * 4 * comp_bytes[img1->data_type];
-	size_t slice2 = (size_t)img2->dim_x * img2->dim_y * 4 * comp_bytes[img2->data_type];
-	// a fixed partition of the sums (not one derived from the SM count), so the figures are the same on every GPU
-	int ctas = 592;
-	size_t texels = (size_t)dim_x * dim_y;
-	if ((size_t)ctas * 256 > texels) {
-		ctas = (int)((texels + 255) / 256);
+	std::vector<MetricEntry> table(1);
+	MetricEntry& e = table[0];
+	e.type1 = (int)img1->data_type;
+	e.type2 = (int)img2->data_type;
+	e.pitch1 = img1->dim_x;
+	e.pitch2 = img2->dim_x;
+	e.stride1 = (size_t)img1->dim_x * img1->dim_y;
+	e.stride2 = (size_t)img2->dim_x * img2->dim_y;
+	e.dim_x = dim_x;
+	e.dim_y = dim_y;
+	e.dim_z = dim_z;
+	e.metrics = nullptr;
+	e.block_error = nullptr;
+	MetricPlan plan;
+	if (!plan_metrics(table, ctx->config.block_x, ctx->config.block_y, ctx->config.block_z > 1 ? ctx->config.block_z : 1, plan)) {
+		return ASTCENC_ERR_BAD_PARAM;
 	}
-	uint8_t* d1 = nullptr;
-	uint8_t* d2 = nullptr;
-	double* d_part = nullptr;
-	astcenc_error status = ASTCENC_SUCCESS;
+	const size_t slice1 = e.stride1 * texel_bytes(e.type1);
+	const size_t slice2 = e.stride2 * texel_bytes(e.type2);
 	double sums[ASTC_METRIC_SUMS];
-	do {
-		if (cudaMalloc(&d1, slice1) != cudaSuccess || cudaMalloc(&d2, slice2) != cudaSuccess ||
-		    cudaMalloc(&d_part, ((size_t)ctas * dim_z + 1) * ASTC_METRIC_SUMS * sizeof(double)) != cudaSuccess) {
-			status = ASTCENC_ERR_OUT_OF_MEM;
-			break;
+	astcenc_error st = scratch_turn(ctx, ctx->stream, [&]() -> astcenc_error {
+		astcenc_error r = ensure_buffer(ctx->image, slice1 * dim_z);
+		if (r == ASTCENC_SUCCESS) r = ensure_buffer(ctx->image2, slice2 * dim_z);
+		if (r == ASTCENC_SUCCESS) r = upload_slices(ctx->image.ptr, img1->data, 0, dim_z, slice1, ctx->stream);
+		if (r == ASTCENC_SUCCESS) r = upload_slices(ctx->image2.ptr, img2->data, 0, dim_z, slice2, ctx->stream);
+		if (r != ASTCENC_SUCCESS) {
+			return r;
 		}
-		MetricArgs a;
-		a.img1.type = (int)img1->data_type;
-		a.img1.dim_x = img1->dim_x;
-		a.img2.type = (int)img2->data_type;
-		a.img2.dim_x = img2->dim_x;
-		a.dim_x = dim_x;
-		a.dim_y = dim_y;
-		a.hdr = compute_hdr_metrics != 0;
-		a.normal = compute_normal_metrics != 0;
-		a.fstop_lo = fstop_lo;
-		a.fstop_hi = fstop_hi;
-		a.inv_pixels = 1.0 / (double)(dim_x * dim_y * dim_z);      // (unsigned product, like the reference's :281)
-		cudaError_t e = cudaSuccess;
-		for (unsigned int z = 0; z < dim_z && e == cudaSuccess; z++) {
-			// (stream-ordered: the next slice's copy waits for this slice's kernel)
-			e = cudaMemcpyAsync(d1, img1->data[z], slice1, cudaMemcpyHostToDevice, ctx->stream);
-			if (e == cudaSuccess) e = cudaMemcpyAsync(d2, img2->data[z], slice2, cudaMemcpyHostToDevice, ctx->stream);
-			a.img1.data = d1;
-			a.img2.data = d2;
-			a.partials = d_part + (size_t)z * ctas * ASTC_METRIC_SUMS;
-			astc_error_metrics_kernel<<<ctas, 256, 0, ctx->stream>>>(a);
-			ctx->launches++;
+		e.img1 = ctx->image.ptr;
+		e.img2 = ctx->image2.ptr;
+		r = launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, fstop_lo, fstop_hi, ctx->stream);
+		if (r == ASTCENC_SUCCESS) {
+			CUDA_TRY(cudaMemcpyAsync(sums, ctx->metric_partials.as<double>() + plan.ctas * ASTC_METRIC_SUMS, sizeof(sums), cudaMemcpyDeviceToHost, ctx->stream),
+			         return ASTCENC_ERR_BAD_CONTEXT);
 		}
-		double* d_out = d_part + (size_t)ctas * dim_z * ASTC_METRIC_SUMS;
-		astc_error_metrics_finish_kernel<<<1, 32, 0, ctx->stream>>>(d_part, ctas * (int)dim_z, d_out);
-		ctx->launches++;
-		if (e == cudaSuccess) e = cudaMemcpyAsync(sums, d_out, sizeof(sums), cudaMemcpyDeviceToHost, ctx->stream);
-		if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-		if (e == cudaSuccess) e = cudaGetLastError();
-		if (e != cudaSuccess) {
-			status = ASTCENC_ERR_BAD_CONTEXT;
-		}
-	} while (false);
-	cudaFree(d1);
-	cudaFree(d2);
-	cudaFree(d_part);
-	if (status != ASTCENC_SUCCESS) {
-		return status;
+		return r;
+	});
+	if (st != ASTCENC_SUCCESS) {
+		return st;
 	}
-	// the closing arithmetic of compute_error_metrics (:285-411)
-	static const int componentmasks[5] = {0x00, 0x07, 0x0C, 0x07, 0x0F};
-	int mask = componentmasks[input_components];
-	double pixels = (double)(dim_x * dim_y * dim_z);
-	double samples = 0.0, num = 0.0, alpha_num = 0.0, log_num = 0.0, mpsnr_num = 0.0;
-	for (int c = 0; c < 4; c++) {
-		if (mask & (1 << c)) {
-			num += sums[MS_ERR + c];
-			alpha_num += sums[MS_AERR + c];
-			if (c < 3) {
-				log_num += sums[MS_LOG + c];
-				mpsnr_num += sums[MS_MPSNR + c];
-			}
-			samples += pixels;
-		}
-	}
-	double stopcount = (double)(fstop_hi - fstop_lo + 1);
-	double mpsnr_denom = pixels * 3.0 * stopcount * 255.0 * 255.0;
-	double psnr = num == 0.0 ? 999.0 : 10.0 * log10(samples / num);
-	double rgb_psnr = psnr;
-	out->psnr = psnr;
-	out->alpha_psnr = psnr;
-	if (mask & 8) {
-		out->alpha_psnr = alpha_num == 0.0 ? 999.0 : 10.0 * log10(samples / alpha_num);
-		double rgb_num = sums[MS_ERR + 0] + sums[MS_ERR + 1] + sums[MS_ERR + 2];
-		rgb_psnr = rgb_num == 0.0 ? 999.0 : 10.0 * log10(pixels * 3.0 / rgb_num);
-	}
-	out->rgb_psnr = rgb_psnr;
-	out->rgb_peak = sums[MS_PEAK];
-	if (compute_hdr_metrics) {
-		out->peak_psnr = rgb_psnr + 20.0 * log10(sums[MS_PEAK]);
-		out->mpsnr = mpsnr_num == 0.0 ? 999.0 : 10.0 * log10(mpsnr_denom / mpsnr_num);
-		out->log_rmse = sqrt(log_num / pixels);
-	}
-	if (compute_normal_metrics) {
-		out->mean_angular_error = sums[MS_ANG_MEAN];
-		out->worst_angular_error = sums[MS_ANG_WORST];
-	}
-	for (int c = 0; c < 4; c++) {
-		out->sum_squared_error[c] = sums[MS_ERR + c];
-	}
+	CUDA_TRY(cudaStreamSynchronize(ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
+	metric_close(sums, compute_hdr_metrics, compute_normal_metrics, input_components, fstop_lo, fstop_hi, (double)(dim_x * dim_y * dim_z), out);
 	return ASTCENC_SUCCESS;
 }
 
@@ -1990,6 +1983,60 @@ astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const 
 	}
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return scratch_turn(ctx, s, [&] { return launch_decode(ctx, table.data(), image_count, blocks, (int)data_type, *swizzle, s); });
+}
+
+// Metrics calls: every pair is checked before anything is enqueued; the table goes up in one copy and the call is two
+// launches, three with a map, in one scratch turn.
+astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* ctx, int compute_hdr_metrics, int compute_normal_metrics,
+                                                               int input_components, const astcenc_b200_device_metrics_image* images,
+                                                               unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream) {
+	if (!ctx || input_components < 1 || input_components > 4) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (fstop_lo < -125 || fstop_hi > 125) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (image_count != 0 && !images) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	auto aligned = [](const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
+	std::vector<MetricEntry> table(image_count);
+	for (unsigned int i = 0; i < image_count; i++) {
+		const astcenc_b200_device_metrics_image& im = images[i];
+		if (!im.original || !im.decoded || !im.metrics || check_texel_count(im.dim_x, im.dim_y, im.dim_z) != ASTCENC_SUCCESS ||
+		    check_data_type(im.original_type) != ASTCENC_SUCCESS || check_data_type(im.decoded_type) != ASTCENC_SUCCESS ||
+		    !aligned(im.original, texel_bytes(im.original_type)) || !aligned(im.decoded, texel_bytes(im.decoded_type)) || !aligned(im.metrics, 8) ||
+		    !aligned(im.block_error, 4)) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		MetricEntry& e = table[i];
+		e.img1 = im.original;
+		e.img2 = im.decoded;
+		e.type1 = (int)im.original_type;
+		e.type2 = (int)im.decoded_type;
+		e.pitch1 = e.pitch2 = im.dim_x;
+		e.stride1 = e.stride2 = (size_t)im.dim_x * im.dim_y;
+		e.dim_x = im.dim_x;
+		e.dim_y = im.dim_y;
+		e.dim_z = im.dim_z;
+		e.metrics = im.metrics;
+		e.block_error = im.block_error;
+	}
+	MetricPlan plan;
+	if (!plan_metrics(table, ctx->config.block_x, ctx->config.block_y, ctx->config.block_z > 1 ? ctx->config.block_z : 1, plan)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (image_count == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return scratch_turn(ctx, s, [&] {
+		return launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, fstop_lo, fstop_hi, s);
+	});
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

@@ -371,6 +371,44 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_error_metrics(struct astc
                                                                      int fstop_lo, int fstop_hi, struct astcenc_b200_error_metrics* metrics);
 
 /**
+ * Error metrics of many device-resident image pairs in one call, such as the levels of a mip chain or a texture set against
+ * their decodes (astcenc_b200_decompress_device_images), with an optional per-block error map.
+ * What each entry gets: *metrics receives the figures astcenc_b200_compute_error_metrics returns for that pair alone, on host
+ * copies of the same images. sum_squared_error, rgb_peak, mean_angular_error, worst_angular_error and log_rmse are bit for bit
+ * the same. The dB figures (psnr, alpha_psnr, rgb_psnr, peak_psnr, mpsnr) are computed on the device, whose log10 may differ
+ * from the host's in the last bits: they agree within 1e-12 dB. Fields not requested are zero.
+ * The per-block error map: block_error, when not NULL, receives one float per block of the context's footprint
+ * (block_x / block_y / block_z) in astcenc_compress_image's block order, the index astcenc_b200_compress_device_blocks takes (a 2D
+ * footprint's z counts the slices of a texture array). Each value is the sum, over the block's texels inside the image, of the
+ * squared differences of the channels input_components selects, in the units of sum_squared_error (U8 scaled to 0..1, F16 / F32
+ * clamped to [0, 65504]); it is accumulated in double in a fixed order and rounded to float once, and depends only on that
+ * block's texels.
+ * The figures are deterministic and do not depend on which other entries share the call or on their order. The call is
+ * enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in order with every other pass of the
+ * context. Works on decompress-only contexts. No progress callback, no cancellation. image_count == 0 does nothing. The
+ * descriptor array is copied: the caller may free it when the call returns. Outputs must not overlap any input (not checked).
+ * Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_PARAM for a NULL context or
+ * input_components outside 1-4, then for fstop_lo < -125 or fstop_hi > 125, then for images == NULL with a non-zero count, then
+ * for an entry with a NULL original, decoded or metrics, a zero or overflowing dimension, a bad data type, or a pointer not
+ * aligned to its element (4 / 8 / 16 bytes for a U8 / F16 / F32 texel, 8 for metrics, 4 for block_error; decode outputs of
+ * one type packed tightly into a cudaMalloc buffer always are), then when the call does not fit a launch (an image with 2^32
+ * blocks or more that asks for a map, or a grid beyond 2^31 - 1 CTAs). All entries are checked before anything is enqueued.
+ * The table goes up in one small copy; the call is two kernel launches, three when any entry asks for a map.
+ */
+struct astcenc_b200_device_metrics_image {
+	const void* original;                         /* device: dim_z slices of dim_x * dim_y texels of original_type, contiguous */
+	const void* decoded;                          /* device: the same shape, texels of decoded_type */
+	enum astcenc_type original_type, decoded_type;
+	unsigned int dim_x, dim_y, dim_z;
+	struct astcenc_b200_error_metrics* metrics;   /* device: receives this image's figures */
+	float* block_error;                           /* device, or NULL: one float per block of the context's footprint */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_error_metrics_device_images(struct astcenc_context* context, int compute_hdr_metrics,
+                                                                                  int compute_normal_metrics, int input_components,
+                                                                                  const struct astcenc_b200_device_metrics_image* images,
+                                                                                  unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream);
+
+/**
  * The .astc container (Docs/FileFormat.md; Source/astcenccli_image_load_store.cpp:2573-2760, load_cimage / store_cimage):
  * a 16-byte header - magic 13 AB A1 5C, block dimensions (one byte each), image dimensions (24 bits each, little endian)
  * - followed by the blocks as astcenc_compress_image() wrote them.

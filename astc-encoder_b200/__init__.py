@@ -78,6 +78,18 @@ class DeviceMetricsImage(C.Structure):
                 ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("metrics", C.c_void_p), ("block_error", C.c_void_p)]
 
 
+class BlockSelection(C.Structure):
+    """struct astcenc_b200_block_selection (include/astcenc.h)."""
+    _fields_ = [("map", C.c_void_p), ("block_count", C.c_uint), ("threshold", C.c_float), ("capacity", C.c_uint), ("indices", C.c_void_p),
+                ("count", C.c_void_p)]
+
+
+class DeviceBlockList(C.Structure):
+    """struct astcenc_b200_device_block_list (include/astcenc.h)."""
+    _fields_ = [("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("payload", C.c_void_p), ("indices", C.c_void_p),
+                ("count", C.c_void_p), ("capacity", C.c_uint)]
+
+
 class ErrorMetrics(C.Structure):
     """struct astcenc_b200_error_metrics (include/astcenc.h)."""
     _fields_ = [(n, C.c_double) for n in ("psnr", "alpha_psnr", "rgb_psnr", "rgb_peak", "peak_psnr", "mpsnr", "log_rmse",
@@ -149,6 +161,10 @@ def lib():
         l.astcenc_b200_compute_error_metrics_device_images.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(DeviceMetricsImage), C.c_uint,
                                                                        C.c_int, C.c_int, C.c_void_p]
         l.astcenc_b200_compute_error_metrics_device_images.restype = C.c_int
+        l.astcenc_b200_select_blocks.argtypes = [C.c_void_p, C.POINTER(BlockSelection), C.c_uint, C.c_void_p]
+        l.astcenc_b200_select_blocks.restype = C.c_int
+        l.astcenc_b200_compress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
+        l.astcenc_b200_compress_device_block_lists.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -456,6 +472,30 @@ class Context:
                                                                      fstop_lo, fstop_hi, C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compute_error_metrics_device_images")
+
+    def select_blocks(self, entries, stream=0):
+        """Block selection from device maps (astcenc_b200_select_blocks). entries: a sequence of (d_map_ptr, block_count,
+        threshold, capacity, d_indices_ptr, d_count_ptr); each keeps the min(capacity, candidates) largest values above its
+        threshold, ties to the lower index, and writes their indices ascending and their number. Enqueued on `stream`, no sync;
+        works on any context."""
+        n = len(entries)
+        table = (BlockSelection * n)(*[BlockSelection(C.c_void_p(m or None), b, t, c, C.c_void_p(i or None), C.c_void_p(k or None))
+                                       for m, b, t, c, i, k in entries])
+        err = lib().astcenc_b200_select_blocks(self.handle, table if n else None, n, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_select_blocks")
+
+    def compress_device_block_lists(self, lists, data_type, swizzle=(0, 1, 2, 3), stream=0):
+        """Recompress device-resident block lists (astcenc_b200_compress_device_block_lists). lists: a sequence of
+        (d_pixels_ptr, dim_x, dim_y, dim_z, d_payload_ptr, d_indices_ptr, d_count_ptr, capacity); the first min(*count, capacity)
+        indices in range are recompressed into the payload, in place. Enqueued on `stream`, no sync."""
+        n = len(lists)
+        table = (DeviceBlockList * n)(*[DeviceBlockList(C.c_void_p(p), x, y, z, C.c_void_p(q), C.c_void_p(i or None), C.c_void_p(k or None), c)
+                                        for p, x, y, z, q, i, k, c in lists])
+        sw = Swizzle(*swizzle)
+        err = lib().astcenc_b200_compress_device_block_lists(self.handle, table if n else None, n, data_type, C.byref(sw), C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compress_device_block_lists")
 
     def last_timing(self):
         ms = C.c_float(); a = C.c_size_t(); b = C.c_size_t()

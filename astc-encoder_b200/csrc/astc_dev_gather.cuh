@@ -13,6 +13,12 @@
 // gather and the scatter find j by binary search over first[]. A chunk of the call (GatherArgs::base) may span several images,
 // and an image several chunks.
 //
+// Device block lists (astcenc_b200_compress_device_block_lists) are image tables whose entry j owns capacity[j] staging blocks
+// (first[] is the prefix sum of the capacities, which the host knows) and a GatherList beside its GatherImage. Staging block c
+// is slot s = c - first[j] of list j: block indices[s] of image j while s < min(*count, capacity) and that index lies inside the
+// image. Any other slot is invalid: the gather stages all-zero texels and zero alpha averages for it, which the pipeline emits
+// as a constant block in wave 0, and the scatter writes nothing for it.
+//
 // A decode call (astcenc_b200_decompress_device_images) walks the same kind of table: each entry's payload is read and its data
 // written.
 #pragma once
@@ -25,6 +31,14 @@ struct GatherImage {
 	size_t avg_offset;          // where the image's alpha-scale averages start in GatherArgs::avg_src
 	unsigned int dim_x, dim_y, dim_z;
 	unsigned int blocks_x, blocks_y;
+};
+
+// The device list of one entry of a block-list table (beside its GatherImage).
+struct GatherList {
+	const uint32_t* indices;    // device: block positions in the image's payload order
+	const uint32_t* count;      // device: how many of them are listed (at most `capacity` are read)
+	unsigned int capacity;
+	unsigned int blocks;        // the image's block count: indices at or beyond it are skipped
 };
 
 struct GatherArgs {
@@ -43,7 +57,21 @@ struct GatherArgs {
 	const GatherImage* images = nullptr;
 	unsigned int image_count = 0;
 	size_t base = 0;
+	// A block-list table: entry j's staging blocks are the slots of lists[j] (null: every block of each image).
+	const GatherList* lists = nullptr;
 };
+
+#define GATHER_INVALID 0xFFFFFFFFu
+
+// The block of slot s of list l, or GATHER_INVALID for a slot past min(*count, capacity) or an index beyond the image.
+ASTC_FN uint32_t list_slot(const GatherList& l, size_t s) {
+	const uint32_t count = ASTC_LDG(l.count);
+	if (s >= (count < l.capacity ? count : l.capacity)) {
+		return GATHER_INVALID;
+	}
+	const uint32_t index = ASTC_LDG(l.indices + s);
+	return index < l.blocks ? index : GATHER_INVALID;
+}
 
 // Texel t (x fastest, then y, then z) of listed block i: where it comes from in the source image (a texel index, clamped to the
 // image's edges) and where it goes in the staging image. inside: the unclamped texel lies in the image (block_has_alpha counts
@@ -128,7 +156,25 @@ ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lan
 		gather_footprint(g, i, ASTC_LDG(g.indices + i), lane, lanes);
 		return;
 	}
-	const GatherImage& im = g.images[table_image(g, i)];
+	const unsigned int j = table_image(g, i);
+	const GatherImage& im = g.images[j];
+	uint32_t index = (uint32_t)(g.base + i - im.first);      // (an image has fewer than 2^32 blocks)
+	if (g.lists != nullptr) {
+		index = list_slot(g.lists[j], g.base + i - im.first);
+		if (index == GATHER_INVALID) {
+			// zero texels and averages: a constant block, emitted in wave 0 and never scattered
+			const unsigned int T = g.bx * g.by * g.bz;
+			uint32_t* dst = static_cast<uint32_t*>(g.dst);
+			for (unsigned int w = (unsigned int)lane; w < T * g.words; w += (unsigned int)lanes) {
+				unsigned int t = w / g.words, k = w - t * g.words;
+				dst[gather_texel(g, i, 0, t).dst * g.words + k] = 0u;
+			}
+			for (unsigned int t = (unsigned int)lane; t < T && g.avg_dst != nullptr; t += (unsigned int)lanes) {
+				g.avg_dst[gather_texel(g, i, 0, t).dst] = 0.0f;
+			}
+			return;
+		}
+	}
 	GatherArgs s = g;
 	s.src = im.data;
 	s.avg_src = g.avg_src != nullptr ? g.avg_src + im.avg_offset : nullptr;
@@ -137,15 +183,21 @@ ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lan
 	s.dim_z = im.dim_z;
 	s.blocks_x = im.blocks_x;
 	s.blocks_y = im.blocks_y;
-	gather_footprint(s, i, (uint32_t)(g.base + i - im.first), lane, lanes);      // (an image has fewer than 2^32 blocks)
+	gather_footprint(s, i, index, lane, lanes);
 }
 
-// Where staging block i goes: the payload position of listed block i, or of its block of an image table.
+// Where staging block i goes: the payload position of listed block i, or of its block of an image table; null for an invalid
+// slot of a block-list table.
 ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i, uint8_t* payload) {
 	if (g.images == nullptr) {
 		return payload + (size_t)ASTC_LDG(g.indices + i) * 16;
 	}
-	const GatherImage& im = g.images[table_image(g, i)];
+	const unsigned int j = table_image(g, i);
+	const GatherImage& im = g.images[j];
+	if (g.lists != nullptr) {
+		const uint32_t index = list_slot(g.lists[j], g.base + i - im.first);
+		return index == GATHER_INVALID ? nullptr : im.payload + (size_t)index * 16;
+	}
 	return im.payload + (g.base + i - im.first) * 16;
 }
 

@@ -23,6 +23,7 @@
 #include "astc_dev_search.cuh"
 #include "astc_dev_gather.cuh"
 #include "astc_dev_metrics.cuh"
+#include "astc_dev_select.cuh"
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
 #include "astc_host_slab.h"
@@ -224,6 +225,9 @@ astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_cons
 		return;
 	}
 	uint8_t* dst = scatter_target(g, i, payload);
+	if (dst == nullptr) {
+		return;      // (an invalid slot of a device block list)
+	}
 	uint4 v = __ldg(reinterpret_cast<const uint4*>(staged) + i);
 	if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
 		*reinterpret_cast<uint4*>(dst) = v;
@@ -412,6 +416,8 @@ struct astcenc_context {
 	DevBuffer list, list_image, list_out, list_alpha;
 	// metrics calls: the partial sums of every virtual CTA and the sums of every pair, grown on demand
 	DevBuffer metric_partials;
+	// selection calls: the entries, their histograms and the tile counts
+	DevBuffer select;
 	// The per-context scratch (records, queues, counters, alpha averages, table and staging buffers) serves ONE pass at a time
 	// (scratch_turn): launch_mtx serialises the host side, scratch_done orders a pass on one stream behind the previous pass on
 	// another.
@@ -653,7 +659,7 @@ void astcenc_context_free(astcenc_context* ctx) {
 	cudaFree(ctx->d_ticket);
 	cudaFree(ctx->d_counters);
 	for (DevBuffer* b : {&ctx->records, &ctx->queues, &ctx->alpha, &ctx->image, &ctx->image2, &ctx->out, &ctx->list, &ctx->list_image, &ctx->list_out,
-	                     &ctx->list_alpha, &ctx->metric_partials}) {
+	                     &ctx->list_alpha, &ctx->metric_partials, &ctx->select}) {
 		cudaFree(b->ptr);
 	}
 	for (cudaEvent_t e : ctx->stage_events) {
@@ -1689,6 +1695,7 @@ struct BlockCall {
 	std::vector<DevImage> srcs;
 	std::vector<GatherImage> table;
 	std::vector<uint32_t> list;
+	std::vector<GatherList> lists;     // (device block lists) one per table entry, whose staging blocks are its list's slots
 	unsigned int row_lo = 0, row_hi = 0;
 	size_t blocks = 0;                 // staging blocks of the whole call
 	size_t texel_bytes = 0;
@@ -1711,7 +1718,8 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	for (const DevImage& s : call.srcs) {
 		avg_floats += (size_t)s.dim_x * s.dim_y;
 	}
-	const size_t list_bytes = table ? call.table.size() * sizeof(GatherImage) : n * sizeof(uint32_t);
+	const size_t table_bytes = call.table.size() * sizeof(GatherImage);
+	const size_t list_bytes = table ? table_bytes + call.lists.size() * sizeof(GatherList) : n * sizeof(uint32_t);
 	astcenc_error st = ensure_buffer(ctx->list, list_bytes);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * call.texel_bytes);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
@@ -1722,6 +1730,13 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	if (st == ASTCENC_SUCCESS) {
 		// (from pageable memory: staged by the driver before the call returns, so the list or table may go when this function does)
 		const void* host = table ? static_cast<const void*>(call.table.data()) : static_cast<const void*>(call.list.data());
+		std::vector<uint8_t> up;
+		if (!call.lists.empty()) {      // (the table, then the lists, in one copy)
+			up.resize(list_bytes);
+			memcpy(up.data(), call.table.data(), table_bytes);
+			memcpy(up.data() + table_bytes, call.lists.data(), list_bytes - table_bytes);
+			host = up.data();
+		}
 		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, host, list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
 	// The staging pass reads averages gathered from the sources', so it runs no pre-pass of its own: its box filter would reach
@@ -1750,6 +1765,7 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	g.bz = bsd.dim_z;
 	g.images = table ? ctx->list.as<const GatherImage>() : nullptr;
 	g.image_count = (unsigned int)call.table.size();
+	g.lists = call.lists.empty() ? nullptr : reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes);
 	for (size_t first = 0; first < n && st == ASTCENC_SUCCESS; first += chunk) {
 		const unsigned int m = (unsigned int)(n - first < chunk ? n - first : chunk);
 		g.indices = table ? nullptr : ctx->list.as<const uint32_t>() + first;
@@ -2036,6 +2052,127 @@ astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* 
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return scratch_turn(ctx, s, [&] {
 		return launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, fstop_lo, fstop_hi, s);
+	});
+}
+
+// Device block lists: an image table whose entry j owns capacity[j] staging blocks, the slots of its device list (GatherList).
+// Checked whole before anything is enqueued, in the image-table order of astcenc_b200_compress_device_images; entries with a
+// capacity of 0 are checked and then left out of the call.
+astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count,
+                                                       astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
+	if (status == ASTCENC_SUCCESS && list_count != 0 && !lists) status = ASTCENC_ERR_BAD_PARAM;
+	auto aligned4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; };
+	std::vector<astcenc_b200_device_image> descs;
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		const astcenc_b200_device_block_list& l = lists[i];
+		if (!l.data || !l.payload || (l.capacity != 0 && (!l.indices || !l.count)) || !aligned4(l.indices) || !aligned4(l.count)) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		}
+		descs.push_back({l.data, l.dim_x, l.dim_y, l.dim_z, l.payload});
+	}
+	BlockCall all;
+	if (status == ASTCENC_SUCCESS) status = plan_image_table(ctx, descs.data(), list_count, data_type, *swizzle, all);
+	if (status != ASTCENC_SUCCESS) {
+		return status;
+	}
+	// the call: the entries with a non-zero capacity, their staging blocks numbered by the prefix sum of the capacities
+	BlockCall call;
+	call.texel_bytes = all.texel_bytes;
+	size_t avg_offset = 0;
+	for (unsigned int i = 0; i < list_count; i++) {
+		const astcenc_b200_device_block_list& l = lists[i];
+		if (l.capacity == 0) {
+			continue;
+		}
+		if (l.capacity > SIZE_MAX - call.blocks) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		GatherImage e = all.table[i];
+		const size_t end = i + 1 < list_count ? all.table[i + 1].first : all.blocks;
+		e.first = call.blocks;
+		e.avg_offset = avg_offset;
+		call.table.push_back(e);
+		call.srcs.push_back(all.srcs[i]);
+		call.lists.push_back({l.indices, l.count, l.capacity, (unsigned int)(end - all.table[i].first)});
+		call.blocks += l.capacity;
+		avg_offset += (size_t)l.dim_x * l.dim_y;
+	}
+	if (call.blocks == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return launch_blocks(ctx, call, *swizzle, s);
+}
+
+// Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table goes
+// up, the histograms are cleared and SELECT_KERNELS kernels run, whatever the number of entries.
+astcenc_error astcenc_b200_select_blocks(astcenc_context* ctx, const astcenc_b200_block_selection* entries, unsigned int entry_count, void* cuda_stream) {
+	if (!ctx || (entry_count != 0 && !entries)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	auto aligned4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; };
+	std::vector<SelectEntry> table(entry_count);
+	for (unsigned int i = 0; i < entry_count; i++) {
+		const astcenc_b200_block_selection& x = entries[i];
+		if (!x.count || (x.block_count != 0 && !x.map) || (x.capacity != 0 && !x.indices) || !aligned4(x.map) || !aligned4(x.indices) ||
+		    !aligned4(x.count) || x.threshold != x.threshold) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		SelectEntry& e = table[i];
+		e.map = x.map;
+		e.indices = x.indices;
+		e.count = x.count;
+		e.threshold = x.threshold;
+		e.capacity = x.capacity;
+		e.block_count = x.block_count;
+	}
+	if (entry_count == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	const size_t tiles = plan_select(table);
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return scratch_turn(ctx, s, [&]() -> astcenc_error {
+		const size_t table_bytes = table.size() * sizeof(SelectEntry);
+		const size_t hist_bytes = table.size() * 1024 * sizeof(uint32_t);
+		astcenc_error r = ensure_buffer(ctx->select, table_bytes + hist_bytes + tiles * 2 * sizeof(uint32_t));
+		if (r != ASTCENC_SUCCESS) {
+			return r;
+		}
+		// (from pageable memory: staged by the driver before the call returns)
+		CUDA_TRY(cudaMemcpyAsync(ctx->select.ptr, table.data(), table_bytes, cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaMemsetAsync(ctx->select.ptr + table_bytes, 0, hist_bytes, s), return ASTCENC_ERR_BAD_CONTEXT);
+		SelectArgs a;
+		a.entries = ctx->select.as<const SelectEntry>();
+		a.count = entry_count;
+		a.tiles = tiles;
+		a.hist = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes);
+		a.tile_counts = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes + hist_bytes);
+		// grid-stride launches of SELECT_WARPS warps per CTA, at least one CTA, so that every call makes the same launches
+		const size_t cap = (size_t)ctx->sm_count * 16;
+		auto grid = [cap](size_t warps) {
+			const size_t g = (warps + SELECT_WARPS - 1) / SELECT_WARPS;
+			return (unsigned int)(g == 0 ? 1 : g < cap ? g : cap);
+		};
+		for (int digit = 0; digit < 4; digit++) {
+			astc_select_hist_kernel<<<grid(tiles), SELECT_WARPS * 32, 0, s>>>(a, digit);
+		}
+		astc_select_count_kernel<<<grid(tiles), SELECT_WARPS * 32, 0, s>>>(a);
+		astc_select_scan_kernel<<<grid(entry_count), SELECT_WARPS * 32, 0, s>>>(a);
+		astc_select_write_kernel<<<grid(tiles), SELECT_WARPS * 32, 0, s>>>(a);
+		ctx->launches += SELECT_KERNELS;
+		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+		return ASTCENC_SUCCESS;
 	});
 }
 

@@ -409,6 +409,70 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_error_metrics_device_imag
                                                                                   unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream);
 
 /**
+ * Block selection on the device: turn per-block error maps (astcenc_b200_compute_error_metrics_device_images) into device block
+ * lists (astcenc_b200_compress_device_block_lists) without a trip through host memory.
+ * One rule per entry: a block is a candidate when map[b] > threshold (NaN never is; -0.0 counts as 0.0). Of c candidates the
+ * k = min(capacity, c) largest values are kept, ties going to the lower block index; their indices are written to indices[0, k)
+ * in ascending order, *count receives k, and indices past k are left untouched. A threshold of -INFINITY with capacity k gives
+ * the k worst blocks; a finite threshold with a large capacity gives every block worse than the threshold. In numpy terms, with
+ * m[~(m > threshold)] = -inf: np.sort(np.argsort(-m, kind="stable")[:k]).
+ * Each entry's output depends only on that entry, never on the other entries of the call or on the GPU. The call is a radix
+ * select over the values' 32-bit keys and an ordered compaction: one memset and 7 kernel launches, whatever the number of
+ * entries, reading each map six times. It uses the context's scratch and works on any context, decompress-only ones included.
+ * Enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in order with every other pass of the
+ * context. The descriptor array is copied: the caller may free it when the call returns. Outputs must not overlap any map or
+ * each other (not checked). entry_count == 0 does nothing.
+ * Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_PARAM for a NULL context or
+ * entries == NULL with a non-zero count, then for an entry with a NULL count, a NULL map with block_count > 0, NULL indices
+ * with capacity > 0, a pointer not aligned to 4 bytes or a NaN threshold. All entries are checked before anything is enqueued.
+ */
+struct astcenc_b200_block_selection {
+	const float* map;              /* device: block_count values, e.g. a per-block error map */
+	unsigned int block_count;
+	float threshold;               /* candidates are the values above it; -INFINITY: every value but NaN and -INFINITY */
+	unsigned int capacity;         /* at most this many blocks are kept */
+	uint32_t* indices;             /* device: receives the kept block indices, ascending (room for capacity) */
+	uint32_t* count;               /* device: receives how many were kept */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_select_blocks(struct astcenc_context* context, const struct astcenc_b200_block_selection* entries,
+                                                             unsigned int entry_count, void* cuda_stream);
+
+/**
+ * Recompress block lists that live in device memory, such as the output of astcenc_b200_select_blocks or a GPU tool's list of
+ * dirty tiles, for many device-resident images in shared pipeline passes.
+ * lists[i] describes an image ALREADY RESIDENT in device memory (data: dim_z slices of dim_x * dim_y texels, contiguous; the
+ * shapes astcenc_compress_image takes), its device payload, a device index list and a device count. The call reads the first
+ * min(*count, capacity) indices; an index at or beyond the image's block count is skipped. Each listed block's 16 bytes are
+ * written, the bytes astcenc_compress_image writes for that block; every other byte of the payload is left untouched, and
+ * duplicate indices write the same bytes. A one-entry call is the single-image case. All entries share data_type and swizzle;
+ * payloads must not overlap (not checked). The descriptor array is copied. Enqueued on `cuda_stream` (0 = the context's own
+ * stream), without synchronising, in order with every other pass of the context: *count and the indices are read on the device
+ * when the call runs. No progress callback, no cancellation.
+ * Cost: the host does not know the counts, so a call costs what astcenc_b200_compress_device_images costs over the sum of
+ * the capacities, not over the counts: each entry owns `capacity` staging blocks, and a slot past the count (or with an index
+ * out of range) is staged as an all-zero block, which the pipeline finishes as a constant block in its first wave and which is
+ * never written back. With a_scale_radius (2D block sizes) each entry gets an alpha-scale pre-pass over its whole image, one
+ * extra launch per entry. Entries with capacity == 0 do nothing; a call whose capacities are all zero launches nothing.
+ * Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_CONTEXT for a decompress-only
+ * context; ASTCENC_ERR_BAD_PARAM for a NULL swizzle, then ASTCENC_ERR_BAD_SWIZZLE; ASTCENC_ERR_BAD_PARAM for lists == NULL with
+ * a non-zero count, or an entry with a NULL data or payload, a NULL indices or count with capacity > 0, indices or count not
+ * aligned to 4 bytes, a zero dimension, or a bad data type; ASTCENC_ERR_NOT_IMPLEMENTED for a_scale_radius on a texture array;
+ * ASTCENC_ERR_BAD_PARAM for an image of 2^32 blocks or more, or when the sum of the capacities overflows. All entries are checked
+ * before anything is enqueued.
+ */
+struct astcenc_b200_device_block_list {
+	const void* data;              /* device: dim_z slices of dim_x * dim_y texels, contiguous */
+	unsigned int dim_x, dim_y, dim_z;
+	uint8_t* payload;              /* device: the image's whole payload, astcenc_compress_image's block order */
+	const uint32_t* indices;       /* device: block positions in that order */
+	const uint32_t* count;         /* device: how many of the indices are listed */
+	unsigned int capacity;         /* at most this many indices are read; the call's cost */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device_block_lists(struct astcenc_context* context, const struct astcenc_b200_device_block_list* lists,
+                                                                          unsigned int list_count, enum astcenc_type data_type,
+                                                                          const struct astcenc_swizzle* swizzle, void* cuda_stream);
+
+/**
  * The .astc container (Docs/FileFormat.md; Source/astcenccli_image_load_store.cpp:2573-2760, load_cimage / store_cimage):
  * a 16-byte header - magic 13 AB A1 5C, block dimensions (one byte each), image dimensions (24 bits each, little endian)
  * - followed by the blocks as astcenc_compress_image() wrote them.

@@ -1,39 +1,37 @@
-// CUDA-native ASTC: block lists (astcenc_b200_compress_device_blocks) and image tables. A block's 16 bytes depend on its texels after clamp-to-edge,
-// the alpha-scale test over its footprint and the context - not on where it sits (void extents carry no coordinates, partition
-// tables are indexed by seed). So the listed blocks are copied, footprint by footprint, into a staging image that is ONE ROW of
-// blocks, an ordinary pass of the wave pipeline compresses that row, and a scatter puts staging block i at the listed position.
-// The stage kernels never see the list.
+// CUDA-native ASTC: staging calls over block-list tables (astcenc_b200_compress_device_images, astcenc_b200_compress_images,
+// astcenc_b200_compress_device_block_lists, astcenc_b200_compress_device_blocks). A block's 16 bytes depend on its texels after
+// clamp-to-edge, the alpha-scale test over its footprint and the context - not on where it sits (void extents carry no
+// coordinates, partition tables are indexed by seed). So the call's blocks are copied, footprint by footprint, into a staging
+// image that is ONE ROW of blocks, an ordinary pass of the wave pipeline compresses that row, and a scatter puts each staging
+// block at its payload position. The stage kernels never see the table.
 //
-// Staging layout of n listed blocks of a bx x by (x bz) footprint: (n * bx) x by texels (x bz slices for 3D block sizes), block i
-// at x = i * bx. Every staged texel lies inside the staging image, so load_block reads it without clamping; the gather has done
-// the clamping against the source image, exactly as load_block clamps in place (astcenc_image.cpp:162-342).
+// Staging layout of n blocks of a bx x by (x bz) footprint: (n * bx) x by texels (x bz slices for 3D block sizes), block i at
+// x = i * bx. Every staged texel lies inside the staging image, so load_block reads it without clamping; the gather has done the
+// clamping against the source image, exactly as load_block clamps in place (astcenc_image.cpp:162-342).
 //
-// Image tables (astcenc_b200_compress_device_images) stage every block of several images the same way. Staging block c of a call
-// is block c - first[j] of image j, where first[] is the exclusive prefix sum of the images' block counts in call order; the
-// gather and the scatter find j by binary search over first[]. A chunk of the call (GatherArgs::base) may span several images,
-// and an image several chunks.
+// Entry j of the table owns the call's staging blocks [first[j], first[j + 1]): every block of image j in payload order, or,
+// when the call has lists, the capacity[j] slots of list j. Staging block c is then slot s = c - first[j] of list j: block
+// indices[s] of image j while s < min(*count, capacity) and that index lies inside the image. Any other slot is invalid: the
+// gather stages all-zero texels and zero alpha averages for it, which the pipeline emits as a constant block in wave 0, and the
+// scatter writes nothing for it. The gather and the scatter find j by binary search over first[]. A chunk of the call
+// (GatherArgs::base) may span several entries, and an entry several chunks. A host list of n blocks of one image is a one-entry
+// table whose list has capacity n and *count n.
 //
-// Device block lists (astcenc_b200_compress_device_block_lists) are image tables whose entry j owns capacity[j] staging blocks
-// (first[] is the prefix sum of the capacities, which the host knows) and a GatherList beside its GatherImage. Staging block c
-// is slot s = c - first[j] of list j: block indices[s] of image j while s < min(*count, capacity) and that index lies inside the
-// image. Any other slot is invalid: the gather stages all-zero texels and zero alpha averages for it, which the pipeline emits
-// as a constant block in wave 0, and the scatter writes nothing for it.
-//
-// A decode call (astcenc_b200_decompress_device_images) walks the same kind of table: each entry's payload is read and its data
-// written.
+// A decode call (astcenc_b200_decompress_device_images) walks the same kind of table without lists: each entry's payload is
+// read and its data written.
 #pragma once
 
 // One image of an image table.
 struct GatherImage {
 	const void* data;           // dim_z slices of dim_x * dim_y texels, contiguous
 	uint8_t* payload;           // the image's whole payload
-	size_t first;               // call block of the image's block 0
+	size_t first;               // call block of the entry's first staging block (decode: of the image's block 0)
 	size_t avg_offset;          // where the image's alpha-scale averages start in GatherArgs::avg_src
 	unsigned int dim_x, dim_y, dim_z;
 	unsigned int blocks_x, blocks_y;
 };
 
-// The device list of one entry of a block-list table (beside its GatherImage).
+// The list of one entry of a block-list table (beside its GatherImage).
 struct GatherList {
 	const uint32_t* indices;    // device: block positions in the image's payload order
 	const uint32_t* count;      // device: how many of them are listed (at most `capacity` are read)
@@ -42,38 +40,30 @@ struct GatherList {
 };
 
 struct GatherArgs {
-	const void* src;            // the caller's image: dim_z slices of dim_x * dim_y texels, contiguous
 	void* dst;                  // the staging image
-	const float* avg_src;       // alpha-scale averages of source slice 0 at image positions (dim_x * dim_y), or null
+	const float* avg_src;       // alpha-scale averages of every entry's slice 0 at image positions (dim_x * dim_y each), or null
 	float* avg_dst;             // the averages in the staging layout ((n * bx) x by), or null
-	const uint32_t* indices;    // the listed blocks (positions in z, y, x order: astcenc_entry.cpp:1036)
-	unsigned int n;             // listed blocks of this gather
+	unsigned int n;             // staging blocks of this gather
 	unsigned int words;         // 32-bit words per texel: 1 (U8), 2 (F16), 4 (F32)
-	unsigned int dim_x, dim_y, dim_z;
-	unsigned int blocks_x, blocks_y;
 	unsigned int bx, by, bz;    // footprint; bz = 1 for 2D block sizes, whose block index then counts slice z of a texture array
-	// An image table: staging block i is call block base + i of `images` (whose entries replace src, avg_src's offset and the
-	// dims above). Null: one source image and the index list.
-	const GatherImage* images = nullptr;
-	unsigned int image_count = 0;
-	size_t base = 0;
-	// A block-list table: entry j's staging blocks are the slots of lists[j] (null: every block of each image).
-	const GatherList* lists = nullptr;
+	// staging block i is call block base + i of the table
+	const GatherImage* images;
+	unsigned int image_count;
+	size_t base;
+	const GatherList* lists;    // one per entry, or null: every block of each image
 };
 
 #define GATHER_INVALID 0xFFFFFFFFu
 
-// The block of slot s of list l, or GATHER_INVALID for a slot past min(*count, capacity) or an index beyond the image.
+// The block of slot s < capacity of list l, or GATHER_INVALID for a slot past min(*count, capacity) or an index beyond the image.
+// (The slot is read together with the count: it lies inside the list's capacity either way.)
 ASTC_FN uint32_t list_slot(const GatherList& l, size_t s) {
 	const uint32_t count = ASTC_LDG(l.count);
-	if (s >= (count < l.capacity ? count : l.capacity)) {
-		return GATHER_INVALID;
-	}
 	const uint32_t index = ASTC_LDG(l.indices + s);
-	return index < l.blocks ? index : GATHER_INVALID;
+	return s < (count < l.capacity ? count : l.capacity) && index < l.blocks ? index : GATHER_INVALID;
 }
 
-// Texel t (x fastest, then y, then z) of listed block i: where it comes from in the source image (a texel index, clamped to the
+// Texel t (x fastest, then y, then z) of a staged block: where it comes from in the source image (a texel index, clamped to the
 // image's edges) and where it goes in the staging image. inside: the unclamped texel lies in the image (block_has_alpha counts
 // only those).
 struct GatherTexel {
@@ -95,16 +85,17 @@ ASTC_FN void footprint_texel(unsigned int blocks_x, unsigned int blocks_y, unsig
 	x = col * bx + tx, y = row * by + ty, z = layer * bz + tz;
 }
 
-ASTC_FN GatherTexel gather_texel(const GatherArgs& g, unsigned int i, uint32_t index, unsigned int t) {
+// Texel t of block `index` of image im, staged as staging block i.
+ASTC_FN GatherTexel gather_texel(const GatherArgs& g, const GatherImage& im, unsigned int i, uint32_t index, unsigned int t) {
 	unsigned int tx, ty, tz, x, y, z;
-	footprint_texel(g.blocks_x, g.blocks_y, g.bx, g.by, g.bz, index, t, tx, ty, tz, x, y, z);
-	unsigned int xi = x < g.dim_x - 1 ? x : g.dim_x - 1;
-	unsigned int yi = y < g.dim_y - 1 ? y : g.dim_y - 1;
-	unsigned int zi = z < g.dim_z - 1 ? z : g.dim_z - 1;
+	footprint_texel(im.blocks_x, im.blocks_y, g.bx, g.by, g.bz, index, t, tx, ty, tz, x, y, z);
+	unsigned int xi = x < im.dim_x - 1 ? x : im.dim_x - 1;
+	unsigned int yi = y < im.dim_y - 1 ? y : im.dim_y - 1;
+	unsigned int zi = z < im.dim_z - 1 ? z : im.dim_z - 1;
 	GatherTexel r;
-	r.src = ((size_t)zi * g.dim_y + yi) * g.dim_x + xi;
+	r.src = ((size_t)zi * im.dim_y + yi) * im.dim_x + xi;
 	r.dst = ((size_t)tz * g.by + ty) * ((size_t)g.n * g.bx) + (size_t)i * g.bx + tx;
-	r.inside = x < g.dim_x && y < g.dim_y;
+	r.inside = x < im.dim_x && y < im.dim_y;
 	return r;
 }
 
@@ -125,80 +116,43 @@ ASTC_FN unsigned int find_image(const E* images, unsigned int image_count, size_
 	return lo;
 }
 
-// The table entry that holds staging block i.
-ASTC_FN unsigned int table_image(const GatherArgs& g, unsigned int i) {
-	return find_image(g.images, g.image_count, g.base + i);
+// Staging block i: the entry that holds it (j) and its block in the entry's image, or GATHER_INVALID for an invalid list slot.
+ASTC_FN uint32_t staged_block(const GatherArgs& g, unsigned int i, unsigned int& j) {
+	j = find_image(g.images, g.image_count, g.base + i);
+	const size_t s = g.base + i - g.images[j].first;
+	return g.lists != nullptr ? list_slot(g.lists[j], s) : (uint32_t)s;      // (an image has fewer than 2^32 blocks)
 }
 
-// Block `index` of the source described by g into staging block i, by the lanes of one warp (lane / lanes): the texels word by
-// word, so that consecutive lanes read consecutive words of a footprint row; then the alpha averages (0 for texels outside the
-// image).
-ASTC_FN void gather_footprint(const GatherArgs& g, unsigned int i, uint32_t index, int lane, int lanes) {
+// Staging block i, by the lanes of one warp (lane / lanes): the texels word by word, so that consecutive lanes read consecutive
+// words of a footprint row; then the alpha averages (0 for texels outside the image). An invalid slot stages zeros: a constant
+// block, emitted in wave 0 and never scattered. The host simulation calls it with 0 / 1 or on its 32 simulated lanes.
+ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lanes) {
+	unsigned int j;
+	const uint32_t index = staged_block(g, i, j);
+	const bool valid = index != GATHER_INVALID;
+	const GatherImage im = g.images[j];      // (a copy: the stores below cannot alias it, so its fields stay in registers)
 	const unsigned int T = g.bx * g.by * g.bz;
-	const uint32_t* src = static_cast<const uint32_t*>(g.src);
+	const uint32_t* src = static_cast<const uint32_t*>(im.data);
 	uint32_t* dst = static_cast<uint32_t*>(g.dst);
 	for (unsigned int w = (unsigned int)lane; w < T * g.words; w += (unsigned int)lanes) {
 		unsigned int t = w / g.words, k = w - t * g.words;
-		GatherTexel p = gather_texel(g, i, index, t);
-		dst[p.dst * g.words + k] = ASTC_LDG(src + p.src * g.words + k);
+		GatherTexel p = gather_texel(g, im, i, valid ? index : 0, t);
+		dst[p.dst * g.words + k] = valid ? ASTC_LDG(src + p.src * g.words + k) : 0u;
 	}
 	if (g.avg_dst != nullptr) {
+		const float* avg = g.avg_src + im.avg_offset;
 		for (unsigned int t = (unsigned int)lane; t < T; t += (unsigned int)lanes) {
-			GatherTexel p = gather_texel(g, i, index, t);
-			g.avg_dst[p.dst] = p.inside ? ASTC_LDG(g.avg_src + p.src) : 0.0f;
+			GatherTexel p = gather_texel(g, im, i, valid ? index : 0, t);
+			g.avg_dst[p.dst] = valid && p.inside ? ASTC_LDG(avg + p.src) : 0.0f;
 		}
 	}
 }
 
-// Staging block i: listed block i of the one source, or its block of an image table. The host simulation calls it with 0 / 1.
-ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lanes) {
-	if (g.images == nullptr) {
-		gather_footprint(g, i, ASTC_LDG(g.indices + i), lane, lanes);
-		return;
-	}
-	const unsigned int j = table_image(g, i);
-	const GatherImage& im = g.images[j];
-	uint32_t index = (uint32_t)(g.base + i - im.first);      // (an image has fewer than 2^32 blocks)
-	if (g.lists != nullptr) {
-		index = list_slot(g.lists[j], g.base + i - im.first);
-		if (index == GATHER_INVALID) {
-			// zero texels and averages: a constant block, emitted in wave 0 and never scattered
-			const unsigned int T = g.bx * g.by * g.bz;
-			uint32_t* dst = static_cast<uint32_t*>(g.dst);
-			for (unsigned int w = (unsigned int)lane; w < T * g.words; w += (unsigned int)lanes) {
-				unsigned int t = w / g.words, k = w - t * g.words;
-				dst[gather_texel(g, i, 0, t).dst * g.words + k] = 0u;
-			}
-			for (unsigned int t = (unsigned int)lane; t < T && g.avg_dst != nullptr; t += (unsigned int)lanes) {
-				g.avg_dst[gather_texel(g, i, 0, t).dst] = 0.0f;
-			}
-			return;
-		}
-	}
-	GatherArgs s = g;
-	s.src = im.data;
-	s.avg_src = g.avg_src != nullptr ? g.avg_src + im.avg_offset : nullptr;
-	s.dim_x = im.dim_x;
-	s.dim_y = im.dim_y;
-	s.dim_z = im.dim_z;
-	s.blocks_x = im.blocks_x;
-	s.blocks_y = im.blocks_y;
-	gather_footprint(s, i, index, lane, lanes);
-}
-
-// Where staging block i goes: the payload position of listed block i, or of its block of an image table; null for an invalid
-// slot of a block-list table.
-ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i, uint8_t* payload) {
-	if (g.images == nullptr) {
-		return payload + (size_t)ASTC_LDG(g.indices + i) * 16;
-	}
-	const unsigned int j = table_image(g, i);
-	const GatherImage& im = g.images[j];
-	if (g.lists != nullptr) {
-		const uint32_t index = list_slot(g.lists[j], g.base + i - im.first);
-		return index == GATHER_INVALID ? nullptr : im.payload + (size_t)index * 16;
-	}
-	return im.payload + (g.base + i - im.first) * 16;
+// Where staging block i goes in its image's payload; null for an invalid list slot.
+ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i) {
+	unsigned int j;
+	const uint32_t index = staged_block(g, i, j);
+	return index == GATHER_INVALID ? nullptr : g.images[j].payload + (size_t)index * 16;
 }
 
 // ---- image tables of a decode call (astc_decompress_images_kernel) ----

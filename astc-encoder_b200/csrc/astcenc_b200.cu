@@ -219,16 +219,16 @@ astc_gather_blocks_kernel(const __grid_constant__ GatherArgs g) {
 
 // staging block i -> its payload position (duplicate list entries write the same bytes); one thread per block
 __global__ void __launch_bounds__(ASTC_GATHER_THREADS)
-astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_constant__ GatherArgs g, uint8_t* payload) {
+astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_constant__ GatherArgs g) {
 	unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= g.n) {
 		return;
 	}
-	uint8_t* dst = scatter_target(g, i, payload);
+	const uint4 v = __ldg(reinterpret_cast<const uint4*>(staged) + i);      // (read while the target is looked up)
+	uint8_t* dst = scatter_target(g, i);
 	if (dst == nullptr) {
-		return;      // (an invalid slot of a device block list)
+		return;      // (an invalid list slot)
 	}
-	uint4 v = __ldg(reinterpret_cast<const uint4*>(staged) + i);
 	if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
 		*reinterpret_cast<uint4*>(dst) = v;
 	} else {
@@ -411,8 +411,8 @@ struct astcenc_context {
 	// staging buffers for the host-pointer API, grown on demand; image2 is the second image buffer of the batch API
 	// (double-buffered uploads)
 	DevBuffer image, image2, out;
-	// block lists (astcenc_b200_compress_device_blocks), grown on demand: the list, the staging image and payload of one chunk,
-	// the pre-pass averages of the source image
+	// staging calls (astc_dev_gather.cuh), grown on demand: the table with its lists, the staging image and payload of one chunk,
+	// the pre-pass averages of the source images
 	DevBuffer list, list_image, list_out, list_alpha;
 	// metrics calls: the partial sums of every virtual CTA and the sums of every pair, grown on demand
 	DevBuffer metric_partials;
@@ -1688,99 +1688,123 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 	return launch_slab(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, 1, *swizzle), block_row0, block_rows, d_out, s);
 }
 
-// What launch_blocks compresses: the listed blocks of one image (`list`), or every block of the images of `table`. `srcs` are
-// the source images as a pass reads them: the list's image, or one per table entry. Their alpha-scale pre-passes cover block
-// rows [row_lo, row_hi] of a list's image and the whole of each table image.
-struct BlockCall {
-	std::vector<DevImage> srcs;
-	std::vector<GatherImage> table;
-	std::vector<uint32_t> list;
-	std::vector<GatherList> lists;     // (device block lists) one per table entry, whose staging blocks are its list's slots
-	unsigned int row_lo = 0, row_hi = 0;
-	size_t blocks = 0;                 // staging blocks of the whole call
-	size_t texel_bytes = 0;
-	uint8_t* payload = nullptr;        // (lists) the image's payload
+// One entry of a staging call: an image and its payload (plan_blocks sets `first` and `avg_offset`), its list (null: every
+// block), the staging blocks it owns (the image's blocks, or the list's capacity) and the block rows [row0, row1) of its
+// alpha-scale pre-pass, clamped to the image: the rows a host list touches, else the whole image.
+struct BlockEntry {
+	GatherImage image{};
+	const GatherList* list = nullptr;
+	size_t blocks = 0;
+	unsigned int row0 = 0, row1 = 0xFFFFFFFFu;
 };
 
-// Block lists and image tables (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk
-// (a staging row is one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most
-// knobs.batch_blocks blocks). A chunk of an image table may span several images. The whole call is one scratch turn
-// (launch_blocks), like a launch_slab.
+// What launch_blocks compresses: a block-list table (astc_dev_gather.cuh). Entry j is table[j], lists[j] (no lists: every block
+// of each image) and the block rows of its alpha-scale pre-pass (rows[j]). `words` go up behind the lists: a host list's count
+// word and indices, at which its GatherList (count and indices null here) is pointed.
+struct BlockCall {
+	std::vector<GatherImage> table;
+	std::vector<GatherList> lists;
+	std::vector<std::pair<unsigned int, unsigned int>> rows;
+	std::vector<uint32_t> words;
+	size_t blocks = 0;                 // staging blocks of the whole call
+	int data_type = 0;
+};
+
+// The staging call of checked `entries`: each owns the staging blocks and averages that follow those of the entries before it;
+// entries of no staging blocks (lists of capacity 0) are left out. ASTCENC_ERR_BAD_PARAM when the total does not fit a size_t.
+static astcenc_error plan_blocks(const std::vector<BlockEntry>& entries, astcenc_type data_type, BlockCall& call) {
+	call.data_type = (int)data_type;
+	size_t avg_offset = 0;
+	for (const BlockEntry& en : entries) {
+		if (en.blocks == 0) {
+			continue;
+		}
+		if (en.blocks > SIZE_MAX - call.blocks) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		GatherImage e = en.image;
+		e.first = call.blocks;
+		e.avg_offset = avg_offset;
+		call.table.push_back(e);
+		if (en.list != nullptr) {
+			call.lists.push_back(*en.list);
+		}
+		call.rows.push_back({en.row0, en.row1 < e.blocks_y ? en.row1 : e.blocks_y});
+		call.blocks += en.blocks;
+		avg_offset += (size_t)e.dim_x * e.dim_y;
+	}
+	return ASTCENC_SUCCESS;
+}
+
+// Staging calls (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk (a staging
+// row is one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks
+// blocks). A chunk may span several entries. The whole call is one scratch turn (launch_blocks), like a launch_slab.
 static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	const bool volume = bsd.dim_z > 1;
-	const bool table = !call.table.empty();
-	const DevImage& src = call.srcs[0];
 	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
 	const size_t n = call.blocks;
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
-	size_t avg_floats = 0;
-	for (const DevImage& s : call.srcs) {
-		avg_floats += (size_t)s.dim_x * s.dim_y;
-	}
+	const size_t avg_floats = call.table.back().avg_offset + (size_t)call.table.back().dim_x * call.table.back().dim_y;
 	const size_t table_bytes = call.table.size() * sizeof(GatherImage);
-	const size_t list_bytes = table ? table_bytes + call.lists.size() * sizeof(GatherList) : n * sizeof(uint32_t);
+	const size_t lists_bytes = call.lists.size() * sizeof(GatherList);
+	const size_t list_bytes = table_bytes + lists_bytes + call.words.size() * sizeof(uint32_t);
 	astcenc_error st = ensure_buffer(ctx->list, list_bytes);
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * call.texel_bytes);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * texel_bytes(call.data_type));
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
 	if (st == ASTCENC_SUCCESS && radius != 0) {
 		st = ensure_buffer(ctx->list_alpha, avg_floats * sizeof(float));
 		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
 	if (st == ASTCENC_SUCCESS) {
-		// (from pageable memory: staged by the driver before the call returns, so the list or table may go when this function does)
-		const void* host = table ? static_cast<const void*>(call.table.data()) : static_cast<const void*>(call.list.data());
-		std::vector<uint8_t> up;
-		if (!call.lists.empty()) {      // (the table, then the lists, in one copy)
-			up.resize(list_bytes);
-			memcpy(up.data(), call.table.data(), table_bytes);
-			memcpy(up.data() + table_bytes, call.lists.data(), list_bytes - table_bytes);
-			host = up.data();
+		// the table, its lists and the words in one copy, from pageable memory: staged by the driver before the call returns, so
+		// a host list may go when this function does
+		std::vector<GatherList> lists = call.lists;
+		for (GatherList& l : lists) {
+			if (l.count == nullptr) {
+				l.count = reinterpret_cast<const uint32_t*>(ctx->list.ptr + table_bytes + lists_bytes);
+				l.indices = l.count + 1;
+			}
 		}
-		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, host, list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(call.table.data()), reinterpret_cast<const uint8_t*>(call.table.data()) + table_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(lists.data()), reinterpret_cast<const uint8_t*>(lists.data()) + lists_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.words.data()), reinterpret_cast<const uint8_t*>(call.words.data()) + call.words.size() * sizeof(uint32_t));
+		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
 	// The staging pass reads averages gathered from the sources', so it runs no pre-pass of its own: its box filter would reach
-	// across the seams between unrelated blocks. A source's averages cover the staged blocks' rows, at their image positions, in
-	// the source's region of list_alpha. The threshold depends on the footprint and the radius alone: one value serves every source.
+	// across the seams between unrelated blocks. A source's averages cover its window's rows, at their image positions, in the
+	// source's region of list_alpha. The threshold depends on the footprint and the radius alone: one value serves every source.
 	float threshold = 0.0f;
-	size_t avg_offset = 0;
-	for (size_t k = 0; k < call.srcs.size() && st == ASTCENC_SUCCESS && radius != 0; k++) {
-		const DevImage& s = call.srcs[k];
-		st = alpha_prepass(ctx, s, table ? 0 : call.row_lo, table ? s.blocks_y : call.row_hi + 1, ctx->list_alpha.as<float>() + avg_offset, stream, threshold);
-		avg_offset += (size_t)s.dim_x * s.dim_y;
+	for (size_t k = 0; k < call.table.size() && st == ASTCENC_SUCCESS && radius != 0; k++) {
+		const GatherImage& e = call.table[k];
+		const DevImage src = pass_image(ctx, e.data, call.data_type, e.dim_x, e.dim_y, e.dim_z, swizzle);
+		st = alpha_prepass(ctx, src, call.rows[k].first, call.rows[k].second, ctx->list_alpha.as<float>() + e.avg_offset, stream, threshold);
 	}
 	GatherArgs g;
-	g.src = src.data;
 	g.dst = ctx->list_image.ptr;
 	g.avg_src = radius != 0 ? ctx->list_alpha.as<const float>() : nullptr;
 	g.avg_dst = radius != 0 ? ctx->alpha.as<float>() : nullptr;
-	g.words = (unsigned int)(call.texel_bytes / 4);
-	g.dim_x = src.dim_x;
-	g.dim_y = src.dim_y;
-	g.dim_z = src.dim_z;
-	g.blocks_x = src.blocks_x;
-	g.blocks_y = src.blocks_y;
+	g.words = (unsigned int)(texel_bytes(call.data_type) / 4);
 	g.bx = bsd.dim_x;
 	g.by = bsd.dim_y;
 	g.bz = bsd.dim_z;
-	g.images = table ? ctx->list.as<const GatherImage>() : nullptr;
+	g.images = ctx->list.as<const GatherImage>();
 	g.image_count = (unsigned int)call.table.size();
 	g.lists = call.lists.empty() ? nullptr : reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes);
 	for (size_t first = 0; first < n && st == ASTCENC_SUCCESS; first += chunk) {
 		const unsigned int m = (unsigned int)(n - first < chunk ? n - first : chunk);
-		g.indices = table ? nullptr : ctx->list.as<const uint32_t>() + first;
 		g.base = first;
 		g.n = m;
 		const unsigned int warps = ASTC_GATHER_THREADS / 32;
 		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->plan.grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->plan.grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
 		ctx->launches++;
 		// (the staging volume is one layer deep)
-		DevImage staged = pass_image(ctx, ctx->list_image.ptr, src.data_type, m * bsd.dim_x, bsd.dim_y, volume ? bsd.dim_z : 1, swizzle);
+		DevImage staged = pass_image(ctx, ctx->list_image.ptr, call.data_type, m * bsd.dim_x, bsd.dim_y, volume ? bsd.dim_z : 1, swizzle);
 		staged.alpha_avg = radius != 0 ? ctx->alpha.as<float>() : nullptr;
 		staged.alpha_threshold = threshold;
 		st = launch_slab_locked(ctx, staged, 0, 1, ctx->list_out.ptr, stream, nullptr);
 		if (st == ASTCENC_SUCCESS) {
-			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g, call.payload);
+			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g);
 			ctx->launches++;
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 		}
@@ -1788,10 +1812,20 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	return st;
 }
 
-static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
+// A staging call on `cuda_stream` (null: the context's stream); a call of no staging blocks launches nothing.
+static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, void* cuda_stream) {
+	if (call.blocks == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t stream = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return scratch_turn(ctx, stream, [&] { return launch_blocks_locked(ctx, call, swizzle, stream); });
 }
 
+// A host list is a one-entry block-list table: its count word and indices go up with the table (BlockCall::words).
 astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const void* d_pixels, astcenc_type data_type, unsigned int dim_x, unsigned int dim_y,
                                                   unsigned int dim_z, const astcenc_swizzle* swizzle, const uint32_t* block_indices, unsigned int block_count,
                                                   uint8_t* d_payload, void* cuda_stream) {
@@ -1808,39 +1842,31 @@ astcenc_error astcenc_b200_compress_device_blocks(astcenc_context* ctx, const vo
 	if (status != ASTCENC_SUCCESS) {
 		return status;
 	}
-	// the list is checked whole before anything is enqueued, and copied: the caller may free it when the call returns
-	BlockCall call;
-	call.list.assign(block_indices, block_indices + block_count);
-	call.row_lo = 0xFFFFFFFFu;
-	for (uint32_t b : call.list) {
-		if (b >= geo.blocks) {
+	// Every index is checked below, so the list's bound is the block count clamped to 32 bits; the one index that skips,
+	// 0xFFFFFFFF in an image of more than 2^32 blocks, lies in an image of at least 256 GiB.
+	const GatherList list{nullptr, nullptr, block_count, geo.blocks < 0xFFFFFFFFu ? (unsigned int)geo.blocks : 0xFFFFFFFFu};
+	BlockEntry e{{d_pixels, d_payload, 0, 0, dim_x, dim_y, dim_z, (unsigned int)geo.blocks_x, (unsigned int)geo.blocks_y}, &list, block_count, 0xFFFFFFFFu, 0};
+	// the list is checked whole before anything is enqueued; the pre-pass window is the block rows it touches (2D images)
+	for (unsigned int i = 0; i < block_count; i++) {
+		if (block_indices[i] >= geo.blocks) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
-		unsigned int row = (unsigned int)(b / geo.blocks_x);      // (2D images: the block row, for the alpha-scale pre-pass window)
-		call.row_lo = row < call.row_lo ? row : call.row_lo;
-		call.row_hi = row > call.row_hi ? row : call.row_hi;
+		const unsigned int row = (unsigned int)(block_indices[i] / geo.blocks_x);
+		e.row0 = row < e.row0 ? row : e.row0;
+		e.row1 = row + 1 > e.row1 ? row + 1 : e.row1;
 	}
-	if (block_count == 0) {
-		return ASTCENC_SUCCESS;
-	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	call.srcs.push_back(pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, dim_z, *swizzle));
-	call.blocks = block_count;
-	call.texel_bytes = geo.texel_bytes;
-	call.payload = d_payload;
-	return launch_blocks(ctx, call, *swizzle, s);
+	BlockCall call;
+	plan_blocks({e}, data_type, call);      // (one entry of fewer than 2^32 blocks: nothing to refuse)
+	call.words.push_back(block_count);
+	call.words.insert(call.words.end(), block_indices, block_indices + block_count);
+	return launch_blocks(ctx, call, *swizzle, cuda_stream);
 }
 
 // The image table of a multi-image call, checked whole before anything is enqueued (the caller has checked the context, the
 // swizzle and the pointers): zero dimensions and the data type (ASTCENC_ERR_BAD_PARAM), a_scale_radius on a texture array
-// (ASTCENC_ERR_NOT_IMPLEMENTED), then the block counts (table_entry). Fills call.table (data and payload as given), call.srcs,
-// call.blocks and call.texel_bytes.
-static astcenc_error plan_image_table(const astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
-                                      const astcenc_swizzle& swizzle, BlockCall& call) {
+// (ASTCENC_ERR_NOT_IMPLEMENTED), then the block counts (table_entry). Fills one entry per image, of all its blocks.
+static astcenc_error check_image_table(const astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
+                                       std::vector<BlockEntry>& entries) {
 	astcenc_error status = ASTCENC_SUCCESS;
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		status = check_texel_count(images[i].dim_x, images[i].dim_y, images[i].dim_z);
@@ -1849,23 +1875,14 @@ static astcenc_error plan_image_table(const astcenc_context* ctx, const astcenc_
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		status = check_alpha_scale(ctx, images[i].dim_z);
 	}
-	call.table.resize(image_count);
-	size_t avg_offset = 0;
+	entries.resize(image_count);
+	size_t first = 0;
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_image& im = images[i];
-		status = table_entry(ctx, (int)data_type, im.dim_x, im.dim_y, im.dim_z, im.data, im.payload, call.blocks, call.table[i]);
-		call.table[i].avg_offset = avg_offset;
-		call.srcs.push_back(pass_image(ctx, im.data, (int)data_type, im.dim_x, im.dim_y, im.dim_z, swizzle));
-		avg_offset += (size_t)im.dim_x * im.dim_y;
+		status = table_entry(ctx, (int)data_type, im.dim_x, im.dim_y, im.dim_z, im.data, im.payload, first, entries[i].image);
+		entries[i].blocks = first - entries[i].image.first;
 	}
-	call.texel_bytes = texel_bytes(data_type);
 	return status;
-}
-
-// Payload bytes of image i of an image-table call.
-static size_t payload_bytes(const BlockCall& call, size_t i) {
-	const size_t end = i + 1 < call.table.size() ? call.table[i + 1].first : call.blocks;
-	return (end - call.table[i].first) * 16;
 }
 
 astcenc_error astcenc_b200_compress_device_images(astcenc_context* ctx, const astcenc_b200_device_image* images, unsigned int image_count, astcenc_type data_type,
@@ -1879,17 +1896,11 @@ astcenc_error astcenc_b200_compress_device_images(astcenc_context* ctx, const as
 			status = ASTCENC_ERR_BAD_PARAM;
 		}
 	}
+	std::vector<BlockEntry> entries;
+	if (status == ASTCENC_SUCCESS) status = check_image_table(ctx, images, image_count, data_type, entries);
 	BlockCall call;
-	if (status == ASTCENC_SUCCESS) status = plan_image_table(ctx, images, image_count, data_type, *swizzle, call);
-	if (status != ASTCENC_SUCCESS || image_count == 0) {
-		return status;
-	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_blocks(ctx, call, *swizzle, s);
+	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
 }
 
 // The host-pointer twin: every image goes up into one device buffer (ctx->image), the table is pointed at it and at one payload
@@ -1910,12 +1921,14 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 			descs.push_back({im->data, im->dim_x, im->dim_y, im->dim_z, data_out[i]});
 		}
 	}
+	std::vector<BlockEntry> entries;
 	BlockCall call;
 	if (status == ASTCENC_SUCCESS && image_count != 0) {
-		status = plan_image_table(ctx, descs.data(), image_count, images[0]->data_type, *swizzle, call);
+		status = check_image_table(ctx, descs.data(), image_count, images[0]->data_type, entries);
+		if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, images[0]->data_type, call);
 	}
 	for (unsigned int i = 0; i < image_count && status == ASTCENC_SUCCESS; i++) {
-		if (data_len[i] < payload_bytes(call, i)) {
+		if (data_len[i] < entries[i].blocks * 16) {
 			status = ASTCENC_ERR_OUT_OF_MEM;
 		}
 	}
@@ -1931,7 +1944,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 	size_t in_bytes = 0;
 	for (unsigned int i = 0; i < image_count; i++) {
 		in_offset[i] = in_bytes;
-		in_bytes += ((size_t)images[i]->dim_x * images[i]->dim_y * images[i]->dim_z * call.texel_bytes + 255) & ~(size_t)255;
+		in_bytes += ((size_t)images[i]->dim_x * images[i]->dim_y * images[i]->dim_z * texel_bytes(call.data_type) + 255) & ~(size_t)255;
 	}
 	astcenc_error st = ensure_buffer(ctx->image, in_bytes);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->out, call.blocks * 16);
@@ -1943,7 +1956,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 	for (unsigned int i = 0; i < image_count; i++) {
 		const astcenc_image& im = *images[i];
 		uint8_t* d_data = ctx->image.ptr + in_offset[i];
-		const size_t slice_bytes = (size_t)im.dim_x * im.dim_y * call.texel_bytes;
+		const size_t slice_bytes = (size_t)im.dim_x * im.dim_y * texel_bytes(call.data_type);
 		st = upload_slices(d_data, im.data, 0, im.dim_z, slice_bytes, ctx->stream);
 		if (st != ASTCENC_SUCCESS) {
 			return st;
@@ -1951,7 +1964,6 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 		ctx->last_h2d += slice_bytes * im.dim_z;
 		call.table[i].data = d_data;
 		call.table[i].payload = ctx->out.ptr + call.table[i].first * 16;
-		call.srcs[i].data = d_data;
 	}
 	CUDA_TRY(cudaEventRecord(ctx->ev0, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	st = launch_blocks(ctx, call, *swizzle, ctx->stream);
@@ -1960,7 +1972,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 	}
 	CUDA_TRY(cudaEventRecord(ctx->ev1, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 	for (unsigned int i = 0; i < image_count; i++) {
-		const size_t bytes = payload_bytes(call, i);
+		const size_t bytes = entries[i].blocks * 16;
 		CUDA_TRY(cudaMemcpyAsync(data_out[i], call.table[i].payload, bytes, cudaMemcpyDeviceToHost, ctx->stream), return ASTCENC_ERR_BAD_CONTEXT);
 		ctx->last_d2h += bytes;
 	}
@@ -2073,42 +2085,17 @@ astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, con
 		}
 		descs.push_back({l.data, l.dim_x, l.dim_y, l.dim_z, l.payload});
 	}
-	BlockCall all;
-	if (status == ASTCENC_SUCCESS) status = plan_image_table(ctx, descs.data(), list_count, data_type, *swizzle, all);
-	if (status != ASTCENC_SUCCESS) {
-		return status;
+	std::vector<BlockEntry> entries;
+	if (status == ASTCENC_SUCCESS) status = check_image_table(ctx, descs.data(), list_count, data_type, entries);
+	std::vector<GatherList> gather_lists(list_count);
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		gather_lists[i] = {lists[i].indices, lists[i].count, lists[i].capacity, (unsigned int)entries[i].blocks};
+		entries[i].list = &gather_lists[i];
+		entries[i].blocks = lists[i].capacity;
 	}
-	// the call: the entries with a non-zero capacity, their staging blocks numbered by the prefix sum of the capacities
 	BlockCall call;
-	call.texel_bytes = all.texel_bytes;
-	size_t avg_offset = 0;
-	for (unsigned int i = 0; i < list_count; i++) {
-		const astcenc_b200_device_block_list& l = lists[i];
-		if (l.capacity == 0) {
-			continue;
-		}
-		if (l.capacity > SIZE_MAX - call.blocks) {
-			return ASTCENC_ERR_BAD_PARAM;
-		}
-		GatherImage e = all.table[i];
-		const size_t end = i + 1 < list_count ? all.table[i + 1].first : all.blocks;
-		e.first = call.blocks;
-		e.avg_offset = avg_offset;
-		call.table.push_back(e);
-		call.srcs.push_back(all.srcs[i]);
-		call.lists.push_back({l.indices, l.count, l.capacity, (unsigned int)(end - all.table[i].first)});
-		call.blocks += l.capacity;
-		avg_offset += (size_t)l.dim_x * l.dim_y;
-	}
-	if (call.blocks == 0) {
-		return ASTCENC_SUCCESS;
-	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_blocks(ctx, call, *swizzle, s);
+	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
 }
 
 // Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table goes

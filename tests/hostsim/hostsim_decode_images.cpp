@@ -1,10 +1,10 @@
 // TEST TOOL (not a product path): decode calls over image tables (decode_table_blocks, astc_dev_gather.cuh) on the host
-// simulation of hostsim.cpp. Everything of hostsim_images.cpp, plus:
+// simulation of hostsim.cpp. Everything of hostsim_blocks.cpp, plus:
 //   hostsim_decompress_images  decode_table_blocks over every block of a decode call, in shares of `share` call blocks, as the
 //                              CTAs of astc_decompress_images_kernel take them (one simulated warp per CTA; one lane or 32)
 // The table is built as astcenc_b200_decompress_device_images builds it (image_table: first[] is the exclusive prefix sum of
 // the images' block counts); each entry's payload is read and its data written.
-#include "hostsim_images.cpp"
+#include "hostsim_blocks.cpp"
 
 // payloads[j] -> outs[j] (dim_z slices of dim_x * dim_y texels of data_type); swz uses astcenc_swz numbering.
 extern "C" int hostsim_decompress_images(int profile, unsigned int bx, unsigned int by, unsigned int bz, unsigned int flags, const uint8_t* const* payloads,

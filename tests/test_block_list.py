@@ -1,49 +1,39 @@
 """Block lists: astcenc_b200_compress_device_blocks recompresses the listed blocks of a device-resident image in place in its
 device-resident payload (gather into a staging row of blocks, one ordinary pass, scatter; astc_dev_gather.cuh).
 
-CPU: the gather's addressing (tests/hostsim/hostsim_blocks.cpp compiles astc_dev_gather.cuh for the host) against a numpy
-restatement of load_block's clamp-to-edge, and the device source's pass over the staging image (one lane and 32 lanes) against
-the oracle's whole-image blocks at the listed positions.
+CPU: the gather's addressing (tests/hostsim/hostsim_blocks.cpp compiles astc_dev_gather.cuh for the host; the list is a
+one-entry block-list table) against a numpy restatement of load_block's clamp-to-edge, and the device source's pass over the
+staging image (one lane and 32 lanes) against the oracle's whole-image blocks at the listed positions.
 GPU: the C ABI against astcenc_compress_image / compress_device / the reference build on the same images: listed blocks equal,
 every other payload byte untouched."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import astc_images as I
 from astc_ref import *  # noqa: F401,F403
+from hostsim_build import host_sim
 
 S = FLG_SELF_DECOMPRESS_ONLY
-HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "astc-encoder_b200", "csrc")
 _DT = {np.dtype(np.uint8): TYPE_U8, np.dtype(np.float16): TYPE_F16, np.dtype(np.float32): TYPE_F32}
 _SIMS = {}
 
 
 def blocks_sim(lanes32=False):
-    """tests/hostsim/hostsim_blocks.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
+    """tests/hostsim/hostsim_blocks.cpp: the gather and scatter of a staging call, the alpha-scale pre-pass and the pass over a
+    staging image."""
     if lanes32 in _SIMS:
         return _SIMS[lanes32]
-    so = os.path.join(HERE, "_build", "libhostsim_blocks%s.so" % ("32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    newest = max([os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)] + [os.path.getmtime(os.path.join(hs, f)) for f in os.listdir(hs)])
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, "hostsim_blocks.cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), os.path.join(CSRC, "astc_host_config.cpp"), "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
-    lib.hostsim_gather.argtypes = [C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_uint, C.c_void_p,
-                                   C.c_void_p, C.c_void_p]
+    lib = host_sim("hostsim_blocks", lanes32)
+    lib.hostsim_gather_table.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.hostsim_scatter_table.argtypes = [C.c_void_p, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint,
+                                          C.c_void_p, C.c_void_p]
     lib.hostsim_alpha_averages_2d.argtypes = [C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_void_p, C.c_uint, C.c_void_p]
     lib.hostsim_compress_staged.argtypes = [C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_float, C.c_uint, C.c_uint, C.c_void_p, C.c_int, C.c_uint, C.c_uint,
                                             C.c_uint, C.c_void_p, C.c_void_p]
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
     _SIMS[lanes32] = lib
     return lib
 
@@ -86,14 +76,24 @@ def staged_reference(vol, fp, idx):
     return out
 
 
-def sim_gather(lib, vol, fp, idx, avg=None):
+def sim_gather_list(lib, vol, fp, idx, count, avg=None, fill=0):
+    """The staging row of one block list of `vol` (a one-entry block-list table with capacity len(idx) and count `count`),
+    gathered over texels preset to `fill` and averages preset to -1."""
     vol = np.ascontiguousarray(vol)
+    idx = np.ascontiguousarray(idx, np.uint32)
     d, h, w = vol.shape[:3]
-    staged = np.zeros((fp[2], fp[1], len(idx) * fp[0], 4), vol.dtype)
+    staged = np.full((fp[2], fp[1], len(idx) * fp[0], 4), fill, vol.dtype)
     savg = np.full((fp[1], len(idx) * fp[0]), -1.0, np.float32) if avg is not None else None
-    lib.hostsim_gather(vol.ctypes.data, _DT[vol.dtype], w, h, d, fp[0], fp[1], fp[2], idx.ctypes.data, len(idx),
-                       avg.ctypes.data if avg is not None else None, staged.ctypes.data, savg.ctypes.data if savg is not None else None)
+    data, lists = (C.c_void_p * 1)(vol.ctypes.data), (C.c_void_p * 1)(idx.ctypes.data)
+    dims, counts, caps = np.array([w, h, d], np.uint32), np.array([count], np.uint32), np.array([len(idx)], np.uint32)
+    lib.hostsim_gather_table(data, dims.ctypes.data, 1, _DT[vol.dtype], fp[0], fp[1], fp[2], lists, counts.ctypes.data, caps.ctypes.data, 0, len(idx),
+                             avg.ctypes.data if avg is not None else None, staged.ctypes.data, savg.ctypes.data if savg is not None else None)
     return staged, savg
+
+
+def sim_gather(lib, vol, fp, idx, avg=None):
+    """The staging row of a host list: every listed block (count = capacity = len(idx))."""
+    return sim_gather_list(lib, vol, fp, idx, len(idx), avg)
 
 
 def ldr_image(h, w, d, seed):

@@ -2,46 +2,25 @@
 (astcenc_b200_compress_device_block_lists, astc_dev_gather.cuh).
 
 CPU: the selection compiled for the host (tests/hostsim/hostsim_select.cpp, one lane and 32 lanes) against the numpy rule of
-the header, and the key order; the count-limited gather (tests/hostsim/hostsim_block_lists.cpp) against the staging image of the
+the header, and the key order; the count-limited gather (tests/hostsim/hostsim_blocks.cpp) against the staging image of the
 valid slots, with zeros for the invalid ones.
 GPU: selection against numpy, alone and inside a shuffled table, twice, inside guard bytes, in a fixed number of launches;
 device block lists against compress_device_blocks with the host list they stand for; the closed loop compress -> decode ->
 measure -> select -> re-encode on one stream; launch counts; the error order of both entries."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import astc_images as I
 from astc_ref import *  # noqa: F401,F403
-from test_block_list import sim_gather, staged_reference
+from hostsim_build import host_sim
+from test_block_list import blocks_sim, sim_gather, sim_gather_list, staged_reference
 
 S = FLG_SELF_DECOMPRESS_ONLY
-HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "astc-encoder_b200", "csrc")
 _DT = {np.dtype(np.uint8): TYPE_U8, np.dtype(np.float16): TYPE_F16, np.dtype(np.float32): TYPE_F32}
 SELECT_LAUNCHES = 7
 _SIMS = {}
-
-
-def host_sim(name, lanes32=False):
-    """tests/hostsim/<name>.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
-    so = os.path.join(HERE, "_build", "lib%s%s.so" % (name, "32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    newest = max([os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)] + [os.path.getmtime(os.path.join(hs, f)) for f in os.listdir(hs)])
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, name + ".cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), os.path.join(CSRC, "astc_host_config.cpp"),
-               "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
-    return lib
 
 
 def select_sim(lanes32=False):
@@ -52,22 +31,6 @@ def select_sim(lanes32=False):
     lib.hostsim_select_key.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]
     lib.hostsim_select_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint]
     _SIMS[lanes32] = lib
-    return lib
-
-
-_LIST_SIMS = {}
-
-
-def lists_sim(lanes32=False):
-    """tests/hostsim/hostsim_block_lists.cpp: the gather of a device block list, and everything of hostsim_blocks.cpp."""
-    if lanes32 in _LIST_SIMS:
-        return _LIST_SIMS[lanes32]
-    lib = host_sim("hostsim_block_lists", lanes32)
-    lib.hostsim_gather.argtypes = [C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_uint, C.c_void_p,
-                                   C.c_void_p, C.c_void_p]
-    lib.hostsim_gather_list.argtypes = [C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_uint32,
-                                        C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p]
-    _LIST_SIMS[lanes32] = lib
     return lib
 
 
@@ -186,7 +149,7 @@ def test_count_limited_gather_stages_valid_slots_and_zeros(case, lanes32):
     """The first min(count, capacity) slots with an index inside the image stage what staged_reference gives; every other
     slot (past the count, whatever its poison, or out of range) stages zero texels and zero averages."""
     _, dtype, shape, fp, with_avg = case
-    lib = lists_sim(lanes32)
+    lib = blocks_sim(lanes32)
     rng = np.random.default_rng(3)
     vol = np.ascontiguousarray(rng.integers(1, 255, size=shape + (4,)).astype(dtype) if dtype == np.uint8 else
                                (rng.random(shape + (4,)) + 0.5).astype(dtype))
@@ -200,10 +163,7 @@ def test_count_limited_gather_stages_valid_slots_and_zeros(case, lanes32):
             idx[2] = idx[0]                         # (a duplicate)
         idx[min(count, capacity):] = rng.integers(0, 2 ** 32, size=capacity - min(count, capacity), dtype=np.uint64).astype(np.uint32)
         valid = np.array([s < min(count, capacity) and idx[s] < total for s in range(capacity)], bool)
-        staged = np.full((fp[2], fp[1], capacity * fp[0], 4), 77, dtype)
-        savg = np.full((fp[1], capacity * fp[0]), -1.0, np.float32) if with_avg else None
-        lib.hostsim_gather_list(vol.ctypes.data, _DT[vol.dtype], shape[2], shape[1], shape[0], fp[0], fp[1], fp[2], idx.ctypes.data, count, capacity,
-                                avg.ctypes.data if with_avg else None, staged.ctypes.data, savg.ctypes.data if with_avg else None)
+        staged, savg = sim_gather_list(lib, vol, fp, idx, count, avg, fill=77)
         ref_idx = np.where(valid, idx, 0).astype(np.uint32)
         want = staged_reference(vol, fp, ref_idx)
         want_avg = sim_gather(lib, vol, fp, ref_idx, avg)[1] if with_avg else None

@@ -7,7 +7,6 @@ each image alone.
 GPU: every output against Context.decompress_image of the same payload, with sentinel bytes around every output."""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -15,6 +14,7 @@ import pytest
 
 import astc_blockgen as G
 from astc_ref import *  # noqa: F401,F403
+from hostsim_build import host_sim
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
@@ -23,7 +23,6 @@ from test_multi_image import mip_chain  # noqa: E402
 
 import astc_images as I  # noqa: E402
 
-CSRC = os.path.join(os.path.dirname(HERE), "astc-encoder_b200", "csrc")
 NP = {TYPE_U8: np.uint8, TYPE_F16: np.float16, TYPE_F32: np.float32}
 PROFILES = (PRF_LDR_SRGB, PRF_LDR, PRF_HDR_RGB_LDR_A, PRF_HDR)
 GAP = 37
@@ -37,21 +36,9 @@ def decode_sim(lanes32=False):
     """tests/hostsim/hostsim_decode_images.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
     if lanes32 in _SIMS:
         return _SIMS[lanes32]
-    so = os.path.join(HERE, "_build", "libhostsim_decode_images%s.so" % ("32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    newest = max([os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)] + [os.path.getmtime(os.path.join(hs, f)) for f in os.listdir(hs)])
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, "hostsim_decode_images.cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), os.path.join(CSRC, "astc_host_config.cpp"),
-               "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
+    lib = host_sim("hostsim_decode_images", lanes32)
     lib.hostsim_decompress_images.argtypes = [C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint, C.c_int,
                                               C.POINTER(C.c_int), C.c_size_t]
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
     _SIMS[lanes32] = lib
     return lib
 

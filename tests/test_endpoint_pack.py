@@ -24,11 +24,11 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-CSRC = os.path.join(ROOT, "astc-encoder_b200", "csrc")
 sys.path.insert(0, os.path.join(HERE, "golden"))
 import make_golden_endpoints as G  # noqa: E402
 import astc_blockgen as B  # noqa: E402
 from astc_ref import ORACLE_SO, have_ref_pack, ref_pack_color_endpoints  # noqa: E402
+from hostsim_build import host_sim  # noqa: E402
 
 VARIANTS = {"serial": 0, "coop": 1, "coop_inl": 2, "hdr": 3}
 VARIANT_FORMATS = {"serial": G.LDR_FORMATS, "coop": (8, 12), "coop_inl": (8, 12), "hdr": G.HDR_FORMATS}
@@ -100,21 +100,9 @@ def endpoints_sim(lanes32=False):
     """tests/hostsim/hostsim_endpoints.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
     if lanes32 in _SIMS:
         return _SIMS[lanes32]
-    so = os.path.join(HERE, "_build", "libhostsim_endpoints%s.so" % ("32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(hs, f) for f in os.listdir(hs)] + \
-        [os.path.join(HERE, "devunit", "pack_endpoints_args.h")]
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(f) for f in srcs):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, "hostsim_endpoints.cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
+    lib = host_sim("hostsim_endpoints", lanes32)
     lib.hostsim_pack_endpoints.argtypes = [C.c_int, C.c_int] + _ARGS
     lib.hostsim_pack_endpoints.restype = C.c_int
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
     _SIMS[lanes32] = lib
     return lib
 

@@ -9,17 +9,16 @@ shuffled 40-entry table; the maps against numpy, with guard bytes around every o
 compress_device_blocks; the error order and the launch count."""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
 from astc_ref import *  # noqa: F401,F403
+from hostsim_build import host_sim
 import astc_images as I
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "astc-encoder_b200", "csrc")
 GOLD = os.path.join(HERE, "golden", "golden_metrics.npz")
 NP = {TYPE_U8: np.uint8, TYPE_F16: np.float16, TYPE_F32: np.float32}
 DT = {np.dtype(np.uint8): TYPE_U8, np.dtype(np.float16): TYPE_F16, np.dtype(np.float32): TYPE_F32}
@@ -39,23 +38,11 @@ def metrics_sim(lanes32=False):
     """tests/hostsim/hostsim_metrics.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
     if lanes32 in _SIMS:
         return _SIMS[lanes32]
-    so = os.path.join(HERE, "_build", "libhostsim_metrics%s.so" % ("32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    newest = max([os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)] + [os.path.getmtime(os.path.join(hs, f)) for f in os.listdir(hs)])
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, "hostsim_metrics.cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), os.path.join(CSRC, "astc_host_config.cpp"),
-               "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
+    lib = host_sim("hostsim_metrics", lanes32)
     lib.hostsim_plan_metrics.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p]
     lib.hostsim_block_error.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_int,
                                         C.c_void_p]
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
     _SIMS[lanes32] = lib
     return lib
 

@@ -2,51 +2,22 @@
 chains, texture sets - in shared pipeline passes (gather into staging rows, one ordinary pass per row, scatter to each image's
 payload; astc_dev_gather.cuh).
 
-CPU: the image-table gather and scatter (tests/hostsim/hostsim_images.cpp compiles astc_dev_gather.cuh for the host) against a
+CPU: the image-table gather and scatter (tests/hostsim/hostsim_blocks.cpp compiles astc_dev_gather.cuh for the host) against a
 numpy restatement of load_block's clamp-to-edge and of the alpha averages, and the device source's pass over a multi-image
 staging row (one lane and 32 lanes) against the oracle's blocks of each image.
 GPU: every payload against Context.compress_image of that image alone, with sentinel gaps between the payloads."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import astc_images as I
 from astc_ref import *  # noqa: F401,F403
+from test_block_list import blocks_sim
 
 S = FLG_SELF_DECOMPRESS_ONLY
-HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "astc-encoder_b200", "csrc")
 _DT = {np.dtype(np.uint8): TYPE_U8, np.dtype(np.float16): TYPE_F16, np.dtype(np.float32): TYPE_F32}
-_SIMS = {}
-
-
-def images_sim(lanes32=False):
-    """tests/hostsim/hostsim_images.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
-    if lanes32 in _SIMS:
-        return _SIMS[lanes32]
-    so = os.path.join(HERE, "_build", "libhostsim_images%s.so" % ("32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    newest = max([os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)] + [os.path.getmtime(os.path.join(hs, f)) for f in os.listdir(hs)])
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, "hostsim_images.cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), os.path.join(CSRC, "astc_host_config.cpp"), "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
-    lib.hostsim_gather_images.argtypes = [C.c_void_p, C.c_void_p, C.c_uint, C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_size_t, C.c_uint, C.c_void_p,
-                                          C.c_void_p, C.c_void_p]
-    lib.hostsim_scatter_images.argtypes = [C.c_void_p, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.c_size_t, C.c_uint, C.c_void_p, C.c_void_p]
-    lib.hostsim_alpha_averages_2d.argtypes = [C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_void_p, C.c_uint, C.c_void_p]
-    lib.hostsim_compress_staged.argtypes = [C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_float, C.c_uint, C.c_uint, C.c_void_p, C.c_int, C.c_uint, C.c_uint,
-                                            C.c_uint, C.c_void_p, C.c_void_p]
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
-    _SIMS[lanes32] = lib
-    return lib
 
 
 def grid(shape, fp):
@@ -95,15 +66,16 @@ def sim_gather(lib, vols, fp, base, n, avgs=None):
     if avgs is not None:
         avg = np.ascontiguousarray(np.concatenate([a.reshape(-1) for a in avgs]).astype(np.float32))
         savg = np.full((fp[1], n * fp[0]), -1.0, np.float32)
-    lib.hostsim_gather_images(ptrs, dims.ctypes.data, len(vols), _DT[vols[0].dtype], fp[0], fp[1], fp[2], base, n,
-                              avg.ctypes.data if avg is not None else None, staged.ctypes.data, savg.ctypes.data if savg is not None else None)
+    lib.hostsim_gather_table(ptrs, dims.ctypes.data, len(vols), _DT[vols[0].dtype], fp[0], fp[1], fp[2], None, None, None, base, n,
+                             avg.ctypes.data if avg is not None else None, staged.ctypes.data, savg.ctypes.data if savg is not None else None)
     return staged, savg
 
 
 def sim_scatter(lib, shapes, fp, base, staged_blocks, payloads):
     dims = np.array([[s[2], s[1], s[0]] for s in shapes], np.uint32).reshape(-1)
     ptrs = (C.c_void_p * len(payloads))(*[p.ctypes.data for p in payloads])
-    lib.hostsim_scatter_images(dims.ctypes.data, len(shapes), fp[0], fp[1], fp[2], base, len(staged_blocks), np.ascontiguousarray(staged_blocks).ctypes.data, ptrs)
+    lib.hostsim_scatter_table(dims.ctypes.data, len(shapes), fp[0], fp[1], fp[2], None, None, None, base, len(staged_blocks),
+                              np.ascontiguousarray(staged_blocks).ctypes.data, ptrs)
 
 
 def random_image(rng, dtype, shape):
@@ -133,7 +105,7 @@ def test_gather_and_scatter_follow_the_image_table(case):
     """Every block of every image lands in call order in the staging row, as load_block reads it, whatever the chunking; the
     scatter puts each staged block at its image's payload position."""
     _, dtype, shapes, fp = case
-    lib = images_sim()
+    lib = blocks_sim()
     rng = np.random.default_rng(17)
     vols = [random_image(rng, dtype, s) for s in shapes]
     flat = all(s[0] == 1 for s in shapes) and fp[2] == 1
@@ -202,7 +174,7 @@ PARITY = [
 def test_pass_over_multi_image_row_equals_each_image(case, oracle):
     """The device source's pass over one staging row of several images, scattered, gives the oracle's payload of each image."""
     _, prof, dtype, fp, q, radius, lanes32 = case
-    lib = images_sim(lanes32)
+    lib = blocks_sim(lanes32)
     hdr = prof in (PRF_HDR, PRF_HDR_RGB_LDR_A)
     if radius:
         vols = [transparent_image(1, 1, 2, (0, 1, 0, 1))[None], transparent_image(7, 5, 3, (0, 0, 0, 0))[None],

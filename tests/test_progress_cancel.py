@@ -5,8 +5,6 @@ device words - the cancel flag, looked at wherever a warp takes new work, and th
 has ended.
 GPU: the progress callback and astcenc_compress_cancel through the C ABI, against passes of the same context without them."""
 import ctypes as C
-import os
-import subprocess
 import threading
 import time
 
@@ -15,15 +13,13 @@ import pytest
 
 import astc_images as I
 from astc_ref import *  # noqa: F401,F403
+from hostsim_build import host_sim
 from golden.make_golden import CASES, make_image
 
 S = FLG_SELF_DECOMPRESS_ONLY
 _DT = {np.dtype(np.uint8): TYPE_U8, np.dtype(np.float16): TYPE_F16, np.dtype(np.float32): TYPE_F32}
 GOLDEN = {c[0]: c for c in CASES}
 
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-CSRC = os.path.join(os.path.dirname(HERE), "astc-encoder_b200", "csrc")
 _SIMS = {}
 
 
@@ -31,23 +27,12 @@ def progress_sim(lanes32):
     """tests/hostsim/hostsim_progress.cpp compiled for the host (one simulated lane, or 32 lanes on 32 threads)."""
     if lanes32 in _SIMS:
         return _SIMS[lanes32]
-    so = os.path.join(HERE, "_build", "libhostsim_progress%s.so" % ("32" if lanes32 else ""))
-    hs = os.path.join(HERE, "hostsim")
-    newest = max([os.path.getmtime(os.path.join(CSRC, f)) for f in os.listdir(CSRC)] + [os.path.getmtime(os.path.join(hs, f)) for f in os.listdir(hs)])
-    if not os.path.exists(so) or os.path.getmtime(so) < newest:
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        cmd = ["g++", "-std=c++14", "-O2", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared"] + \
-              (["-pthread", "-DASTC_HOSTSIM_LANES32=1"] if lanes32 else []) + \
-              ["-x", "c++", os.path.join(hs, "hostsim_progress.cpp"), os.path.join(CSRC, "astc_host_tables.cpp"), os.path.join(CSRC, "astc_host_config.cpp"), "-o", so]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-3000:]
-    lib = C.CDLL(so)
+    lib = host_sim("hostsim_progress", lanes32)
     lib.hostsim_set_cancel.argtypes = [C.c_int]
     lib.hostsim_done.restype = C.c_uint
     lib.hostsim_set_a_scale_radius.argtypes = [C.c_uint]
     lib.hostsim_progress_volume.argtypes = [C.c_int, C.c_uint, C.c_uint, C.c_uint, C.c_float, C.c_uint, C.c_void_p, C.c_int, C.c_uint, C.c_uint, C.c_uint,
                                             C.POINTER(C.c_int), C.c_void_p]
-    assert lib.hostsim_lanes() == (32 if lanes32 else 1)
     _SIMS[lanes32] = lib
     return lib
 

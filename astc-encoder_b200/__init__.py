@@ -90,6 +90,19 @@ class DeviceBlockList(C.Structure):
                 ("count", C.c_void_p), ("capacity", C.c_uint)]
 
 
+class DeviceDecodeBlockList(C.Structure):
+    """struct astcenc_b200_device_decode_block_list (include/astcenc.h)."""
+    _fields_ = [("payload", C.c_void_p), ("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("indices", C.c_void_p),
+                ("count", C.c_void_p), ("capacity", C.c_uint)]
+
+
+class DeviceBlockErrorList(C.Structure):
+    """struct astcenc_b200_device_block_error_list (include/astcenc.h)."""
+    _fields_ = [("original", C.c_void_p), ("decoded", C.c_void_p), ("original_type", C.c_int), ("decoded_type", C.c_int), ("dim_x", C.c_uint),
+                ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("block_error", C.c_void_p), ("indices", C.c_void_p), ("count", C.c_void_p),
+                ("capacity", C.c_uint)]
+
+
 class ErrorMetrics(C.Structure):
     """struct astcenc_b200_error_metrics (include/astcenc.h)."""
     _fields_ = [(n, C.c_double) for n in ("psnr", "alpha_psnr", "rgb_psnr", "rgb_peak", "peak_psnr", "mpsnr", "log_rmse",
@@ -165,6 +178,11 @@ def lib():
         l.astcenc_b200_select_blocks.restype = C.c_int
         l.astcenc_b200_compress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
         l.astcenc_b200_compress_device_block_lists.restype = C.c_int
+        l.astcenc_b200_decompress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceDecodeBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle),
+                                                                 C.c_void_p]
+        l.astcenc_b200_decompress_device_block_lists.restype = C.c_int
+        l.astcenc_b200_compute_block_errors_device_block_lists.argtypes = [C.c_void_p, C.c_int, C.POINTER(DeviceBlockErrorList), C.c_uint, C.c_void_p]
+        l.astcenc_b200_compute_block_errors_device_block_lists.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -496,6 +514,33 @@ class Context:
         err = lib().astcenc_b200_compress_device_block_lists(self.handle, table if n else None, n, data_type, C.byref(sw), C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compress_device_block_lists")
+
+    def decompress_device_block_lists(self, lists, data_type, swizzle=(0, 1, 2, 3), stream=0):
+        """Decode device-resident block lists into device images (astcenc_b200_decompress_device_block_lists). lists: a sequence of
+        (d_payload_ptr, d_image_ptr, dim_x, dim_y, dim_z, d_indices_ptr, d_count_ptr, capacity); for the first min(*count, capacity)
+        indices in range, the block's texels receive what decompress_device_images writes there for the whole payload, and no other
+        byte changes. Enqueued on `stream`, no sync; works on decompress-only contexts."""
+        n = len(lists)
+        table = (DeviceDecodeBlockList * n)(*[DeviceDecodeBlockList(C.c_void_p(p), C.c_void_p(d), x, y, z, C.c_void_p(i or None), C.c_void_p(k or None), c)
+                                              for p, d, x, y, z, i, k, c in lists])
+        sw = Swizzle(*swizzle) if swizzle is not None else None
+        err = lib().astcenc_b200_decompress_device_block_lists(self.handle, table if n else None, n, data_type, C.byref(sw) if sw is not None else None,
+                                                               C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_decompress_device_block_lists")
+
+    def compute_block_errors_device_block_lists(self, lists, input_components=4, stream=0):
+        """Refresh per-block error maps at device-resident block lists (astcenc_b200_compute_block_errors_device_block_lists).
+        lists: a sequence of (d_original_ptr, d_decoded_ptr, original_type, decoded_type, dim_x, dim_y, dim_z, d_block_error_ptr,
+        d_indices_ptr, d_count_ptr, capacity); each listed map value receives what compute_error_metrics_device_images writes for
+        that block, and no other value changes. Enqueued on `stream`, no sync; works on decompress-only contexts."""
+        n = len(lists)
+        table = (DeviceBlockErrorList * n)(*[DeviceBlockErrorList(C.c_void_p(o), C.c_void_p(d), ot, dt, x, y, z, C.c_void_p(b or None), C.c_void_p(i or None),
+                                                                  C.c_void_p(k or None), c)
+                                             for o, d, ot, dt, x, y, z, b, i, k, c in lists])
+        err = lib().astcenc_b200_compute_block_errors_device_block_lists(self.handle, input_components, table if n else None, n, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compute_block_errors_device_block_lists")
 
     def last_timing(self):
         ms = C.c_float(); a = C.c_size_t(); b = C.c_size_t()

@@ -18,7 +18,7 @@
 // table whose list has capacity n and *count n.
 //
 // A decode call (astcenc_b200_decompress_device_images) walks the same kind of table without lists: each entry's payload is
-// read and its data written.
+// read and its data written. A list decode (astcenc_b200_decompress_device_block_lists) walks it with lists, slot by slot.
 #pragma once
 
 // One image of an image table.
@@ -190,5 +190,50 @@ ASTC_FN void decode_table_blocks(const GatherImage* images, unsigned int image_c
 			decompress_block(lane, slice, im.payload + (b - im.first) * 16, k - by * im.blocks_x, by);
 		}
 		c = end;
+	}
+}
+
+// ---- block lists of a decode call (astc_decompress_block_lists_kernel) ----
+// Entry j owns the call's slots [first[j], first[j + 1]), the capacity[j] slots of its list; slot s of the entry decodes block
+// indices[s] of its image when list_slot finds it valid, and does nothing otherwise. Consecutive slots may jump between
+// entries and planes, so a warp restages IMG only when a slot's (entry, plane) differs from the one staged last. The CTA is
+// this one warp: __syncwarp orders the restaging against the decodes around it. Sorted lists (what select_blocks writes) stay
+// in one plane for long runs.
+//
+// Slots [c0, c1) by one warp (lane `lane`; the host simulation runs it with one lane or 32). On entry IMG holds the call's data
+// type and swizzle; its pointer and dimensions are restaged here.
+ASTC_FN void decode_list_blocks(const GatherImage* images, const GatherList* lists, unsigned int image_count, size_t c0, size_t c1, int lane,
+                                uint32_t slice) {
+	DevImage& img = reinterpret_cast<SmemHdr*>(astc_smem)->img;
+	const unsigned int bz = BSD.dim_z;
+	const size_t texel_bytes = img.data_type == 0 ? 4 : img.data_type == 1 ? 8 : 16;
+	unsigned int staged_j = 0xFFFFFFFFu, staged_plane = 0;      // (nothing staged yet)
+	for (size_t c = c0; c < c1; c++) {
+		const unsigned int j = find_image(images, image_count, c);
+		const GatherImage& im = images[j];
+		const uint32_t index = list_slot(lists[j], c - im.first);
+		if (index == GATHER_INVALID) {
+			continue;      // (the whole warp: every lane reads the same slot)
+		}
+		// a plane: the whole volume of a 3D block size, one slice of a 2D one (an image has fewer than 2^32 blocks)
+		const unsigned int plane_blocks = im.blocks_x * im.blocks_y * (bz > 1 ? (im.dim_z + bz - 1) / bz : 1);
+		const unsigned int plane = index / plane_blocks;
+		if (j != staged_j || plane != staged_plane) {
+			wsync();      // the warp is done with the previous plane
+			if (lane == 0) {
+				img.data = static_cast<const uint8_t*>(im.data) + plane * (size_t)im.dim_x * im.dim_y * texel_bytes;
+				img.dim_x = im.dim_x;
+				img.dim_y = im.dim_y;
+				img.dim_z = bz > 1 ? im.dim_z : 1;
+				img.blocks_x = im.blocks_x;
+				img.blocks_y = im.blocks_y;
+			}
+			wsync();
+			staged_j = j;
+			staged_plane = plane;
+		}
+		const unsigned int k = index - plane * plane_blocks;
+		const unsigned int by = k / im.blocks_x;
+		decompress_block(lane, slice, im.payload + (size_t)index * 16, k - by * im.blocks_x, by);
 	}
 }

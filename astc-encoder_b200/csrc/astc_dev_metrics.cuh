@@ -15,7 +15,9 @@
 // v of `ctas`. Partials go out [slice][virtual CTA] per entry, and the finish kernel walks them in that order.
 //
 // The per-block error map (block_error_sum) is one warp per block of the context's footprint, in astcenc_compress_image's
-// block order; it compiles for the host simulation too (tests/hostsim/hostsim_metrics.cpp).
+// block order; it compiles for the host simulation too (tests/hostsim/hostsim_metrics.cpp). A list refresh
+// (astcenc_b200_compute_block_errors_device_block_lists) runs the same function at the slots of device block lists, one warp per
+// slot (tests/hostsim/hostsim_map_lists.cpp).
 #pragma once
 #include <vector>
 #include "../../include/astcenc.h"
@@ -125,6 +127,55 @@ static inline bool plan_metrics(std::vector<MetricEntry>& table, unsigned int bx
 	return true;
 }
 
+// ---- map refreshes over block lists (astcenc_b200_compute_block_errors_device_block_lists) ----
+// Entry j of the call owns the slots [maps[j].first, maps[j].first + lists[j].capacity): slot s of the entry refreshes map value
+// indices[s] of its pair when list_slot finds it valid, and does nothing otherwise. maps[j].entry is j.
+struct MetricListArgs {
+	const MetricEntry* entries;
+	const MetricMap* maps;            // one per entry: its first slot
+	const GatherList* lists;          // one per entry
+	unsigned int count;
+	size_t slots;                     // the sum of the capacities: warps of the launch
+	unsigned int bx, by, bz;          // the map footprint
+	int components;
+};
+
+struct MetricListPlan {
+	std::vector<MetricMap> maps;
+	size_t slots = 0;
+	unsigned int grid = 0;            // CTAs of ASTC_METRIC_MAP_WARPS warps
+};
+
+// Fills in the planned fields of `table` (images, types, pitches, strides, dims and block_error set; every entry has a map) and the
+// slots of its lists, whose capacities are capacities[j], for the footprint bx x by x bz. The map values depend on the same fields
+// plan_metrics fills, so a list refresh and a whole map agree bit for bit. false: the call does not fit a launch (an entry has
+// 2^32 blocks or more, the sum of the capacities overflows, or the grid exceeds 2^31 - 1).
+static inline bool plan_block_error_lists(std::vector<MetricEntry>& table, const unsigned int* capacities, unsigned int bx, unsigned int by, unsigned int bz,
+                                          MetricListPlan& p) {
+	const size_t grid_max = 0x7FFFFFFF;
+	p = MetricListPlan();
+	for (size_t i = 0; i < table.size(); i++) {
+		MetricEntry& e = table[i];
+		e.ctas = 0;
+		e.first = 0;
+		e.inv_pixels = 0.0;
+		e.blocks_x = (e.dim_x + bx - 1) / bx;
+		e.blocks_y = (e.dim_y + by - 1) / by;
+		const size_t blocks = (size_t)e.blocks_x * e.blocks_y * ((e.dim_z + bz - 1) / bz);
+		if (blocks > 0xFFFFFFFFu || capacities[i] > SIZE_MAX - p.slots) {
+			return false;
+		}
+		p.maps.push_back({p.slots, (unsigned int)i});
+		p.slots += capacities[i];
+	}
+	const size_t grid = (p.slots + ASTC_METRIC_MAP_WARPS - 1) / ASTC_METRIC_MAP_WARPS;
+	if (grid > grid_max) {
+		return false;
+	}
+	p.grid = (unsigned int)grid;
+	return true;
+}
+
 // ---- per-texel values ----
 
 // Texel t (index in texels) of an image of `type`: U8 scaled to 0..1, F16 / F32 clamped to [0, 65504] (:187, :200). One vector
@@ -190,6 +241,21 @@ ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned i
 	}
 #endif
 	return acc;
+}
+
+// Slot w < a.slots of a list refresh, by `lanes` lanes of one warp: block_error_sum of the listed block into its map value. An
+// entry with capacity 0 owns no slot, and a slot past the count or out of range writes nothing.
+ASTC_FN void block_error_list_slot(const MetricListArgs& a, size_t w, int lane, int lanes) {
+	const MetricMap& m = a.maps[find_image(a.maps, a.count, w)];
+	const uint32_t index = list_slot(a.lists[m.entry], w - m.first);
+	if (index == GATHER_INVALID) {
+		return;      // (the whole warp)
+	}
+	const MetricEntry& e = a.entries[m.entry];
+	const double s = block_error_sum(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), lane, lanes);
+	if (lane == 0) {
+		e.block_error[index] = (float)s;
+	}
 }
 
 // ---- the closing arithmetic of compute_error_metrics (:285-411) ----
@@ -404,6 +470,15 @@ astc_block_error_kernel(const __grid_constant__ MetricArgs a) {
 	const double s = block_error_sum(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), threadIdx.x & 31, ASTC_WARP);
 	if ((threadIdx.x & 31) == 0) {
 		e.block_error[index] = (float)s;
+	}
+}
+
+// A list refresh of maps: warp w of the launch is slot w of the call.
+__global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
+astc_block_error_lists_kernel(const __grid_constant__ MetricListArgs a) {
+	const size_t w = (size_t)blockIdx.x * ASTC_METRIC_MAP_WARPS + (threadIdx.x >> 5);
+	if (w < a.slots) {
+		block_error_list_slot(a, w, threadIdx.x & 31, ASTC_WARP);
 	}
 }
 #endif

@@ -253,6 +253,19 @@ astc_decompress_images_kernel(const __grid_constant__ DevBsd bsd, const __grid_c
 	                    ASTC_SMEM_HDR + (threadIdx.x >> 5) * D_SLICE);
 }
 
+// ---- decompression of block lists (astcenc_b200_decompress_device_block_lists): one warp per CTA, each CTA over a contiguous
+// share of the call's slots (decode_list_blocks restages IMG behind __syncwarp); img carries the call's data type and swizzle ----
+#define ASTC_DECODE_LIST_CTAS_PER_SM 32
+__global__ void __launch_bounds__(32)
+astc_decompress_block_lists_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
+                                   const GatherImage* __restrict__ images, const GatherList* __restrict__ lists, unsigned int image_count, size_t total) {
+	stage_launch_constants(bsd, cfg, img);
+	const size_t per = (total + gridDim.x - 1) / gridDim.x;
+	const size_t c0 = blockIdx.x * per;
+	const size_t c1 = c0 + per < total ? c0 + per : total;
+	decode_list_blocks(images, lists, image_count, c0, c1, (int)threadIdx.x, ASTC_SMEM_HDR);
+}
+
 __global__ void __launch_bounds__(32, 1)
 astc_block_info_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
                        unsigned long long lo, unsigned long long hi, DevBlockInfo* out) {
@@ -2096,6 +2109,157 @@ astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, con
 	BlockCall call;
 	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
 	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
+}
+
+// Decode calls over device block lists: the image table of astcenc_b200_decompress_device_images whose entry j owns capacity[j]
+// slots, the slots of its device list (GatherList). Checked whole before anything is enqueued, in the order of the image-table
+// decode plus the list checks of astcenc_b200_compress_device_block_lists; entries with a capacity of 0 are checked and then
+// left out. The table and its lists go up in one copy and one launch decodes every slot, in one scratch turn.
+astcenc_error astcenc_b200_decompress_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_decode_block_list* lists, unsigned int list_count,
+                                                         astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
+	astcenc_error status = swizzle ? check_swizzle(*swizzle, ASTCENC_SWZ_Z) : ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS && list_count != 0 && !lists) status = ASTCENC_ERR_BAD_PARAM;
+	auto aligned4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; };
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		const astcenc_b200_device_decode_block_list& l = lists[i];
+		if (!l.payload || !l.data || (l.capacity != 0 && (!l.indices || !l.count)) || !aligned4(l.indices) || !aligned4(l.count)) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		} else {
+			status = check_texel_count(l.dim_x, l.dim_y, l.dim_z);
+		}
+	}
+	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
+	std::vector<GatherImage> table;
+	std::vector<GatherList> gather_lists;
+	size_t slots = 0;
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		const astcenc_b200_device_decode_block_list& l = lists[i];
+		GatherImage e;
+		size_t blocks = 0;
+		// (the payload is read, never written)
+		status = table_entry(ctx, (int)data_type, l.dim_x, l.dim_y, l.dim_z, l.data, const_cast<uint8_t*>(l.payload), blocks, e);
+		if (status == ASTCENC_SUCCESS && l.capacity > SIZE_MAX - slots) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		}
+		if (status == ASTCENC_SUCCESS && l.capacity != 0) {
+			e.first = slots;
+			table.push_back(e);
+			gather_lists.push_back({l.indices, l.count, l.capacity, (unsigned int)blocks});
+			slots += l.capacity;
+		}
+	}
+	if (status != ASTCENC_SUCCESS || slots == 0) {
+		return status;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return scratch_turn(ctx, s, [&]() -> astcenc_error {
+		const size_t table_bytes = table.size() * sizeof(GatherImage);
+		const size_t lists_bytes = gather_lists.size() * sizeof(GatherList);
+		astcenc_error r = ensure_buffer(ctx->list, table_bytes + lists_bytes);
+		if (r != ASTCENC_SUCCESS) {
+			return r;
+		}
+		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(gather_lists.data()), reinterpret_cast<const uint8_t*>(gather_lists.data()) + lists_bytes);
+		// (from pageable memory: staged by the driver before the call returns)
+		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+		const size_t cap = (size_t)ctx->sm_count * ASTC_DECODE_LIST_CTAS_PER_SM;
+		const unsigned int grid = (unsigned int)(slots < cap ? slots : cap);
+		astc_decompress_block_lists_kernel<<<grid, 32, ASTC_SMEM_HDR + D_SLICE, s>>>(
+		    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, (int)data_type, 0, 0, 0, *swizzle), ctx->list.as<const GatherImage>(),
+		    reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes), (unsigned int)table.size(), slots);
+		ctx->launches++;
+		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+		return ASTCENC_SUCCESS;
+	});
+}
+
+// Map refreshes over device block lists: every entry is checked before anything is enqueued, in the order of the metrics call;
+// the table, its first slots and its lists go up in one copy and one launch refreshes every slot, in one scratch turn.
+astcenc_error astcenc_b200_compute_block_errors_device_block_lists(astcenc_context* ctx, int input_components,
+                                                                   const astcenc_b200_device_block_error_list* lists, unsigned int list_count,
+                                                                   void* cuda_stream) {
+	if (!ctx || input_components < 1 || input_components > 4) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (list_count != 0 && !lists) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	auto aligned = [](const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
+	std::vector<MetricEntry> table(list_count);
+	std::vector<GatherList> gather_lists(list_count);
+	std::vector<unsigned int> capacities(list_count);
+	for (unsigned int i = 0; i < list_count; i++) {
+		const astcenc_b200_device_block_error_list& l = lists[i];
+		if (!l.original || !l.decoded || (l.capacity != 0 && (!l.block_error || !l.indices || !l.count)) ||
+		    check_texel_count(l.dim_x, l.dim_y, l.dim_z) != ASTCENC_SUCCESS || check_data_type(l.original_type) != ASTCENC_SUCCESS ||
+		    check_data_type(l.decoded_type) != ASTCENC_SUCCESS || !aligned(l.original, texel_bytes(l.original_type)) ||
+		    !aligned(l.decoded, texel_bytes(l.decoded_type)) || !aligned(l.block_error, 4) || !aligned(l.indices, 4) || !aligned(l.count, 4)) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		MetricEntry& e = table[i];
+		memset(&e, 0, sizeof(e));
+		e.img1 = l.original;
+		e.img2 = l.decoded;
+		e.type1 = (int)l.original_type;
+		e.type2 = (int)l.decoded_type;
+		e.pitch1 = e.pitch2 = l.dim_x;
+		e.stride1 = e.stride2 = (size_t)l.dim_x * l.dim_y;
+		e.dim_x = l.dim_x;
+		e.dim_y = l.dim_y;
+		e.dim_z = l.dim_z;
+		e.block_error = l.block_error;
+		capacities[i] = l.capacity;
+	}
+	const unsigned int bz = ctx->config.block_z > 1 ? ctx->config.block_z : 1;
+	MetricListPlan plan;
+	if (!plan_block_error_lists(table, capacities.data(), ctx->config.block_x, ctx->config.block_y, bz, plan)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (plan.slots == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	for (unsigned int i = 0; i < list_count; i++) {
+		// (the planner has refused images of 2^32 blocks or more)
+		gather_lists[i] = {lists[i].indices, lists[i].count, lists[i].capacity, table[i].blocks_x * table[i].blocks_y * ((table[i].dim_z + bz - 1) / bz)};
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return scratch_turn(ctx, s, [&]() -> astcenc_error {
+		const size_t table_bytes = table.size() * sizeof(MetricEntry);
+		const size_t maps_bytes = plan.maps.size() * sizeof(MetricMap);
+		const size_t lists_bytes = gather_lists.size() * sizeof(GatherList);
+		astcenc_error r = ensure_buffer(ctx->list, table_bytes + maps_bytes + lists_bytes);
+		if (r != ASTCENC_SUCCESS) {
+			return r;
+		}
+		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(plan.maps.data()), reinterpret_cast<const uint8_t*>(plan.maps.data()) + maps_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(gather_lists.data()), reinterpret_cast<const uint8_t*>(gather_lists.data()) + lists_bytes);
+		// (from pageable memory: staged by the driver before the call returns)
+		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+		MetricListArgs a;
+		a.entries = ctx->list.as<const MetricEntry>();
+		a.maps = reinterpret_cast<const MetricMap*>(ctx->list.ptr + table_bytes);
+		a.lists = reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes + maps_bytes);
+		a.count = list_count;
+		a.slots = plan.slots;
+		a.bx = ctx->config.block_x;
+		a.by = ctx->config.block_y;
+		a.bz = bz;
+		a.components = input_components;
+		astc_block_error_lists_kernel<<<plan.grid, ASTC_METRIC_MAP_WARPS * 32, 0, s>>>(a);
+		ctx->launches++;
+		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+		return ASTCENC_SUCCESS;
+	});
 }
 
 // Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table goes

@@ -473,6 +473,74 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device_block_lists(struc
                                                                           const struct astcenc_swizzle* swizzle, void* cuda_stream);
 
 /**
+ * Decode block lists that live in device memory into device images: bring a decoded copy up to date after
+ * astcenc_b200_compress_device_block_lists (or compress_device_blocks) has re-encoded some of its blocks, without decoding the
+ * whole payload again.
+ * lists[i] describes a payload ALREADY RESIDENT in device memory (astcenc_compress_image's block order), the device image it
+ * decodes into (dim_z slices of dim_x * dim_y texels of data_type, contiguous, starting at any byte), a device index list and a
+ * device count. The list rule is that of astcenc_b200_compress_device_block_lists: the call reads the first min(*count, capacity)
+ * indices, and an index at or beyond the image's block count is skipped. For each listed block, the texels of its footprint that
+ * lie inside the image receive exactly the bytes astcenc_b200_decompress_device_images writes there for the whole payload (the
+ * swizzle, Z reconstruction, the error colour and the F16 void-extent behaviour included); every other byte of data is left
+ * untouched, and duplicate indices write the same texels. Takes 2D images, texture arrays (2D block sizes; z counts the slices)
+ * and volumes of 3D block sizes; works on decompress-only contexts. Outputs must not overlap each other or any payload (not
+ * checked). The descriptor array is copied. Enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in
+ * order with every other pass of the context: *count and the indices are read on the device when the call runs.
+ * Cost: the host does not know the counts, so the call is one table copy and one kernel launch over the sum of the capacities;
+ * a slot past the count does no work. Entries with capacity == 0 do nothing; a call whose capacities are all zero launches nothing.
+ * Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_PARAM for a NULL swizzle, then
+ * ASTCENC_ERR_BAD_SWIZZLE; ASTCENC_ERR_BAD_PARAM for lists == NULL with a non-zero count, an entry with a NULL payload or data, a
+ * NULL indices or count with capacity > 0, indices or count not aligned to 4 bytes, or a zero or overflowing dimension, then for a
+ * bad data type, then for an image of 2^32 blocks or more, or when the sum of the capacities overflows. All entries are checked
+ * before anything is enqueued.
+ */
+struct astcenc_b200_device_decode_block_list {
+	const uint8_t* payload;        /* device: the image's whole payload, astcenc_compress_image's block order */
+	void* data;                    /* device: dim_z slices of dim_x * dim_y texels of data_type, contiguous */
+	unsigned int dim_x, dim_y, dim_z;
+	const uint32_t* indices;       /* device: block positions in that order */
+	const uint32_t* count;         /* device: how many of the indices are listed */
+	unsigned int capacity;         /* at most this many indices are read; the call's cost */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_decompress_device_block_lists(struct astcenc_context* context,
+                                                                            const struct astcenc_b200_device_decode_block_list* lists,
+                                                                            unsigned int list_count, enum astcenc_type data_type,
+                                                                            const struct astcenc_swizzle* swizzle, void* cuda_stream);
+
+/**
+ * Refresh per-block error maps at the blocks of device block lists: after listed blocks have been re-encoded and re-decoded
+ * (astcenc_b200_decompress_device_block_lists), bring the map of astcenc_b200_compute_error_metrics_device_images up to date
+ * without measuring the whole image pair again.
+ * lists[i] describes an image pair ALREADY RESIDENT in device memory (as astcenc_b200_device_metrics_image does), its whole map
+ * (one float per block of the context's footprint, in astcenc_compress_image's block order), a device index list and a device
+ * count, read by the list rule of astcenc_b200_decompress_device_block_lists. For each listed block, block_error[index] receives
+ * bit for bit the value astcenc_b200_compute_error_metrics_device_images writes for that block of the same pair with the same
+ * input_components; every other map value is left untouched. No PSNR figures are produced. Works on decompress-only contexts.
+ * The descriptor array is copied. Enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in order with
+ * every other pass of the context. Cost: one table copy and one kernel launch, one warp per slot over the sum of the capacities.
+ * Entries with capacity == 0 do nothing; a call whose capacities are all zero launches nothing.
+ * Errors, in this order; on error nothing is launched and nothing is written: ASTCENC_ERR_BAD_PARAM for a NULL context or
+ * input_components outside 1-4, then for lists == NULL with a non-zero count, then for an entry with a NULL original or decoded, a
+ * NULL block_error, indices or count with capacity > 0, a zero or overflowing dimension, a bad data type, or a pointer not aligned
+ * to its element (4 / 8 / 16 bytes for a U8 / F16 / F32 texel, 4 for block_error, indices and count), then when the call does not
+ * fit a launch (an image of 2^32 blocks or more, or a grid beyond 2^31 - 1 CTAs). All entries are checked before anything is
+ * enqueued.
+ */
+struct astcenc_b200_device_block_error_list {
+	const void* original;          /* device: dim_z slices of dim_x * dim_y texels of original_type, contiguous */
+	const void* decoded;           /* device: the same shape, texels of decoded_type */
+	enum astcenc_type original_type, decoded_type;
+	unsigned int dim_x, dim_y, dim_z;
+	float* block_error;            /* device: the image's whole map, one float per block of the context's footprint */
+	const uint32_t* indices;       /* device: block positions in astcenc_compress_image's order */
+	const uint32_t* count;         /* device: how many of the indices are listed */
+	unsigned int capacity;         /* at most this many indices are read; the call's cost */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_errors_device_block_lists(struct astcenc_context* context, int input_components,
+                                                                                      const struct astcenc_b200_device_block_error_list* lists,
+                                                                                      unsigned int list_count, void* cuda_stream);
+
+/**
  * The .astc container (Docs/FileFormat.md; Source/astcenccli_image_load_store.cpp:2573-2760, load_cimage / store_cimage):
  * a 16-byte header - magic 13 AB A1 5C, block dimensions (one byte each), image dimensions (24 bits each, little endian)
  * - followed by the blocks as astcenc_compress_image() wrote them.

@@ -28,6 +28,8 @@ ERROR_NAMES = ["ASTCENC_SUCCESS", "ASTCENC_ERR_OUT_OF_MEM", "ASTCENC_ERR_BAD_CPU
 
 
 ERR_OUT_OF_MEM, ERR_BAD_PARAM, ERR_BAD_BLOCK_SIZE, ERR_BAD_SWIZZLE, ERR_BAD_CONTEXT, ERR_NOT_IMPLEMENTED = 1, 3, 4, 7, 9, 10
+# enum astcenc_b200_block_metric: what a per-block error map measures
+BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR, BLOCK_LOG2_ERROR = 0, 1, 2
 
 
 class AstcencError(RuntimeError):
@@ -174,6 +176,9 @@ def lib():
         l.astcenc_b200_compute_error_metrics_device_images.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(DeviceMetricsImage), C.c_uint,
                                                                        C.c_int, C.c_int, C.c_void_p]
         l.astcenc_b200_compute_error_metrics_device_images.restype = C.c_int
+        l.astcenc_b200_compute_block_metric_device_images.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(DeviceMetricsImage), C.c_uint,
+                                                                      C.c_int, C.c_int, C.c_void_p]
+        l.astcenc_b200_compute_block_metric_device_images.restype = C.c_int
         l.astcenc_b200_select_blocks.argtypes = [C.c_void_p, C.POINTER(BlockSelection), C.c_uint, C.c_void_p]
         l.astcenc_b200_select_blocks.restype = C.c_int
         l.astcenc_b200_compress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
@@ -183,6 +188,9 @@ def lib():
         l.astcenc_b200_decompress_device_block_lists.restype = C.c_int
         l.astcenc_b200_compute_block_errors_device_block_lists.argtypes = [C.c_void_p, C.c_int, C.POINTER(DeviceBlockErrorList), C.c_uint, C.c_void_p]
         l.astcenc_b200_compute_block_errors_device_block_lists.restype = C.c_int
+        l.astcenc_b200_compute_block_metric_device_block_lists.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(DeviceBlockErrorList), C.c_uint,
+                                                                           C.c_void_p]
+        l.astcenc_b200_compute_block_metric_device_block_lists.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -484,12 +492,23 @@ class Context:
         pair alone, and every block_error pointer one float per block of the context's footprint. Enqueued on `stream`, no sync;
         works on decompress-only contexts. ErrorMetrics.from_buffer_copy reads a struct back."""
         n = len(images)
-        table = (DeviceMetricsImage * n)(*[DeviceMetricsImage(C.c_void_p(o), C.c_void_p(d), ot, dt, x, y, z, C.c_void_p(m), C.c_void_p(b or None))
-                                           for o, d, ot, dt, x, y, z, m, b in images])
+        table = _metrics_table(images)
         err = lib().astcenc_b200_compute_error_metrics_device_images(self.handle, int(hdr), int(normal), input_components, table if n else None, n,
                                                                      fstop_lo, fstop_hi, C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compute_error_metrics_device_images")
+
+    def compute_block_metric_device_images(self, images, block_metric, hdr=False, normal=False, input_components=4, fstop_lo=-10, fstop_hi=10,
+                                           stream=0):
+        """compute_error_metrics_device_images with maps of `block_metric` (astcenc_b200_compute_block_metric_device_images):
+        BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR (each block's share of alpha_psnr's error sum) or BLOCK_LOG2_ERROR (each
+        block's share of log_rmse's). Same tuples, same figures; enqueued on `stream`, no sync."""
+        n = len(images)
+        table = _metrics_table(images)
+        err = lib().astcenc_b200_compute_block_metric_device_images(self.handle, int(hdr), int(normal), input_components, block_metric, table if n else None,
+                                                                    n, fstop_lo, fstop_hi, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compute_block_metric_device_images")
 
     def select_blocks(self, entries, stream=0):
         """Block selection from device maps (astcenc_b200_select_blocks). entries: a sequence of (d_map_ptr, block_count,
@@ -535,17 +554,41 @@ class Context:
         d_indices_ptr, d_count_ptr, capacity); each listed map value receives what compute_error_metrics_device_images writes for
         that block, and no other value changes. Enqueued on `stream`, no sync; works on decompress-only contexts."""
         n = len(lists)
-        table = (DeviceBlockErrorList * n)(*[DeviceBlockErrorList(C.c_void_p(o), C.c_void_p(d), ot, dt, x, y, z, C.c_void_p(b or None), C.c_void_p(i or None),
-                                                                  C.c_void_p(k or None), c)
-                                             for o, d, ot, dt, x, y, z, b, i, k, c in lists])
+        table = _block_error_list_table(lists)
         err = lib().astcenc_b200_compute_block_errors_device_block_lists(self.handle, input_components, table if n else None, n, C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compute_block_errors_device_block_lists")
+
+    def compute_block_metric_device_block_lists(self, lists, block_metric, input_components=4, stream=0):
+        """compute_block_errors_device_block_lists for maps of `block_metric` (astcenc_b200_compute_block_metric_device_block_lists):
+        each listed map value receives what compute_block_metric_device_images writes for that block with the same metric, and no
+        other value changes. Same tuples; enqueued on `stream`, no sync."""
+        n = len(lists)
+        table = _block_error_list_table(lists)
+        err = lib().astcenc_b200_compute_block_metric_device_block_lists(self.handle, input_components, block_metric, table if n else None, n,
+                                                                         C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compute_block_metric_device_block_lists")
 
     def last_timing(self):
         ms = C.c_float(); a = C.c_size_t(); b = C.c_size_t()
         lib().astcenc_b200_last_timing(self.handle, C.byref(ms), C.byref(a), C.byref(b))
         return ms.value, a.value, b.value
+
+
+def _metrics_table(images):
+    """The astcenc_b200_device_metrics_image array of (d_original_ptr, d_decoded_ptr, original_type, decoded_type, dim_x, dim_y,
+    dim_z, d_metrics_ptr, d_block_error_ptr or 0) tuples."""
+    return (DeviceMetricsImage * len(images))(*[DeviceMetricsImage(C.c_void_p(o), C.c_void_p(d), ot, dt, x, y, z, C.c_void_p(m), C.c_void_p(b or None))
+                                                for o, d, ot, dt, x, y, z, m, b in images])
+
+
+def _block_error_list_table(lists):
+    """The astcenc_b200_device_block_error_list array of (d_original_ptr, d_decoded_ptr, original_type, decoded_type, dim_x, dim_y,
+    dim_z, d_block_error_ptr, d_indices_ptr, d_count_ptr, capacity) tuples."""
+    return (DeviceBlockErrorList * len(lists))(*[DeviceBlockErrorList(C.c_void_p(o), C.c_void_p(d), ot, dt, x, y, z, C.c_void_p(b or None),
+                                                                      C.c_void_p(i or None), C.c_void_p(k or None), c)
+                                                 for o, d, ot, dt, x, y, z, b, i, k, c in lists])
 
 
 def store_cimage(filename, blocks, dim_x, dim_y, block_x, block_y, dim_z=1, block_z=1):

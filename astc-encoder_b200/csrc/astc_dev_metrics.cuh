@@ -17,7 +17,9 @@
 // The per-block error map (block_error_sum) is one warp per block of the context's footprint, in astcenc_compress_image's
 // block order; it compiles for the host simulation too (tests/hostsim/hostsim_metrics.cpp). A list refresh
 // (astcenc_b200_compute_block_errors_device_block_lists) runs the same function at the slots of device block lists, one warp per
-// slot (tests/hostsim/hostsim_map_lists.cpp).
+// slot (tests/hostsim/hostsim_map_lists.cpp). A map measures one enum astcenc_b200_block_metric (metric_block_terms): the
+// squared error on astc_block_error_kernel / astc_block_error_lists_kernel, the alpha-weighted and log2 errors on
+// astc_block_metric_kernel<M> / astc_block_metric_lists_kernel<M>, all through block_error_sum<M>.
 #pragma once
 #include <vector>
 #include "../../include/astcenc.h"
@@ -211,13 +213,53 @@ ASTC_HD int metric_component_mask(int input_components) {
 	return input_components == 2 ? 0x0C : input_components == 4 ? 0x0F : 0x07;
 }
 
+// the reference's approximate log2 (astcenc_vecmathlib.h:416-441), unfused
+ASTC_FN float metric_log2(float x) {
+	int i = (int)ASTC_F2U(x);
+	float e = (float)(((i & 0x7F800000) >> 23) - 127);
+	float m = ASTC_U2F((uint32_t)((i & 0x007FFFFF) | 0x3F800000));
+	float p = 0.0596515482674574969533f;
+	p = p * m + -0.465725644288844778798f;
+	p = p * m + 1.48116647521213171641f;
+	p = p * m + -2.52074962577807006663f;
+	p = p * m + 2.8882704548164776201f;
+	p = p * (m - 1.0f);
+	return p + e;
+}
+
 // ---- the per-block error map ----
+
+// The terms of one texel of a map of metric M (enum astcenc_b200_block_metric) over the channels in `mask`, c1 the original and
+// c2 the decoded texel, added to acc in channel order. Each term is a float square of float values, added in double:
+//   SQUARED_ERROR         (c1 - c2)^2 per channel, the MS_ERR terms of the sums
+//   ALPHA_WEIGHTED_ERROR  ((c1 - c2) * c1.w)^2 per RGB channel and (c1.w - c2.w)^2 for alpha, the MS_AERR terms
+//   LOG2_ERROR            (log2(c1) - log2(c2))^2 per RGB channel, the MS_LOG terms
+template <int M>
+ASTC_FN void metric_block_terms(const f4& c1, const f4& c2, int mask, double& acc) {
+	if (M == ASTCENC_B200_BLOCK_LOG2_ERROR) {
+		const float o[3] = {c1.x, c1.y, c1.z}, q[3] = {c2.x, c2.y, c2.z};
+		for (int k = 0; k < 3; k++) {
+			if (mask & (1 << k)) {
+				const float l = metric_log2(o[k]) - metric_log2(q[k]);
+				acc += (double)(l * l);
+			}
+		}
+		return;
+	}
+	const float d[4] = {c1.x - c2.x, c1.y - c2.y, c1.z - c2.z, c1.w - c2.w};
+	for (int k = 0; k < 4; k++) {
+		if (mask & (1 << k)) {
+			const float v = M == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR && k < 3 ? d[k] * c1.w : d[k];
+			acc += (double)(v * v);
+		}
+	}
+}
 
 // Map block `index` of entry e (astcenc_compress_image's block order for the footprint bx x by x bz; a 2D footprint's index
 // counts the slices of a texture array), by `lanes` lanes of one warp: the sum, over the block's texels inside the image, of
-// the squared differences of the channels in `mask`, each the float square of a float difference as in the sums, added in
-// double. Lane l takes texels l, l + lanes, ... in footprint order, then the lanes are summed in a fixed xor-shuffle order.
-// Every lane returns the sum.
+// the terms of metric M (metric_block_terms) of the channels in `mask`, added in double. Lane l takes texels l, l + lanes, ... in
+// footprint order, then the lanes are summed in a fixed xor-shuffle order. Every lane returns the sum.
+template <int M = ASTCENC_B200_BLOCK_SQUARED_ERROR>
 ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index, int mask, int lane, int lanes) {
 	double acc = 0.0;
 	for (unsigned int t = (unsigned int)lane; t < bx * by * bz; t += (unsigned int)lanes) {
@@ -228,12 +270,7 @@ ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned i
 		}
 		const f4 c1 = metric_texel(e.img1, e.type1, z * e.stride1 + (size_t)e.pitch1 * y + x);
 		const f4 c2 = metric_texel(e.img2, e.type2, z * e.stride2 + (size_t)e.pitch2 * y + x);
-		const float d[4] = {c1.x - c2.x, c1.y - c2.y, c1.z - c2.z, c1.w - c2.w};
-		for (int k = 0; k < 4; k++) {
-			if (mask & (1 << k)) {
-				acc += (double)(d[k] * d[k]);
-			}
-		}
+		metric_block_terms<M>(c1, c2, mask, acc);
 	}
 #if !defined(ASTC_ONE_LANE)
 	for (int o = lanes / 2; o > 0; o >>= 1) {
@@ -243,8 +280,9 @@ ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned i
 	return acc;
 }
 
-// Slot w < a.slots of a list refresh, by `lanes` lanes of one warp: block_error_sum of the listed block into its map value. An
+// Slot w < a.slots of a list refresh, by `lanes` lanes of one warp: block_error_sum<M> of the listed block into its map value. An
 // entry with capacity 0 owns no slot, and a slot past the count or out of range writes nothing.
+template <int M = ASTCENC_B200_BLOCK_SQUARED_ERROR>
 ASTC_FN void block_error_list_slot(const MetricListArgs& a, size_t w, int lane, int lanes) {
 	const MetricMap& m = a.maps[find_image(a.maps, a.count, w)];
 	const uint32_t index = list_slot(a.lists[m.entry], w - m.first);
@@ -252,7 +290,7 @@ ASTC_FN void block_error_list_slot(const MetricListArgs& a, size_t w, int lane, 
 		return;      // (the whole warp)
 	}
 	const MetricEntry& e = a.entries[m.entry];
-	const double s = block_error_sum(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), lane, lanes);
+	const double s = block_error_sum<M>(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), lane, lanes);
 	if (lane == 0) {
 		e.block_error[index] = (float)s;
 	}
@@ -306,20 +344,6 @@ ASTC_HD void metric_close(const double* sums, int hdr, int normal, int input_com
 }
 
 #if !defined(ASTC_HOSTSIM)
-// the reference's approximate log2 (astcenc_vecmathlib.h:416-441), unfused
-static __device__ __forceinline__ float metric_log2(float x) {
-	int i = __float_as_int(x);
-	float e = (float)(((i & 0x7F800000) >> 23) - 127);
-	float m = __int_as_float((i & 0x007FFFFF) | 0x3F800000);
-	float p = 0.0596515482674574969533f;
-	p = p * m + -0.465725644288844778798f;
-	p = p * m + 1.48116647521213171641f;
-	p = p * m + -2.52074962577807006663f;
-	p = p * m + 2.8882704548164776201f;
-	p = p * (m - 1.0f);
-	return p + e;
-}
-
 // mpsnr_operator / mpsnr_sumdiff (astcenccli_error_metrics.cpp:69-107)
 static __device__ __forceinline__ float metric_mpsnr_operator(float val, int fstop) {
 	float scale = __uint_as_float(0x3f800000u + ((unsigned int)fstop << 23));
@@ -457,9 +481,9 @@ astc_error_metrics_finish_kernel(const __grid_constant__ MetricArgs a) {
 	}
 }
 
-// The map: warp w of the launch is block w - first of its mapped entry.
-__global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
-astc_block_error_kernel(const __grid_constant__ MetricArgs a) {
+// The map of metric M: warp w of the launch is block w - first of its mapped entry.
+template <int M>
+static __device__ __forceinline__ void block_map_warp(const MetricArgs& a) {
 	const size_t w = (size_t)blockIdx.x * ASTC_METRIC_MAP_WARPS + (threadIdx.x >> 5);
 	if (w >= a.map_blocks) {
 		return;      // (the whole warp)
@@ -467,18 +491,41 @@ astc_block_error_kernel(const __grid_constant__ MetricArgs a) {
 	const MetricMap& m = a.maps[find_image(a.maps, a.map_count, w)];
 	const MetricEntry& e = a.entries[m.entry];
 	const uint32_t index = (uint32_t)(w - m.first);      // (a mapped entry has fewer than 2^32 blocks)
-	const double s = block_error_sum(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), threadIdx.x & 31, ASTC_WARP);
+	const double s = block_error_sum<M>(e, a.bx, a.by, a.bz, index, metric_component_mask(a.components), threadIdx.x & 31, ASTC_WARP);
 	if ((threadIdx.x & 31) == 0) {
 		e.block_error[index] = (float)s;
 	}
 }
 
-// A list refresh of maps: warp w of the launch is slot w of the call.
+// The squared-error map (ASTCENC_B200_BLOCK_SQUARED_ERROR).
+__global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
+astc_block_error_kernel(const __grid_constant__ MetricArgs a) {
+	block_map_warp<ASTCENC_B200_BLOCK_SQUARED_ERROR>(a);
+}
+
+// The maps of the other metrics: one instantiation each (ALPHA_WEIGHTED_ERROR, LOG2_ERROR).
+template <int M>
+__global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
+astc_block_metric_kernel(const __grid_constant__ MetricArgs a) {
+	block_map_warp<M>(a);
+}
+
+// A list refresh of squared-error maps: warp w of the launch is slot w of the call.
 __global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
 astc_block_error_lists_kernel(const __grid_constant__ MetricListArgs a) {
 	const size_t w = (size_t)blockIdx.x * ASTC_METRIC_MAP_WARPS + (threadIdx.x >> 5);
 	if (w < a.slots) {
 		block_error_list_slot(a, w, threadIdx.x & 31, ASTC_WARP);
+	}
+}
+
+// A list refresh of maps of metric M (ALPHA_WEIGHTED_ERROR, LOG2_ERROR).
+template <int M>
+__global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
+astc_block_metric_lists_kernel(const __grid_constant__ MetricListArgs a) {
+	const size_t w = (size_t)blockIdx.x * ASTC_METRIC_MAP_WARPS + (threadIdx.x >> 5);
+	if (w < a.slots) {
+		block_error_list_slot<M>(a, w, threadIdx.x & 31, ASTC_WARP);
 	}
 }
 #endif

@@ -1536,10 +1536,10 @@ astcenc_error astcenc_get_block_info(astcenc_context* ctx, const uint8_t data[16
 }
 
 // One metrics call of a planned table (plan_metrics) on `stream`, inside a scratch turn: the table and the map list go up into
-// the context's table buffer (ctx->list) in one copy, the metrics kernel and the finish kernel run, then the map kernel when
-// an entry asks for a map. The sums of entry j are left at ctx->metric_partials + (plan.ctas + j) * ASTC_METRIC_SUMS doubles.
+// the context's table buffer (ctx->list) in one copy, the metrics kernel and the finish kernel run, then the map kernel of
+// block_metric when an entry asks for a map. The sums of entry j are left at ctx->metric_partials + (plan.ctas + j) * ASTC_METRIC_SUMS doubles.
 static astcenc_error launch_metrics(astcenc_context* ctx, const std::vector<MetricEntry>& table, const MetricPlan& plan, int hdr, int normal,
-                                    int input_components, int fstop_lo, int fstop_hi, cudaStream_t stream) {
+                                    int input_components, astcenc_b200_block_metric block_metric, int fstop_lo, int fstop_hi, cudaStream_t stream) {
 	const size_t table_bytes = table.size() * sizeof(MetricEntry);
 	const size_t map_bytes = plan.maps.size() * sizeof(MetricMap);
 	std::vector<uint8_t> up(table_bytes + map_bytes);
@@ -1575,7 +1575,14 @@ static astcenc_error launch_metrics(astcenc_context* ctx, const std::vector<Metr
 	astc_error_metrics_finish_kernel<<<plan.finish_grid, ASTC_METRIC_FINISH_GROUPS * ASTC_METRIC_SUMS, 0, stream>>>(a);
 	ctx->launches++;
 	if (plan.map_grid != 0) {
-		astc_block_error_kernel<<<plan.map_grid, ASTC_METRIC_MAP_WARPS * 32, 0, stream>>>(a);
+		const dim3 grid(plan.map_grid), cta(ASTC_METRIC_MAP_WARPS * 32);
+		if (block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
+			astc_block_metric_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, cta, 0, stream>>>(a);
+		} else if (block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
+			astc_block_metric_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, cta, 0, stream>>>(a);
+		} else {
+			astc_block_error_kernel<<<grid, cta, 0, stream>>>(a);
+		}
 		ctx->launches++;
 	}
 	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
@@ -1639,7 +1646,8 @@ astcenc_error astcenc_b200_compute_error_metrics(astcenc_context* ctx, int compu
 		}
 		e.img1 = ctx->image.ptr;
 		e.img2 = ctx->image2.ptr;
-		r = launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, fstop_lo, fstop_hi, ctx->stream);
+		r = launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, ASTCENC_B200_BLOCK_SQUARED_ERROR, fstop_lo,
+		                   fstop_hi, ctx->stream);
 		if (r == ASTCENC_SUCCESS) {
 			CUDA_TRY(cudaMemcpyAsync(sums, ctx->metric_partials.as<double>() + plan.ctas * ASTC_METRIC_SUMS, sizeof(sums), cudaMemcpyDeviceToHost, ctx->stream),
 			         return ASTCENC_ERR_BAD_CONTEXT);
@@ -2026,12 +2034,22 @@ astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const 
 	return scratch_turn(ctx, s, [&] { return launch_decode(ctx, table.data(), image_count, blocks, (int)data_type, *swizzle, s); });
 }
 
+// A map's metric is one of enum astcenc_b200_block_metric (the value arrives through the C ABI as any int).
+static bool check_block_metric(astcenc_b200_block_metric block_metric) {
+	const int m = (int)block_metric;
+	return m >= ASTCENC_B200_BLOCK_SQUARED_ERROR && m <= ASTCENC_B200_BLOCK_LOG2_ERROR;
+}
+
 // Metrics calls: every pair is checked before anything is enqueued; the table goes up in one copy and the call is two
-// launches, three with a map, in one scratch turn.
-astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* ctx, int compute_hdr_metrics, int compute_normal_metrics,
-                                                               int input_components, const astcenc_b200_device_metrics_image* images,
-                                                               unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream) {
+// launches, three with a map (of block_metric), in one scratch turn.
+astcenc_error astcenc_b200_compute_block_metric_device_images(astcenc_context* ctx, int compute_hdr_metrics, int compute_normal_metrics,
+                                                              int input_components, astcenc_b200_block_metric block_metric,
+                                                              const astcenc_b200_device_metrics_image* images, unsigned int image_count,
+                                                              int fstop_lo, int fstop_hi, void* cuda_stream) {
 	if (!ctx || input_components < 1 || input_components > 4) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (!check_block_metric(block_metric)) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
 	if (fstop_lo < -125 || fstop_hi > 125) {
@@ -2076,8 +2094,15 @@ astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* 
 	}
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return scratch_turn(ctx, s, [&] {
-		return launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, fstop_lo, fstop_hi, s);
+		return launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, block_metric, fstop_lo, fstop_hi, s);
 	});
+}
+
+astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* ctx, int compute_hdr_metrics, int compute_normal_metrics,
+                                                               int input_components, const astcenc_b200_device_metrics_image* images,
+                                                               unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream) {
+	return astcenc_b200_compute_block_metric_device_images(ctx, compute_hdr_metrics, compute_normal_metrics, input_components, ASTCENC_B200_BLOCK_SQUARED_ERROR,
+	                                                       images, image_count, fstop_lo, fstop_hi, cuda_stream);
 }
 
 // Device block lists: an image table whose entry j owns capacity[j] staging blocks, the slots of its device list (GatherList).
@@ -2179,11 +2204,15 @@ astcenc_error astcenc_b200_decompress_device_block_lists(astcenc_context* ctx, c
 }
 
 // Map refreshes over device block lists: every entry is checked before anything is enqueued, in the order of the metrics call;
-// the table, its first slots and its lists go up in one copy and one launch refreshes every slot, in one scratch turn.
-astcenc_error astcenc_b200_compute_block_errors_device_block_lists(astcenc_context* ctx, int input_components,
-                                                                   const astcenc_b200_device_block_error_list* lists, unsigned int list_count,
-                                                                   void* cuda_stream) {
+// the table, its first slots and its lists go up in one copy and one launch of block_metric's kernel refreshes every slot, in
+// one scratch turn.
+astcenc_error astcenc_b200_compute_block_metric_device_block_lists(astcenc_context* ctx, int input_components, astcenc_b200_block_metric block_metric,
+                                                                  const astcenc_b200_device_block_error_list* lists, unsigned int list_count,
+                                                                  void* cuda_stream) {
 	if (!ctx || input_components < 1 || input_components > 4) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (!check_block_metric(block_metric)) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
 	if (list_count != 0 && !lists) {
@@ -2255,11 +2284,24 @@ astcenc_error astcenc_b200_compute_block_errors_device_block_lists(astcenc_conte
 		a.by = ctx->config.block_y;
 		a.bz = bz;
 		a.components = input_components;
-		astc_block_error_lists_kernel<<<plan.grid, ASTC_METRIC_MAP_WARPS * 32, 0, s>>>(a);
+		const dim3 grid(plan.grid), cta(ASTC_METRIC_MAP_WARPS * 32);
+		if (block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
+			astc_block_metric_lists_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, cta, 0, s>>>(a);
+		} else if (block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
+			astc_block_metric_lists_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, cta, 0, s>>>(a);
+		} else {
+			astc_block_error_lists_kernel<<<grid, cta, 0, s>>>(a);
+		}
 		ctx->launches++;
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		return ASTCENC_SUCCESS;
 	});
+}
+
+astcenc_error astcenc_b200_compute_block_errors_device_block_lists(astcenc_context* ctx, int input_components,
+                                                                   const astcenc_b200_device_block_error_list* lists, unsigned int list_count,
+                                                                   void* cuda_stream) {
+	return astcenc_b200_compute_block_metric_device_block_lists(ctx, input_components, ASTCENC_B200_BLOCK_SQUARED_ERROR, lists, list_count, cuda_stream);
 }
 
 // Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table goes

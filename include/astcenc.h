@@ -409,6 +409,42 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_error_metrics_device_imag
                                                                                   unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream);
 
 /**
+ * What a per-block error map measures (astcenc_b200_compute_block_metric_device_images and
+ * astcenc_b200_compute_block_metric_device_block_lists). Every map value is a sum over the block's texels inside the image, with
+ * o the original texel and d the decoded one in the units of sum_squared_error (U8 scaled to 0..1, F16 / F32 clamped to
+ * [0, 65504]) and m the channels input_components selects. Each term is computed in float, added in double in a fixed order, and
+ * the block's sum is rounded to float once; a value depends only on that block's texels.
+ * ASTCENC_B200_BLOCK_SQUARED_ERROR: (o_c - d_c)^2 for c in m; the map of astcenc_b200_compute_error_metrics_device_images. Summed
+ *   over the image, the masked sum of sum_squared_error.
+ * ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR: ((o_c - d_c) * o_A)^2 for c in m among R, G, B, plus (o_A - d_A)^2 when A is in m. The
+ *   block's share of the error sum behind alpha_psnr: RGB error under transparent texels does not count. Summed over the image
+ *   with input_components == 4, samples / 10^(alpha_psnr / 10).
+ * ASTCENC_B200_BLOCK_LOG2_ERROR: (L(o_c) - L(d_c))^2 for c in m among R, G, B, L the polynomial log2 the HDR figures use. The
+ *   block's share of the error sum behind log_rmse, measured whether or not HDR figures are asked for: errors in dark and mid
+ *   tones weigh as much as errors in the brightest blocks. Summed over the image and divided by the pixel count, log_rmse^2.
+ * The image sums agree with the figures up to the per-block float rounding.
+ */
+enum astcenc_b200_block_metric {
+	ASTCENC_B200_BLOCK_SQUARED_ERROR = 0,
+	ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR = 1,
+	ASTCENC_B200_BLOCK_LOG2_ERROR = 2
+};
+
+/**
+ * astcenc_b200_compute_error_metrics_device_images with a chosen per-block error map: every block_error map receives
+ * block_metric (enum astcenc_b200_block_metric) instead of the squared error. Everything else is that call's: the figures (bit for
+ * bit the same), the stream, the descriptor table, decompress-only contexts, the launch count (two kernel launches, three when any
+ * entry asks for a map) and the error order, into which one check is inserted: ASTCENC_ERR_BAD_PARAM for block_metric outside 0-2
+ * comes right after the check of input_components. With ASTCENC_B200_BLOCK_SQUARED_ERROR the call is
+ * astcenc_b200_compute_error_metrics_device_images.
+ */
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_metric_device_images(struct astcenc_context* context, int compute_hdr_metrics,
+                                                                                 int compute_normal_metrics, int input_components,
+                                                                                 enum astcenc_b200_block_metric block_metric,
+                                                                                 const struct astcenc_b200_device_metrics_image* images,
+                                                                                 unsigned int image_count, int fstop_lo, int fstop_hi, void* cuda_stream);
+
+/**
  * Block selection on the device: turn per-block error maps (astcenc_b200_compute_error_metrics_device_images) into device block
  * lists (astcenc_b200_compress_device_block_lists) without a trip through host memory.
  * One rule per entry: a block is a candidate when map[b] > threshold (NaN never is; -0.0 counts as 0.0). Of c candidates the
@@ -537,6 +573,19 @@ struct astcenc_b200_device_block_error_list {
 	unsigned int capacity;         /* at most this many indices are read; the call's cost */
 };
 ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_errors_device_block_lists(struct astcenc_context* context, int input_components,
+                                                                                      const struct astcenc_b200_device_block_error_list* lists,
+                                                                                      unsigned int list_count, void* cuda_stream);
+
+/**
+ * astcenc_b200_compute_block_errors_device_block_lists for a map of block_metric (enum astcenc_b200_block_metric): each listed
+ * value receives bit for bit what astcenc_b200_compute_block_metric_device_images writes for that block with the same
+ * input_components and block_metric, and every other value is left untouched. Everything else is that call's: the list rule, the
+ * stream, decompress-only contexts, one kernel launch (none when the capacities are all zero) and the error order, into which one
+ * check is inserted: ASTCENC_ERR_BAD_PARAM for block_metric outside 0-2 comes right after the check of input_components. With
+ * ASTCENC_B200_BLOCK_SQUARED_ERROR the call is astcenc_b200_compute_block_errors_device_block_lists.
+ */
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_metric_device_block_lists(struct astcenc_context* context, int input_components,
+                                                                                      enum astcenc_b200_block_metric block_metric,
                                                                                       const struct astcenc_b200_device_block_error_list* lists,
                                                                                       unsigned int list_count, void* cuda_stream);
 

@@ -105,6 +105,12 @@ class DeviceBlockErrorList(C.Structure):
                 ("capacity", C.c_uint)]
 
 
+class DeviceRefineList(C.Structure):
+    """struct astcenc_b200_device_refine_list (include/astcenc.h)."""
+    _fields_ = [("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("payload", C.c_void_p), ("decoded", C.c_void_p),
+                ("block_error", C.c_void_p), ("indices", C.c_void_p), ("count", C.c_void_p), ("capacity", C.c_uint)]
+
+
 class ErrorMetrics(C.Structure):
     """struct astcenc_b200_error_metrics (include/astcenc.h)."""
     _fields_ = [(n, C.c_double) for n in ("psnr", "alpha_psnr", "rgb_psnr", "rgb_peak", "peak_psnr", "mpsnr", "log_rmse",
@@ -191,6 +197,9 @@ def lib():
         l.astcenc_b200_compute_block_metric_device_block_lists.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(DeviceBlockErrorList), C.c_uint,
                                                                            C.c_void_p]
         l.astcenc_b200_compute_block_metric_device_block_lists.restype = C.c_int
+        l.astcenc_b200_refine_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceRefineList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_int,
+                                                             C.POINTER(Swizzle), C.c_int, C.c_int, C.c_void_p]
+        l.astcenc_b200_refine_device_block_lists.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -569,6 +578,25 @@ class Context:
                                                                          C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_compute_block_metric_device_block_lists")
+
+    def refine_device_block_lists(self, lists, data_type, decoded_type, block_metric, swizzle=(0, 1, 2, 3), decode_swizzle=(0, 1, 2, 3),
+                                  input_components=4, stream=0):
+        """Re-encode device-resident block lists and keep each new block only where it lowers the block's value in its map
+        (astcenc_b200_refine_device_block_lists). lists: a sequence of (d_pixels_ptr, dim_x, dim_y, dim_z, d_payload_ptr,
+        d_decoded_ptr or 0, d_block_error_ptr, d_indices_ptr, d_count_ptr, capacity). For the first min(*count, capacity) indices
+        in range, the candidate (what compress_device_block_lists would write) is decoded by this context to decoded_type with
+        decode_swizzle and measured in block_metric over input_components; where that value is below the map's, the payload
+        bytes, the decoded texels and the map value are replaced. Enqueued on `stream`, no sync."""
+        n = len(lists)
+        table = (DeviceRefineList * n)(*[DeviceRefineList(C.c_void_p(p), x, y, z, C.c_void_p(q), C.c_void_p(d or None), C.c_void_p(b or None),
+                                                          C.c_void_p(i or None), C.c_void_p(k or None), c)
+                                         for p, x, y, z, q, d, b, i, k, c in lists])
+        sw = Swizzle(*swizzle)
+        dsw = Swizzle(*decode_swizzle)
+        err = lib().astcenc_b200_refine_device_block_lists(self.handle, table if n else None, n, data_type, C.byref(sw), decoded_type, C.byref(dsw),
+                                                           input_components, block_metric, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_refine_device_block_lists")
 
     def last_timing(self):
         ms = C.c_float(); a = C.c_size_t(); b = C.c_size_t()

@@ -155,6 +155,20 @@ ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i) {
 	return index == GATHER_INVALID ? nullptr : g.images[j].payload + (size_t)index * 16;
 }
 
+#if !defined(ASTC_HOSTSIM)
+// A block's 16 bytes to its payload position: one vector store where the position is aligned, byte stores otherwise.
+static __device__ __forceinline__ void store_block(uint8_t* dst, const uint4& v) {
+	if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
+		*reinterpret_cast<uint4*>(dst) = v;
+	} else {
+		const uint8_t* b = reinterpret_cast<const uint8_t*>(&v);
+		for (int k = 0; k < 16; k++) {
+			dst[k] = b[k];
+		}
+	}
+}
+#endif
+
 // ---- image tables of a decode call (astc_decompress_images_kernel) ----
 // Call block c is block c - first[j] of image j, found by find_image. decompress_block reads its image from the CTA's launch
 // constants (IMG), so a CTA decodes its blocks one plane at a time and restages IMG between planes behind a barrier. A plane is

@@ -256,11 +256,14 @@ ASTC_FN void metric_block_terms(const f4& c1, const f4& c2, int mask, double& ac
 }
 
 // Map block `index` of entry e (astcenc_compress_image's block order for the footprint bx x by x bz; a 2D footprint's index
-// counts the slices of a texture array), by `lanes` lanes of one warp: the sum, over the block's texels inside the image, of
-// the terms of metric M (metric_block_terms) of the channels in `mask`, added in double. Lane l takes texels l, l + lanes, ... in
-// footprint order, then the lanes are summed in a fixed xor-shuffle order. Every lane returns the sum.
-template <int M = ASTCENC_B200_BLOCK_SQUARED_ERROR>
-ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index, int mask, int lane, int lanes) {
+// counts the slices of a texture array), by `lanes` lanes of one warp, against the decoded texels `decoded` gives: the sum, over
+// the block's texels inside the image, of the terms of metric M (metric_block_terms) of the channels in `mask`, added in double.
+// decoded(t, x, y, z) is the decoded texel of footprint texel t at image position (x, y, z). Lane l takes texels l, l + lanes, ...
+// in footprint order, then the lanes are summed in a fixed xor-shuffle order. Every lane returns the sum. So a value depends on
+// where the decoded texels live only through what `decoded` returns.
+template <int M, typename Decoded>
+ASTC_FN double block_error_sum_of(const MetricEntry& e, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index, int mask, int lane, int lanes,
+                                  const Decoded& decoded) {
 	double acc = 0.0;
 	for (unsigned int t = (unsigned int)lane; t < bx * by * bz; t += (unsigned int)lanes) {
 		unsigned int tx, ty, tz, x, y, z;
@@ -269,7 +272,7 @@ ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned i
 			continue;
 		}
 		const f4 c1 = metric_texel(e.img1, e.type1, z * e.stride1 + (size_t)e.pitch1 * y + x);
-		const f4 c2 = metric_texel(e.img2, e.type2, z * e.stride2 + (size_t)e.pitch2 * y + x);
+		const f4 c2 = decoded(t, x, y, z);
 		metric_block_terms<M>(c1, c2, mask, acc);
 	}
 #if !defined(ASTC_ONE_LANE)
@@ -278,6 +281,14 @@ ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned i
 	}
 #endif
 	return acc;
+}
+
+// block_error_sum_of against the pair's decoded image (img2).
+template <int M = ASTCENC_B200_BLOCK_SQUARED_ERROR>
+ASTC_FN double block_error_sum(const MetricEntry& e, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index, int mask, int lane, int lanes) {
+	return block_error_sum_of<M>(e, bx, by, bz, index, mask, lane, lanes, [&](unsigned int, unsigned int x, unsigned int y, unsigned int z) {
+		return metric_texel(e.img2, e.type2, z * e.stride2 + (size_t)e.pitch2 * y + x);
+	});
 }
 
 // Slot w < a.slots of a list refresh, by `lanes` lanes of one warp: block_error_sum<M> of the listed block into its map value. An

@@ -23,6 +23,7 @@
 #include "astc_dev_search.cuh"
 #include "astc_dev_gather.cuh"
 #include "astc_dev_metrics.cuh"
+#include "astc_dev_refine.cuh"
 #include "astc_dev_select.cuh"
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
@@ -229,14 +230,7 @@ astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_cons
 	if (dst == nullptr) {
 		return;      // (an invalid list slot)
 	}
-	if ((reinterpret_cast<uintptr_t>(dst) & 15) == 0) {
-		*reinterpret_cast<uint4*>(dst) = v;
-	} else {
-		const uint8_t* b = reinterpret_cast<const uint8_t*>(&v);
-		for (int k = 0; k < 16; k++) {
-			dst[k] = b[k];
-		}
-	}
+	store_block(dst, v);
 }
 
 // ---- decompression (SURVEY.md section 8f) over image tables (astcenc_decompress_image, astcenc_b200_decompress_device_images):
@@ -427,6 +421,8 @@ struct astcenc_context {
 	// staging calls (astc_dev_gather.cuh), grown on demand: the table with its lists, the staging image and payload of one chunk,
 	// the pre-pass averages of the source images
 	DevBuffer list, list_image, list_out, list_alpha;
+	// refine calls: one chunk's decoded candidates (a staging row), then its candidate values and decisions
+	DevBuffer refine;
 	// metrics calls: the partial sums of every virtual CTA and the sums of every pair, grown on demand
 	DevBuffer metric_partials;
 	// selection calls: the entries, their histograms and the tile counts
@@ -672,7 +668,7 @@ void astcenc_context_free(astcenc_context* ctx) {
 	cudaFree(ctx->d_ticket);
 	cudaFree(ctx->d_counters);
 	for (DevBuffer* b : {&ctx->records, &ctx->queues, &ctx->alpha, &ctx->image, &ctx->image2, &ctx->out, &ctx->list, &ctx->list_image, &ctx->list_out,
-	                     &ctx->list_alpha, &ctx->metric_partials, &ctx->select}) {
+	                     &ctx->list_alpha, &ctx->refine, &ctx->metric_partials, &ctx->select}) {
 		cudaFree(b->ptr);
 	}
 	for (cudaEvent_t e : ctx->stage_events) {
@@ -1388,6 +1384,17 @@ static astcenc_error table_entry(const astcenc_context* ctx, int data_type, unsi
 	return ASTCENC_SUCCESS;
 }
 
+// One launch decodes the `blocks` call blocks of the image table at `d_table` (device) on `stream`.
+static void enqueue_decode(astcenc_context* ctx, const GatherImage* d_table, unsigned int image_count, size_t blocks, int data_type,
+                           const astcenc_swizzle& swizzle, cudaStream_t stream) {
+	const unsigned int warps = ASTC_DECODE_THREADS / 32;
+	const size_t ctas = (blocks + warps - 1) / warps;
+	const unsigned int grid = ctas < (size_t)ctx->sm_count * 8 ? (unsigned int)ctas : (unsigned int)ctx->sm_count * 8;
+	astc_decompress_images_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, stream>>>(
+	    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, data_type, 0, 0, 0, swizzle), d_table, image_count, blocks);
+	ctx->launches++;
+}
+
 // One launch decodes the `blocks` call blocks of an image table on `stream` (inside a scratch turn: the table goes up into the
 // context's table buffer, ctx->list).
 static astcenc_error launch_decode(astcenc_context* ctx, const GatherImage* table, unsigned int image_count, size_t blocks, int data_type,
@@ -1398,12 +1405,7 @@ static astcenc_error launch_decode(astcenc_context* ctx, const GatherImage* tabl
 	}
 	// (from pageable memory: staged by the driver before the call returns)
 	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, table, image_count * sizeof(GatherImage), cudaMemcpyHostToDevice, stream), return ASTCENC_ERR_BAD_CONTEXT);
-	const unsigned int warps = ASTC_DECODE_THREADS / 32;
-	const size_t ctas = (blocks + warps - 1) / warps;
-	const unsigned int grid = ctas < (size_t)ctx->sm_count * 8 ? (unsigned int)ctas : (unsigned int)ctx->sm_count * 8;
-	astc_decompress_images_kernel<<<grid, ASTC_DECODE_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, stream>>>(
-	    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, data_type, 0, 0, 0, swizzle), ctx->list.as<const GatherImage>(), image_count, blocks);
-	ctx->launches++;
+	enqueue_decode(ctx, ctx->list.as<const GatherImage>(), image_count, blocks, data_type, swizzle, stream);
 	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 	return ASTCENC_SUCCESS;
 }
@@ -1710,25 +1712,38 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 }
 
 // One entry of a staging call: an image and its payload (plan_blocks sets `first` and `avg_offset`), its list (null: every
-// block), the staging blocks it owns (the image's blocks, or the list's capacity) and the block rows [row0, row1) of its
-// alpha-scale pre-pass, clamped to the image: the rows a host list touches, else the whole image.
+// block), the staging blocks it owns (the image's blocks, or the list's capacity), the block rows [row0, row1) of its
+// alpha-scale pre-pass, clamped to the image: the rows a host list touches, else the whole image; and in a refine call its pair.
 struct BlockEntry {
 	GatherImage image{};
 	const GatherList* list = nullptr;
 	size_t blocks = 0;
 	unsigned int row0 = 0, row1 = 0xFFFFFFFFu;
+	const MetricEntry* pair = nullptr;
+};
+
+// What a refine call does after each chunk's pass in place of the scatter (astc_dev_refine.cuh): decode the candidates to
+// decoded_type with decode_swizzle, measure them in block_metric over the channels of input_components, keep the better.
+struct RefineSpec {
+	int decoded_type = 0;
+	astcenc_swizzle decode_swizzle{};
+	int block_metric = 0;
+	int components = 0;
 };
 
 // What launch_blocks compresses: a block-list table (astc_dev_gather.cuh). Entry j is table[j], lists[j] (no lists: every block
-// of each image) and the block rows of its alpha-scale pre-pass (rows[j]). `words` go up behind the lists: a host list's count
-// word and indices, at which its GatherList (count and indices null here) is pointed.
+// of each image), the block rows of its alpha-scale pre-pass (rows[j]) and, in a refine call, its pair (pairs[j]; no pairs: the
+// staged blocks are scattered). `words` go up behind the lists: a host list's count word and indices, at which its GatherList
+// (count and indices null here) is pointed.
 struct BlockCall {
 	std::vector<GatherImage> table;
 	std::vector<GatherList> lists;
 	std::vector<std::pair<unsigned int, unsigned int>> rows;
+	std::vector<MetricEntry> pairs;
 	std::vector<uint32_t> words;
 	size_t blocks = 0;                 // staging blocks of the whole call
 	int data_type = 0;
+	RefineSpec refine;                 // (refine calls)
 };
 
 // The staging call of checked `entries`: each owns the staging blocks and averages that follow those of the entries before it;
@@ -1750,6 +1765,9 @@ static astcenc_error plan_blocks(const std::vector<BlockEntry>& entries, astcenc
 		if (en.list != nullptr) {
 			call.lists.push_back(*en.list);
 		}
+		if (en.pair != nullptr) {
+			call.pairs.push_back(*en.pair);
+		}
 		call.rows.push_back({en.row0, en.row1 < e.blocks_y ? en.row1 : e.blocks_y});
 		call.blocks += en.blocks;
 		avg_offset += (size_t)e.dim_x * e.dim_y;
@@ -1759,7 +1777,9 @@ static astcenc_error plan_blocks(const std::vector<BlockEntry>& entries, astcenc
 
 // Staging calls (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk (a staging
 // row is one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks
-// blocks). A chunk may span several entries. The whole call is one scratch turn (launch_blocks), like a launch_slab.
+// blocks). A chunk may span several entries. A refine call (astc_dev_refine.cuh) replaces each chunk's scatter by a decode of
+// the staged blocks into a staging decode row, the decisions and the commits. The whole call is one scratch turn
+// (launch_blocks), like a launch_slab.
 static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	const bool volume = bsd.dim_z > 1;
@@ -1767,30 +1787,59 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	const size_t n = call.blocks;
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
 	const size_t avg_floats = call.table.back().avg_offset + (size_t)call.table.back().dim_x * call.table.back().dim_y;
+	const bool refine = !call.pairs.empty();
+	// in the table buffer: the table, its lists, a refine call's pairs and its two decode tables (a full chunk's decode row, the
+	// last chunk's), then the words
 	const size_t table_bytes = call.table.size() * sizeof(GatherImage);
 	const size_t lists_bytes = call.lists.size() * sizeof(GatherList);
-	const size_t list_bytes = table_bytes + lists_bytes + call.words.size() * sizeof(uint32_t);
+	const size_t pairs_bytes = call.pairs.size() * sizeof(MetricEntry);
+	const size_t rows_bytes = refine ? 2 * sizeof(GatherImage) : 0;
+	const size_t words_at = table_bytes + lists_bytes + pairs_bytes + rows_bytes;
+	const size_t list_bytes = words_at + call.words.size() * sizeof(uint32_t);
+	// the refine buffer: the decode row of a chunk, then its values and decisions
+	const size_t row_bytes = (chunk * bsd.texel_count * texel_bytes(call.refine.decoded_type) + 255) & ~(size_t)255;
 	astcenc_error st = ensure_buffer(ctx->list, list_bytes);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * texel_bytes(call.data_type));
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
+	if (st == ASTCENC_SUCCESS && refine) st = ensure_buffer(ctx->refine, row_bytes + chunk * (sizeof(float) + 1));
 	if (st == ASTCENC_SUCCESS && radius != 0) {
 		st = ensure_buffer(ctx->list_alpha, avg_floats * sizeof(float));
 		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
 	if (st == ASTCENC_SUCCESS) {
-		// the table, its lists and the words in one copy, from pageable memory: staged by the driver before the call returns, so
-		// a host list may go when this function does
+		// the table, its lists, the pairs, the decode tables and the words in one copy, from pageable memory: staged by the driver
+		// before the call returns, so a host list may go when this function does
 		std::vector<GatherList> lists = call.lists;
 		for (GatherList& l : lists) {
 			if (l.count == nullptr) {
-				l.count = reinterpret_cast<const uint32_t*>(ctx->list.ptr + table_bytes + lists_bytes);
+				l.count = reinterpret_cast<const uint32_t*>(ctx->list.ptr + words_at);
 				l.indices = l.count + 1;
+			}
+		}
+		// a decode row of m blocks is an image of m x 1 blocks: the staged candidates (list_out) decoded into the refine buffer
+		std::vector<GatherImage> rows;
+		for (size_t m : {chunk, n - (n - 1) / chunk * chunk}) {
+			if (refine) {
+				rows.push_back({ctx->refine.ptr, ctx->list_out.ptr, 0, 0, (unsigned int)(m * bsd.dim_x), bsd.dim_y, volume ? bsd.dim_z : 1u, (unsigned int)m, 1});
 			}
 		}
 		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(call.table.data()), reinterpret_cast<const uint8_t*>(call.table.data()) + table_bytes);
 		up.insert(up.end(), reinterpret_cast<const uint8_t*>(lists.data()), reinterpret_cast<const uint8_t*>(lists.data()) + lists_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.pairs.data()), reinterpret_cast<const uint8_t*>(call.pairs.data()) + pairs_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(rows.data()), reinterpret_cast<const uint8_t*>(rows.data()) + rows_bytes);
 		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.words.data()), reinterpret_cast<const uint8_t*>(call.words.data()) + call.words.size() * sizeof(uint32_t));
 		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+	}
+	// (refine calls) the decide and commit arguments and the decode tables
+	RefineArgs r{};
+	const GatherImage* d_rows = nullptr;
+	if (refine && st == ASTCENC_SUCCESS) {
+		r.pairs = reinterpret_cast<const MetricEntry*>(ctx->list.ptr + table_bytes + lists_bytes);
+		r.row = ctx->refine.ptr;
+		r.values = reinterpret_cast<float*>(ctx->refine.ptr + row_bytes);
+		r.keep = ctx->refine.ptr + row_bytes + chunk * sizeof(float);
+		r.components = call.refine.components;
+		d_rows = reinterpret_cast<const GatherImage*>(ctx->list.ptr + table_bytes + lists_bytes + pairs_bytes);
 	}
 	// The staging pass reads averages gathered from the sources', so it runs no pre-pass of its own: its box filter would reach
 	// across the seams between unrelated blocks. A source's averages cover its window's rows, at their image positions, in the
@@ -1824,7 +1873,20 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 		staged.alpha_avg = radius != 0 ? ctx->alpha.as<float>() : nullptr;
 		staged.alpha_threshold = threshold;
 		st = launch_slab_locked(ctx, staged, 0, 1, ctx->list_out.ptr, stream, nullptr);
-		if (st == ASTCENC_SUCCESS) {
+		if (st == ASTCENC_SUCCESS && refine) {
+			enqueue_decode(ctx, d_rows + (m == chunk ? 0 : 1), 1, m, call.refine.decoded_type, call.refine.decode_swizzle, stream);
+			const unsigned int grid = (m + ASTC_REFINE_LIST_WARPS - 1) / ASTC_REFINE_LIST_WARPS;
+			if (call.refine.block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
+				astc_refine_decide_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+			} else if (call.refine.block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
+				astc_refine_decide_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+			} else {
+				astc_refine_decide_kernel<ASTCENC_B200_BLOCK_SQUARED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+			}
+			astc_refine_commit_kernel<<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(ctx->list_out.ptr, g, r);
+			ctx->launches += 2;
+			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
+		} else if (st == ASTCENC_SUCCESS) {
 			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g);
 			ctx->launches++;
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
@@ -2134,6 +2196,72 @@ astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, con
 	BlockCall call;
 	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
 	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
+}
+
+// Refine calls (astc_dev_refine.cuh): the block-list table of astcenc_b200_compress_device_block_lists, each entry with its pair
+// (original, decode and map). Checked whole before anything is enqueued, in the order include/astcenc.h gives; entries with a
+// capacity of 0 are checked and then left out of the call.
+astcenc_error astcenc_b200_refine_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_refine_list* lists, unsigned int list_count,
+                                                     astcenc_type data_type, const astcenc_swizzle* swizzle, astcenc_type decoded_type,
+                                                     const astcenc_swizzle* decode_swizzle, int input_components, astcenc_b200_block_metric block_metric,
+                                                     void* cuda_stream) {
+	astcenc_error status = check_compress_context(ctx);
+	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
+	if (status == ASTCENC_SUCCESS && !decode_swizzle) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS) status = check_swizzle(*decode_swizzle, ASTCENC_SWZ_Z);
+	if (status == ASTCENC_SUCCESS && (input_components < 1 || input_components > 4)) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS && !check_block_metric(block_metric)) status = ASTCENC_ERR_BAD_PARAM;
+	if (status == ASTCENC_SUCCESS && list_count != 0 && !lists) status = ASTCENC_ERR_BAD_PARAM;
+	// (both types before the entries: the decide kernel reads data and the commit kernel writes decoded one texel per vector
+	// access, so each must be aligned to its texel)
+	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
+	if (status == ASTCENC_SUCCESS) status = check_data_type(decoded_type);
+	auto aligned = [](const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
+	std::vector<astcenc_b200_device_image> descs;
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		const astcenc_b200_device_refine_list& l = lists[i];
+		if (!l.data || !l.payload || (l.capacity != 0 && (!l.indices || !l.count || !l.block_error)) || !aligned(l.indices, 4) || !aligned(l.count, 4) ||
+		    !aligned(l.block_error, 4) || !aligned(l.data, texel_bytes(data_type)) || !aligned(l.decoded, texel_bytes(decoded_type))) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		}
+		descs.push_back({l.data, l.dim_x, l.dim_y, l.dim_z, l.payload});
+	}
+	std::vector<BlockEntry> entries;
+	if (status == ASTCENC_SUCCESS) status = check_image_table(ctx, descs.data(), list_count, data_type, entries);
+	std::vector<GatherList> gather_lists(list_count);
+	std::vector<MetricEntry> pairs(list_count);
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		const astcenc_b200_device_refine_list& l = lists[i];
+		gather_lists[i] = {l.indices, l.count, l.capacity, (unsigned int)entries[i].blocks};
+		MetricEntry& e = pairs[i];
+		memset(&e, 0, sizeof(e));
+		e.img1 = l.data;
+		e.img2 = l.decoded;
+		e.type1 = (int)data_type;
+		e.type2 = (int)decoded_type;
+		e.pitch1 = e.pitch2 = l.dim_x;
+		e.stride1 = e.stride2 = (size_t)l.dim_x * l.dim_y;
+		e.dim_x = l.dim_x;
+		e.dim_y = l.dim_y;
+		e.dim_z = l.dim_z;
+		e.blocks_x = entries[i].image.blocks_x;
+		e.blocks_y = entries[i].image.blocks_y;
+		e.block_error = l.block_error;
+		entries[i].list = &gather_lists[i];
+		entries[i].blocks = l.capacity;
+		entries[i].pair = &pairs[i];
+	}
+	BlockCall call;
+	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	if (status != ASTCENC_SUCCESS) {
+		return status;
+	}
+	call.refine.decoded_type = (int)decoded_type;
+	call.refine.decode_swizzle = *decode_swizzle;
+	call.refine.block_metric = (int)block_metric;
+	call.refine.components = input_components;
+	return launch_blocks(ctx, call, *swizzle, cuda_stream);
 }
 
 // Decode calls over device block lists: the image table of astcenc_b200_decompress_device_images whose entry j owns capacity[j]

@@ -590,6 +590,68 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_metric_device_block
                                                                                       unsigned int list_count, void* cuda_stream);
 
 /**
+ * Re-encode device block lists and keep each new block only where it lowers the block's error: one round of a device refinement
+ * loop (compress, decode, map, astcenc_b200_select_blocks, then this call, repeated) that never makes a block worse under the
+ * caller's own metric. It replaces astcenc_b200_compress_device_block_lists followed by the list decode and the list map, and
+ * needs no decode context of its own: each candidate is decoded by the context that encoded it.
+ * lists[i] describes an image ALREADY RESIDENT in device memory (data: dim_z slices of dim_x * dim_y texels of data_type,
+ * contiguous), its payload (astcenc_compress_image's block order), its decode (the same shape, texels of decoded_type) or NULL,
+ * its per-block map of block_metric (one float per block of the context's footprint) and a device index list with a device count.
+ * - List rule: that of astcenc_b200_compress_device_block_lists. The call reads the first min(*count, capacity) indices; an index
+ *   at or beyond the image's block count is skipped.
+ * - Candidate: for each listed block, the 16 bytes astcenc_b200_compress_device_block_lists would write with this context,
+ *   data_type and swizzle.
+ * - Candidate value v': bit for bit what astcenc_b200_compute_block_metric_device_images writes for that block with
+ *   input_components and block_metric when it compares data against this context's decode of the candidate, the decode
+ *   astcenc_b200_decompress_device_images on this context writes with decoded_type and decode_swizzle.
+ * - Commit rule: the block is committed iff v' < block_error[index] as a float comparison, with the map as it stood before the
+ *   call: ties keep the old block, and a NaN on either side never commits. A committed block gets its 16 payload bytes replaced,
+ *   the texels of its footprint inside the image replaced in decoded (when decoded is not NULL), and block_error[index] = v'.
+ *   Nothing else is written: payload bytes and texels of blocks that are not committed, invalid slots and unlisted blocks keep
+ *   their values. A block listed more than once ends as if listed once (its candidates are the same bytes with the same value).
+ * - Consistency: if payload, decoded and block_error agree on entry (decoded is what this context decodes from payload, and
+ *   block_error is the whole map of data against decoded), they agree after the call. The call does not check that they agree.
+ *   So the decode and map the caller passes in should come from a context with the same profile and the same
+ *   ASTCENC_FLG_USE_DECODE_UNORM8 flag as this one, and the same decoded_type, decode_swizzle, input_components and block_metric.
+ * All entries share data_type, swizzle, decoded_type and decode_swizzle; payloads, decodes and maps must not overlap each other
+ * (not checked). The descriptor array is copied. Enqueued on `cuda_stream` (0 = the context's own stream) without
+ * synchronising, in order with every other pass of the context: *count, the indices and the map are read on the device when the
+ * call runs. No progress callback, no cancellation.
+ * Cost: that of astcenc_b200_compress_device_block_lists over the sum of the capacities, with each chunk's scatter replaced by
+ * three launches (a decode of the chunk's candidates, the decisions, the commits). With a_scale_radius (2D block sizes) each
+ * entry gets an alpha-scale pre-pass over its whole image. Entries with capacity == 0 do nothing; a call whose capacities are all
+ * zero launches nothing.
+ * Errors, in this order; on error nothing is launched and nothing is written:
+ *   1. ASTCENC_ERR_BAD_CONTEXT for a decompress-only context;
+ *   2. ASTCENC_ERR_BAD_PARAM for a NULL swizzle, then ASTCENC_ERR_BAD_SWIZZLE for a swizzle with a selector beyond
+ *      ASTCENC_SWZ_1; then the same two for decode_swizzle, whose selectors may go up to ASTCENC_SWZ_Z;
+ *   3. ASTCENC_ERR_BAD_PARAM for input_components outside 1-4;
+ *   4. ASTCENC_ERR_BAD_PARAM for block_metric outside 0-2;
+ *   5. ASTCENC_ERR_BAD_PARAM for lists == NULL with a non-zero count, then for a bad data_type, then for a bad decoded_type,
+ *      then for an entry with a NULL data or payload, a NULL indices, count or block_error with capacity > 0, indices, count or
+ *      block_error not aligned to 4 bytes, or data or decoded not aligned to its texel (4 / 8 / 16 bytes for U8 / F16 / F32:
+ *      the call reads the original one texel per vector load), then for a zero or overflowing dimension;
+ *   6. ASTCENC_ERR_NOT_IMPLEMENTED for a_scale_radius on a texture array;
+ *   7. ASTCENC_ERR_BAD_PARAM for an image of 2^32 blocks or more, or when the sum of the capacities overflows.
+ * All entries are checked before anything is enqueued.
+ */
+struct astcenc_b200_device_refine_list {
+	const void* data;              /* device: the original, dim_z slices of dim_x * dim_y texels of data_type, contiguous */
+	unsigned int dim_x, dim_y, dim_z;
+	uint8_t* payload;              /* device: the image's whole payload (astcenc_compress_image's block order) */
+	void* decoded;                 /* device: its decode, texels of decoded_type, or NULL */
+	float* block_error;            /* device: its per-block map of block_metric, one float per block */
+	const uint32_t* indices;       /* device: block positions */
+	const uint32_t* count;         /* device: how many are listed */
+	unsigned int capacity;         /* at most this many are read; the call's cost */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_refine_device_block_lists(struct astcenc_context* context, const struct astcenc_b200_device_refine_list* lists,
+                                                                        unsigned int list_count, enum astcenc_type data_type,
+                                                                        const struct astcenc_swizzle* swizzle, enum astcenc_type decoded_type,
+                                                                        const struct astcenc_swizzle* decode_swizzle, int input_components,
+                                                                        enum astcenc_b200_block_metric block_metric, void* cuda_stream);
+
+/**
  * The .astc container (Docs/FileFormat.md; Source/astcenccli_image_load_store.cpp:2573-2760, load_cimage / store_cimage):
  * a 16-byte header - magic 13 AB A1 5C, block dimensions (one byte each), image dimensions (24 bits each, little endian)
  * - followed by the blocks as astcenc_compress_image() wrote them.

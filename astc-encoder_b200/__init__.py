@@ -86,6 +86,16 @@ class BlockSelection(C.Structure):
                 ("count", C.c_void_p)]
 
 
+class BlockPool(C.Structure):
+    """struct astcenc_b200_block_pool (include/astcenc.h)."""
+    _fields_ = [("entry_count", C.c_uint), ("threshold", C.c_float), ("capacity", C.c_uint)]
+
+
+class PooledSelection(C.Structure):
+    """struct astcenc_b200_pooled_selection (include/astcenc.h)."""
+    _fields_ = [("map", C.c_void_p), ("block_count", C.c_uint), ("weight", C.c_void_p), ("indices", C.c_void_p), ("count", C.c_void_p)]
+
+
 class DeviceBlockList(C.Structure):
     """struct astcenc_b200_device_block_list (include/astcenc.h)."""
     _fields_ = [("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("payload", C.c_void_p), ("indices", C.c_void_p),
@@ -187,6 +197,8 @@ def lib():
         l.astcenc_b200_compute_block_metric_device_images.restype = C.c_int
         l.astcenc_b200_select_blocks.argtypes = [C.c_void_p, C.POINTER(BlockSelection), C.c_uint, C.c_void_p]
         l.astcenc_b200_select_blocks.restype = C.c_int
+        l.astcenc_b200_select_blocks_pooled.argtypes = [C.c_void_p, C.POINTER(BlockPool), C.c_uint, C.POINTER(PooledSelection), C.c_uint, C.c_void_p]
+        l.astcenc_b200_select_blocks_pooled.restype = C.c_int
         l.astcenc_b200_compress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
         l.astcenc_b200_compress_device_block_lists.restype = C.c_int
         l.astcenc_b200_decompress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceDecodeBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle),
@@ -530,6 +542,20 @@ class Context:
         err = lib().astcenc_b200_select_blocks(self.handle, table if n else None, n, C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_select_blocks")
+
+    def select_blocks_pooled(self, pools, entries, stream=0):
+        """Block selection under shared budgets (astcenc_b200_select_blocks_pooled). pools: a sequence of (entry_count,
+        threshold, capacity), splitting `entries` into consecutive runs; entries: a sequence of (d_map_ptr, block_count,
+        d_weight_ptr or 0, d_indices_ptr, d_count_ptr). Each pool keeps its min(capacity, candidates) largest products
+        map[b] * *weight above its threshold, ties to the earlier entry, then the lower index; each entry receives its kept
+        indices ascending and their number. Enqueued on `stream`, no sync; works on any context."""
+        np_, n = len(pools), len(entries)
+        ptab = (BlockPool * np_)(*[BlockPool(e, t, c) for e, t, c in pools])
+        etab = (PooledSelection * n)(*[PooledSelection(C.c_void_p(m or None), b, C.c_void_p(w or None), C.c_void_p(i or None), C.c_void_p(k or None))
+                                       for m, b, w, i, k in entries])
+        err = lib().astcenc_b200_select_blocks_pooled(self.handle, ptab if np_ else None, np_, etab if n else None, n, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_select_blocks_pooled")
 
     def compress_device_block_lists(self, lists, data_type, swizzle=(0, 1, 2, 3), stream=0):
         """Recompress device-resident block lists (astcenc_b200_compress_device_block_lists). lists: a sequence of

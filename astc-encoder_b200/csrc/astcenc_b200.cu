@@ -2432,32 +2432,15 @@ astcenc_error astcenc_b200_compute_block_errors_device_block_lists(astcenc_conte
 	return astcenc_b200_compute_block_metric_device_block_lists(ctx, input_components, ASTCENC_B200_BLOCK_SQUARED_ERROR, lists, list_count, cuda_stream);
 }
 
-// Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table goes
-// up, the histograms are cleared and SELECT_KERNELS kernels run, whatever the number of entries.
-astcenc_error astcenc_b200_select_blocks(astcenc_context* ctx, const astcenc_b200_block_selection* entries, unsigned int entry_count, void* cuda_stream) {
-	if (!ctx || (entry_count != 0 && !entries)) {
-		return ASTCENC_ERR_BAD_PARAM;
-	}
-	auto aligned4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; };
-	std::vector<SelectEntry> table(entry_count);
-	for (unsigned int i = 0; i < entry_count; i++) {
-		const astcenc_b200_block_selection& x = entries[i];
-		if (!x.count || (x.block_count != 0 && !x.map) || (x.capacity != 0 && !x.indices) || !aligned4(x.map) || !aligned4(x.indices) ||
-		    !aligned4(x.count) || x.threshold != x.threshold) {
-			return ASTCENC_ERR_BAD_PARAM;
-		}
-		SelectEntry& e = table[i];
-		e.map = x.map;
-		e.indices = x.indices;
-		e.count = x.count;
-		e.threshold = x.threshold;
-		e.capacity = x.capacity;
-		e.block_count = x.block_count;
-	}
-	if (entry_count == 0) {
+// Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table and
+// the pools go up, the pools' histograms are cleared and SELECT_KERNELS kernels run, whatever the number of pools and entries.
+static bool select_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+static astcenc_error enqueue_select(astcenc_context* ctx, std::vector<SelectEntry>& table, std::vector<SelectPool>& pools, void* cuda_stream) {
+	if (table.empty()) {
 		return ASTCENC_SUCCESS;
 	}
-	const size_t tiles = plan_select(table);
+	const size_t tiles = plan_select(table, pools);
 	DeviceGuard guard(ctx->device);
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
@@ -2465,20 +2448,26 @@ astcenc_error astcenc_b200_select_blocks(astcenc_context* ctx, const astcenc_b20
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return scratch_turn(ctx, s, [&]() -> astcenc_error {
 		const size_t table_bytes = table.size() * sizeof(SelectEntry);
-		const size_t hist_bytes = table.size() * 1024 * sizeof(uint32_t);
-		astcenc_error r = ensure_buffer(ctx->select, table_bytes + hist_bytes + tiles * 2 * sizeof(uint32_t));
+		const size_t pool_bytes = pools.size() * sizeof(SelectPool);
+		const size_t hist_bytes = pools.size() * 1024 * sizeof(uint32_t);
+		astcenc_error r = ensure_buffer(ctx->select, table_bytes + pool_bytes + hist_bytes + tiles * 2 * sizeof(uint32_t));
 		if (r != ASTCENC_SUCCESS) {
 			return r;
 		}
-		// (from pageable memory: staged by the driver before the call returns)
-		CUDA_TRY(cudaMemcpyAsync(ctx->select.ptr, table.data(), table_bytes, cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
-		CUDA_TRY(cudaMemsetAsync(ctx->select.ptr + table_bytes, 0, hist_bytes, s), return ASTCENC_ERR_BAD_CONTEXT);
+		// the table and the pools in one copy (from pageable memory: staged by the driver before the call returns)
+		std::vector<uint8_t> up(table_bytes + pool_bytes);
+		memcpy(up.data(), table.data(), table_bytes);
+		memcpy(up.data() + table_bytes, pools.data(), pool_bytes);
+		CUDA_TRY(cudaMemcpyAsync(ctx->select.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaMemsetAsync(ctx->select.ptr + table_bytes + pool_bytes, 0, hist_bytes, s), return ASTCENC_ERR_BAD_CONTEXT);
 		SelectArgs a;
 		a.entries = ctx->select.as<const SelectEntry>();
-		a.count = entry_count;
+		a.pools = reinterpret_cast<const SelectPool*>(ctx->select.ptr + table_bytes);
+		a.count = (unsigned int)table.size();
+		a.pool_count = (unsigned int)pools.size();
 		a.tiles = tiles;
-		a.hist = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes);
-		a.tile_counts = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes + hist_bytes);
+		a.hist = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes + pool_bytes);
+		a.tile_counts = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes + pool_bytes + hist_bytes);
 		// grid-stride launches of SELECT_WARPS warps per CTA, at least one CTA, so that every call makes the same launches
 		const size_t cap = (size_t)ctx->sm_count * 16;
 		auto grid = [cap](size_t warps) {
@@ -2489,12 +2478,75 @@ astcenc_error astcenc_b200_select_blocks(astcenc_context* ctx, const astcenc_b20
 			astc_select_hist_kernel<<<grid(tiles), SELECT_WARPS * 32, 0, s>>>(a, digit);
 		}
 		astc_select_count_kernel<<<grid(tiles), SELECT_WARPS * 32, 0, s>>>(a);
-		astc_select_scan_kernel<<<grid(entry_count), SELECT_WARPS * 32, 0, s>>>(a);
+		astc_select_scan_kernel<<<grid(pools.size()), SELECT_WARPS * 32, 0, s>>>(a);
 		astc_select_write_kernel<<<grid(tiles), SELECT_WARPS * 32, 0, s>>>(a);
 		ctx->launches += SELECT_KERNELS;
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		return ASTCENC_SUCCESS;
 	});
+}
+
+// One entry's device fields (its pool's threshold and capacity), or false for a NULL count, a NULL map with blocks, NULL
+// indices with a capacity or a pointer not aligned to 4 bytes.
+static bool select_entry(const float* map, unsigned int block_count, const float* weight, float threshold, unsigned int capacity, uint32_t* indices,
+                         uint32_t* count, SelectEntry& e) {
+	if (!count || (block_count != 0 && !map) || (capacity != 0 && !indices) || !select_aligned(map) || !select_aligned(weight) ||
+	    !select_aligned(indices) || !select_aligned(count)) {
+		return false;
+	}
+	e.map = map;
+	e.weight = weight;
+	e.indices = indices;
+	e.count = count;
+	e.threshold = threshold;
+	e.capacity = capacity;
+	e.block_count = block_count;
+	return true;
+}
+
+astcenc_error astcenc_b200_select_blocks(astcenc_context* ctx, const astcenc_b200_block_selection* entries, unsigned int entry_count, void* cuda_stream) {
+	if (!ctx || (entry_count != 0 && !entries)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	// one pool per entry, no weights
+	std::vector<SelectEntry> table(entry_count);
+	for (unsigned int i = 0; i < entry_count; i++) {
+		const astcenc_b200_block_selection& x = entries[i];
+		if (!select_entry(x.map, x.block_count, nullptr, x.threshold, x.capacity, x.indices, x.count, table[i]) || x.threshold != x.threshold) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+	}
+	std::vector<SelectPool> pools = select_pools_one_each(entry_count);
+	return enqueue_select(ctx, table, pools, cuda_stream);
+}
+
+astcenc_error astcenc_b200_select_blocks_pooled(astcenc_context* ctx, const astcenc_b200_block_pool* pools, unsigned int pool_count,
+                                                const astcenc_b200_pooled_selection* entries, unsigned int entry_count, void* cuda_stream) {
+	if (!ctx || (pool_count != 0 && !pools) || (entry_count != 0 && !entries)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	std::vector<SelectPool> plan(pool_count);
+	uint64_t total = 0;
+	for (unsigned int p = 0; p < pool_count; p++) {
+		if (pools[p].threshold != pools[p].threshold) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		plan[p].entries = pools[p].entry_count;
+		total += pools[p].entry_count;
+	}
+	if (total != entry_count) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	std::vector<SelectEntry> table(entry_count);
+	for (unsigned int p = 0, j = 0; p < pool_count; p++) {
+		for (unsigned int n = 0; n < pools[p].entry_count; n++, j++) {
+			const astcenc_b200_pooled_selection& x = entries[j];
+			if (!select_entry(x.map, x.block_count, x.weight, pools[p].threshold, pools[p].capacity, x.indices, x.count, table[j])) {
+				return ASTCENC_ERR_BAD_PARAM;
+			}
+		}
+	}
+	return enqueue_select(ctx, table, plan, cuda_stream);
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

@@ -474,6 +474,58 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_select_blocks(struct astcenc_cont
                                                              unsigned int entry_count, void* cuda_stream);
 
 /**
+ * Block selection over a set of maps under one shared budget, such as the worst blocks of a texture set or of a mip chain:
+ * "the K worst blocks of the whole set", in a unit chosen per image by a device-resident weight.
+ * The pools split the entry array into consecutive runs, in order: pools[0] owns the first pools[0].entry_count entries, and so
+ * on. The rule for each pool:
+ * - Product. Block b of entry j has the product p = map[b] * *weight, one float multiply. Without a weight, p = map[b].
+ * - Candidates. A block is a candidate when p > threshold. NaN is never a candidate, and -0.0 counts as 0.0, as in
+ *   astcenc_b200_select_blocks.
+ * - Which blocks are kept. Of the pool's c candidates, the k = min(capacity, c) largest products are kept. Ties go to the lower
+ *   entry position in the pool, then to the lower block index.
+ * - Output. Each entry gets its own kept indices in ascending order and its own *count, which is 0 when none of its blocks are
+ *   kept. Indices past the count are left untouched.
+ * - In numpy terms: concatenate the entries' products in order, set non-candidates to -inf, run
+ *   np.argsort(-pp, kind="stable")[:k], split the result by entry, and sort each part.
+ * - Independence. A pool's outputs depend only on that pool, never on the other pools in the call, their order, or the GPU.
+ * astcenc_b200_select_blocks is this call with one pool per entry and no weights, and writes the same bytes.
+ * The weight is read on the device when the call runs, so a weight derived from device figures (for example
+ * 1 / sum_squared_error from an astcenc_b200_error_metrics record) needs no host round trip. As first-order statements, not
+ * promises, with each map an image's per-block error (astcenc_b200_compute_block_metric_device_images) and a -INFINITY
+ * threshold, a block ranks by its share of:
+ * - NULL weights: the pool's total map sum;
+ * - 1 / texels_j (texels of image j): the mean over the images of the per-texel error;
+ * - 1 / E_j, E_j being image j's map total: the mean PSNR over the images (a block of error e holds image j's PSNR down by
+ *   about (10 / ln 10) * e / E_j dB).
+ * Stream, scratch and tables are those of astcenc_b200_select_blocks: enqueued on `cuda_stream` (0 = the context's own stream)
+ * without synchronising, on any context, decompress-only ones included. The descriptor arrays are copied. The call costs one
+ * memset and 7 kernel launches, whatever the number of pools and entries, reading each map six times; entry_count == 0 launches
+ * nothing. Outputs must not overlap any map, weight or each other (not checked).
+ * Errors, in this order; on error nothing is launched and nothing is written:
+ *   1. ASTCENC_ERR_BAD_PARAM for a NULL context, pools == NULL with pool_count > 0, or entries == NULL with entry_count > 0;
+ *   2. ASTCENC_ERR_BAD_PARAM for a pool with a NaN threshold, or when the pools' entry_counts, summed without overflow, differ
+ *      from entry_count;
+ *   3. ASTCENC_ERR_BAD_PARAM for an entry with a NULL count, a NULL map with block_count > 0, NULL indices when its pool's
+ *      capacity is > 0, or a map, weight, indices or count not aligned to 4 bytes.
+ * All entries are checked before anything is enqueued.
+ */
+struct astcenc_b200_block_pool {
+	unsigned int entry_count;      /* the next entry_count entries of the call share this pool */
+	float threshold;               /* candidates are the products above it */
+	unsigned int capacity;         /* at most this many blocks are kept, over all the pool's entries */
+};
+struct astcenc_b200_pooled_selection {
+	const float* map;              /* device: block_count values, e.g. a per-block error map */
+	unsigned int block_count;
+	const float* weight;           /* device: one float, read when the call runs; NULL = no weight */
+	uint32_t* indices;             /* device: room for min(pool capacity, block_count) indices */
+	uint32_t* count;               /* device: receives how many of this entry's blocks were kept */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_select_blocks_pooled(struct astcenc_context* context, const struct astcenc_b200_block_pool* pools,
+                                                                    unsigned int pool_count, const struct astcenc_b200_pooled_selection* entries,
+                                                                    unsigned int entry_count, void* cuda_stream);
+
+/**
  * Recompress block lists that live in device memory, such as the output of astcenc_b200_select_blocks or a GPU tool's list of
  * dirty tiles, for many device-resident images in shared pipeline passes.
  * lists[i] describes an image ALREADY RESIDENT in device memory (data: dim_z slices of dim_x * dim_y texels, contiguous; the

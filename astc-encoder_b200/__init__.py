@@ -30,6 +30,8 @@ ERROR_NAMES = ["ASTCENC_SUCCESS", "ASTCENC_ERR_OUT_OF_MEM", "ASTCENC_ERR_BAD_CPU
 ERR_OUT_OF_MEM, ERR_BAD_PARAM, ERR_BAD_BLOCK_SIZE, ERR_BAD_SWIZZLE, ERR_BAD_CONTEXT, ERR_NOT_IMPLEMENTED = 1, 3, 4, 7, 9, 10
 # enum astcenc_b200_block_metric: what a per-block error map measures
 BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR, BLOCK_LOG2_ERROR = 0, 1, 2
+# enum astcenc_b200_weight_rule: the selection weight of an image that misses its target
+WEIGHT_ONE, WEIGHT_INVERSE_TOTAL = 0, 1
 
 
 class AstcencError(RuntimeError):
@@ -94,6 +96,11 @@ class BlockPool(C.Structure):
 class PooledSelection(C.Structure):
     """struct astcenc_b200_pooled_selection (include/astcenc.h)."""
     _fields_ = [("map", C.c_void_p), ("block_count", C.c_uint), ("weight", C.c_void_p), ("indices", C.c_void_p), ("count", C.c_void_p)]
+
+
+class BlockMapTotal(C.Structure):
+    """struct astcenc_b200_block_map_total (include/astcenc.h)."""
+    _fields_ = [("map", C.c_void_p), ("block_count", C.c_uint), ("limit", C.c_double), ("total", C.c_void_p), ("weight", C.c_void_p)]
 
 
 class DeviceBlockList(C.Structure):
@@ -199,6 +206,8 @@ def lib():
         l.astcenc_b200_select_blocks.restype = C.c_int
         l.astcenc_b200_select_blocks_pooled.argtypes = [C.c_void_p, C.POINTER(BlockPool), C.c_uint, C.POINTER(PooledSelection), C.c_uint, C.c_void_p]
         l.astcenc_b200_select_blocks_pooled.restype = C.c_int
+        l.astcenc_b200_total_block_maps.argtypes = [C.c_void_p, C.POINTER(BlockMapTotal), C.c_uint, C.c_int, C.c_void_p]
+        l.astcenc_b200_total_block_maps.restype = C.c_int
         l.astcenc_b200_compress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_void_p]
         l.astcenc_b200_compress_device_block_lists.restype = C.c_int
         l.astcenc_b200_decompress_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceDecodeBlockList), C.c_uint, C.c_int, C.POINTER(Swizzle),
@@ -556,6 +565,18 @@ class Context:
         err = lib().astcenc_b200_select_blocks_pooled(self.handle, ptab if np_ else None, np_, etab if n else None, n, C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_select_blocks_pooled")
+
+    def total_block_maps(self, entries, rule, stream=0):
+        """Map totals and gated selection weights (astcenc_b200_total_block_maps). entries: a sequence of (d_map_ptr, block_count,
+        limit, d_total_ptr or 0, d_weight_ptr or 0); each total pointer receives the map's double total, in a fixed order set by
+        block_count alone, and each weight pointer 0 unless total > limit and total > 0, else 1 (WEIGHT_ONE) or 1 / total
+        (WEIGHT_INVERSE_TOTAL) as a float. Enqueued on `stream`, no sync; works on any context."""
+        n = len(entries)
+        table = (BlockMapTotal * n)(*[BlockMapTotal(C.c_void_p(m or None), b, lim, C.c_void_p(t or None), C.c_void_p(w or None))
+                                      for m, b, lim, t, w in entries])
+        err = lib().astcenc_b200_total_block_maps(self.handle, table if n else None, n, rule, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_total_block_maps")
 
     def compress_device_block_lists(self, lists, data_type, swizzle=(0, 1, 2, 3), stream=0):
         """Recompress device-resident block lists (astcenc_b200_compress_device_block_lists). lists: a sequence of

@@ -25,6 +25,7 @@
 #include "astc_dev_metrics.cuh"
 #include "astc_dev_refine.cuh"
 #include "astc_dev_select.cuh"
+#include "astc_dev_totals.cuh"
 #include "astc_host_pack.h"
 #include "astc_host_config.h"
 #include "astc_host_slab.h"
@@ -425,7 +426,7 @@ struct astcenc_context {
 	DevBuffer refine;
 	// metrics calls: the partial sums of every virtual CTA and the sums of every pair, grown on demand
 	DevBuffer metric_partials;
-	// selection calls: the entries, their histograms and the tile counts
+	// selection calls: the entries, their histograms and the tile counts; totals calls: the entries and their partials
 	DevBuffer select;
 	// The per-context scratch (records, queues, counters, alpha averages, table and staging buffers) serves ONE pass at a time
 	// (scratch_turn): launch_mtx serialises the host side, scratch_done orders a pass on one stream behind the previous pass on
@@ -2547,6 +2548,60 @@ astcenc_error astcenc_b200_select_blocks_pooled(astcenc_context* ctx, const astc
 		}
 	}
 	return enqueue_select(ctx, table, plan, cuda_stream);
+}
+
+// Totals calls (astc_dev_totals.cuh): every entry is checked before anything is enqueued; in one scratch turn the table goes up
+// and TOTAL_KERNELS kernels run, whatever the number of entries.
+astcenc_error astcenc_b200_total_block_maps(astcenc_context* ctx, const astcenc_b200_block_map_total* entries, unsigned int entry_count,
+                                            astcenc_b200_weight_rule rule, void* cuda_stream) {
+	if (!ctx || (entry_count != 0 && !entries)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if ((int)rule != ASTCENC_B200_WEIGHT_ONE && (int)rule != ASTCENC_B200_WEIGHT_INVERSE_TOTAL) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	std::vector<TotalEntry> table(entry_count);
+	for (unsigned int j = 0; j < entry_count; j++) {
+		const astcenc_b200_block_map_total& x = entries[j];
+		if ((x.block_count != 0 && !x.map) || x.limit != x.limit || !select_aligned(x.map) || !select_aligned(x.weight) ||
+		    (reinterpret_cast<uintptr_t>(x.total) & 7) != 0) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		table[j] = {x.map, x.total, x.weight, x.limit, x.block_count, 0, 0};
+	}
+	size_t ctas = 0;
+	if (!plan_map_totals(table, ctas)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	if (table.empty()) {
+		return ASTCENC_SUCCESS;
+	}
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+	return scratch_turn(ctx, s, [&]() -> astcenc_error {
+		const size_t table_bytes = table.size() * sizeof(TotalEntry);      // (a multiple of 8: the partials follow)
+		astcenc_error r = ensure_buffer(ctx->select, table_bytes + ctas * sizeof(double));
+		if (r != ASTCENC_SUCCESS) {
+			return r;
+		}
+		// (from pageable memory: staged by the driver before the call returns)
+		CUDA_TRY(cudaMemcpyAsync(ctx->select.ptr, table.data(), table_bytes, cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+		TotalArgs a;
+		a.entries = ctx->select.as<const TotalEntry>();
+		a.count = (unsigned int)table.size();
+		a.rule = (int)rule;
+		a.ctas = ctas;
+		a.partials = reinterpret_cast<double*>(ctx->select.ptr + table_bytes);
+		const size_t grid = (ctas + TOTAL_WARPS - 1) / TOTAL_WARPS;      // (at least one CTA, so that every call makes the same launches)
+		astc_map_total_partial_kernel<<<(unsigned int)(grid == 0 ? 1 : grid), TOTAL_WARPS * 32, 0, s>>>(a);
+		astc_map_total_finish_kernel<<<(unsigned int)((table.size() + TOTAL_FINISH_THREADS - 1) / TOTAL_FINISH_THREADS), TOTAL_FINISH_THREADS, 0, s>>>(a);
+		ctx->launches += TOTAL_KERNELS;
+		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+		return ASTCENC_SUCCESS;
+	});
 }
 
 astcenc_error astcenc_b200_stage_timing(astcenc_context* ctx, int enable, float stage_ms[4], unsigned int stage_launches[4]) {

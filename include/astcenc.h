@@ -704,6 +704,57 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_refine_device_block_lists(struct 
                                                                         enum astcenc_b200_block_metric block_metric, void* cuda_stream);
 
 /**
+ * Totals of device-resident per-block maps, and from each total a selection weight that is zero once the image meets a target:
+ * the device side of a per-image quality target ("every texture at 40 dB or better") in the refinement loop.
+ * - Total. The sum of the entry's block_count map values, accumulated in double in a fixed order that depends only on
+ *   block_count: never on the GPU, on the other entries of the call or on their order. NaN values propagate into the total;
+ *   block_count == 0 gives 0.
+ * - Weight. 0 unless total > limit and total > 0 (so a NaN total gives 0); otherwise 1.0f under ASTCENC_B200_WEIGHT_ONE and
+ *   (float)(1.0 / total) under ASTCENC_B200_WEIGHT_INVERSE_TOTAL (0 for an infinite total). A weight of 0 in
+ *   astcenc_b200_select_blocks_pooled with a pool threshold of 0 makes none of the image's blocks a candidate (the product is 0,
+ *   or NaN where the map holds inf): that is how an image that meets its target leaves the pool.
+ * - Targets. With each map a whole per-block map of astcenc_b200_compute_block_metric_device_images (and the identities stated
+ *   above enum astcenc_b200_block_metric), the image meets a target when total <= limit with:
+ *     SQUARED_ERROR, PSNR of at least P dB:               limit = samples * 10^(-P / 10);
+ *     ALPHA_WEIGHTED_ERROR, alpha_psnr of at least P dB:  limit = samples * 10^(-P / 10), input_components == 4;
+ *     LOG2_ERROR, log_rmse of at most R:                  limit = R^2 * pixels;
+ *   samples being pixels times the number of channels input_components selects. A total agrees with the figure's error sum up
+ *   to the per-block float rounding of the map, so a target met within that rounding may be judged either way. limit
+ *   = -INFINITY never meets the target.
+ * - The closed loop. Compress, decode and map the set once; then enqueue every round up front, each one this call (then the
+ *   weights are current), astcenc_b200_select_blocks_pooled with these weights, a threshold of 0 and the round's budget, and
+ *   astcenc_b200_refine_device_block_lists, which keeps the maps current. Images that reach their target get no blocks in later
+ *   rounds and the budget goes to those that still miss theirs, with no host synchronisation between rounds.
+ *   ASTCENC_B200_WEIGHT_INVERSE_TOTAL gives the weights 1 / E_j (rule (d) of the pooled selection: a block ranks by its share
+ *   of its image's error) with the same gate.
+ * Enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in order with every other pass of the
+ * context; works on any context, decompress-only ones included. The descriptor array is copied. The call is one table copy and
+ * two kernel launches, whatever the number of entries; entry_count == 0 launches nothing. Outputs must not overlap any map or
+ * each other (not checked).
+ * Errors, in this order; on error nothing is launched and nothing is written:
+ *   1. ASTCENC_ERR_BAD_PARAM for a NULL context or entries == NULL with entry_count > 0;
+ *   2. ASTCENC_ERR_BAD_PARAM for a rule outside 0-1;
+ *   3. ASTCENC_ERR_BAD_PARAM for an entry with a NULL map and block_count > 0, a NaN limit, a map or weight not aligned to 4
+ *      bytes, or a total not aligned to 8;
+ *   4. ASTCENC_ERR_BAD_PARAM when the call does not fit a launch (more than 2^31 - 1 virtual CTAs: a few million entries of
+ *      large maps).
+ * All entries are checked before anything is enqueued.
+ */
+enum astcenc_b200_weight_rule {
+	ASTCENC_B200_WEIGHT_ONE = 0,            /* weight 1 while the image misses its target */
+	ASTCENC_B200_WEIGHT_INVERSE_TOTAL = 1   /* weight 1 / total while the image misses its target (rule (d)) */
+};
+struct astcenc_b200_block_map_total {
+	const float* map;              /* device: block_count values, e.g. a map of astcenc_b200_compute_block_metric_device_images */
+	unsigned int block_count;
+	double limit;                  /* the image meets its target when total <= limit; -INFINITY: never */
+	double* total;                 /* device, or NULL: receives the map's total */
+	float* weight;                 /* device, or NULL: receives the selection weight */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_total_block_maps(struct astcenc_context* context, const struct astcenc_b200_block_map_total* entries,
+                                                                unsigned int entry_count, enum astcenc_b200_weight_rule rule, void* cuda_stream);
+
+/**
  * The .astc container (Docs/FileFormat.md; Source/astcenccli_image_load_store.cpp:2573-2760, load_cimage / store_cimage):
  * a 16-byte header - magic 13 AB A1 5C, block dimensions (one byte each), image dimensions (24 bits each, little endian)
  * - followed by the blocks as astcenc_compress_image() wrote them.

@@ -221,6 +221,12 @@ def lib():
         l.astcenc_b200_refine_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceRefineList), C.c_uint, C.c_int, C.POINTER(Swizzle), C.c_int,
                                                              C.POINTER(Swizzle), C.c_int, C.c_int, C.c_void_p]
         l.astcenc_b200_refine_device_block_lists.restype = C.c_int
+        l.astcenc_b200_compress_device_block_lists_packed.argtypes = [C.c_void_p, C.POINTER(DeviceBlockList), C.c_uint, C.c_uint, C.c_void_p, C.c_int,
+                                                                      C.POINTER(Swizzle), C.c_void_p]
+        l.astcenc_b200_compress_device_block_lists_packed.restype = C.c_int
+        l.astcenc_b200_refine_device_block_lists_packed.argtypes = [C.c_void_p, C.POINTER(DeviceRefineList), C.c_uint, C.c_uint, C.c_void_p, C.c_int,
+                                                                    C.POINTER(Swizzle), C.c_int, C.POINTER(Swizzle), C.c_int, C.c_int, C.c_void_p]
+        l.astcenc_b200_refine_device_block_lists_packed.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -590,6 +596,20 @@ class Context:
         if err:
             raise AstcencError(err, "astcenc_b200_compress_device_block_lists")
 
+    def compress_device_block_lists_packed(self, lists, budget, data_type, swizzle=(0, 1, 2, 3), overflow=0, stream=0):
+        """compress_device_block_lists at a cost set by `budget` (astcenc_b200_compress_device_block_lists_packed): the listed
+        slots v_j = min(*count_j, capacity_j) of the same tuples take consecutive packed positions in entry order, and only those
+        below `budget` are processed; `overflow` (a device uint32 pointer, or 0) receives max(sum of v_j - budget, 0). Stages
+        min(budget, sum of capacities) slots. Enqueued on `stream`, no sync."""
+        n = len(lists)
+        table = (DeviceBlockList * n)(*[DeviceBlockList(C.c_void_p(p), x, y, z, C.c_void_p(q), C.c_void_p(i or None), C.c_void_p(k or None), c)
+                                        for p, x, y, z, q, i, k, c in lists])
+        sw = Swizzle(*swizzle)
+        err = lib().astcenc_b200_compress_device_block_lists_packed(self.handle, table if n else None, n, budget, C.c_void_p(overflow or None), data_type,
+                                                                    C.byref(sw), C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_compress_device_block_lists_packed")
+
     def decompress_device_block_lists(self, lists, data_type, swizzle=(0, 1, 2, 3), stream=0):
         """Decode device-resident block lists into device images (astcenc_b200_decompress_device_block_lists). lists: a sequence of
         (d_payload_ptr, d_image_ptr, dim_x, dim_y, dim_z, d_indices_ptr, d_count_ptr, capacity); for the first min(*count, capacity)
@@ -644,6 +664,22 @@ class Context:
                                                            input_components, block_metric, C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_refine_device_block_lists")
+
+    def refine_device_block_lists_packed(self, lists, budget, data_type, decoded_type, block_metric, swizzle=(0, 1, 2, 3), decode_swizzle=(0, 1, 2, 3),
+                                         input_components=4, overflow=0, stream=0):
+        """refine_device_block_lists at a cost set by `budget` (astcenc_b200_refine_device_block_lists_packed): the same tuples,
+        packed and truncated as in compress_device_block_lists_packed; `overflow` (a device uint32 pointer, or 0) receives
+        max(sum of v_j - budget, 0). Enqueued on `stream`, no sync."""
+        n = len(lists)
+        table = (DeviceRefineList * n)(*[DeviceRefineList(C.c_void_p(p), x, y, z, C.c_void_p(q), C.c_void_p(d or None), C.c_void_p(b or None),
+                                                          C.c_void_p(i or None), C.c_void_p(k or None), c)
+                                         for p, x, y, z, q, d, b, i, k, c in lists])
+        sw = Swizzle(*swizzle)
+        dsw = Swizzle(*decode_swizzle)
+        err = lib().astcenc_b200_refine_device_block_lists_packed(self.handle, table if n else None, n, budget, C.c_void_p(overflow or None), data_type,
+                                                                  C.byref(sw), decoded_type, C.byref(dsw), input_components, block_metric, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_refine_device_block_lists_packed")
 
     def last_timing(self):
         ms = C.c_float(); a = C.c_size_t(); b = C.c_size_t()

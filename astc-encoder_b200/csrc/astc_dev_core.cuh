@@ -50,7 +50,9 @@
 	#define ASTC_U2F(u) astc_u2f(u)
 	#define ASTC_CLZ(v) __builtin_clz(v)
 	#define ASTC_POPCLL(v) __builtin_popcountll(v)
-	#define ASTC_LDG(p) (*(p))
+	#if !defined(ASTC_LDG)      /* (a host simulation may define its own: tests/hostsim/hostsim_pack_lists.cpp checks every read) */
+		#define ASTC_LDG(p) (*(p))
+	#endif
 	static const DevConstTables* g_astc_ct;
 	#define ASTC_CT g_astc_ct
 	static uint8_t* astc_smem;           // stands in for the CTA's shared window

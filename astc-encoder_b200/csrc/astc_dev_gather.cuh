@@ -17,6 +17,13 @@
 // (GatherArgs::base) may span several entries, and an entry several chunks. A host list of n blocks of one image is a one-entry
 // table whose list has capacity n and *count n.
 //
+// A packed call (astcenc_b200_compress_device_block_lists_packed, refine_device_block_lists_packed; astc_dev_pack.cuh) gives
+// entry j the listed slots v_j = min(*count, capacity) alone: first[j] = v_0 + ... + v_(j-1), written on the device when the
+// call runs, and the packed total T = min(sum of v, budget) sits in the `first` of a sentinel GatherImage after the table
+// (images[image_count]). Staging block c < T is slot c - first[j] < v_j of the entry j that find_image returns (entries with
+// v_j = 0 share the next entry's first); a staging block at or beyond T is invalid and reads no list. The packed resolution is
+// the PACKED instantiation of staged_block and its users; the unpacked instantiations never read the sentinel.
+//
 // A decode call (astcenc_b200_decompress_device_images) walks the same kind of table without lists: each entry's payload is
 // read and its data written. A list decode (astcenc_b200_decompress_device_block_lists) walks it with lists, slot by slot.
 #pragma once
@@ -117,7 +124,13 @@ ASTC_FN unsigned int find_image(const E* images, unsigned int image_count, size_
 }
 
 // Staging block i: the entry that holds it (j) and its block in the entry's image, or GATHER_INVALID for an invalid list slot.
+// PACKED: a packed table; a staging block at or beyond the packed total is invalid (j = 0) before any list is read.
+template <bool PACKED = false>
 ASTC_FN uint32_t staged_block(const GatherArgs& g, unsigned int i, unsigned int& j) {
+	if (PACKED && g.base + i >= g.images[g.image_count].first) {
+		j = 0;
+		return GATHER_INVALID;
+	}
 	j = find_image(g.images, g.image_count, g.base + i);
 	const size_t s = g.base + i - g.images[j].first;
 	return g.lists != nullptr ? list_slot(g.lists[j], s) : (uint32_t)s;      // (an image has fewer than 2^32 blocks)
@@ -126,9 +139,10 @@ ASTC_FN uint32_t staged_block(const GatherArgs& g, unsigned int i, unsigned int&
 // Staging block i, by the lanes of one warp (lane / lanes): the texels word by word, so that consecutive lanes read consecutive
 // words of a footprint row; then the alpha averages (0 for texels outside the image). An invalid slot stages zeros: a constant
 // block, emitted in wave 0 and never scattered. The host simulation calls it with 0 / 1 or on its 32 simulated lanes.
+template <bool PACKED = false>
 ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lanes) {
 	unsigned int j;
-	const uint32_t index = staged_block(g, i, j);
+	const uint32_t index = staged_block<PACKED>(g, i, j);
 	const bool valid = index != GATHER_INVALID;
 	const GatherImage im = g.images[j];      // (a copy: the stores below cannot alias it, so its fields stay in registers)
 	const unsigned int T = g.bx * g.by * g.bz;
@@ -149,9 +163,10 @@ ASTC_FN void gather_block(const GatherArgs& g, unsigned int i, int lane, int lan
 }
 
 // Where staging block i goes in its image's payload; null for an invalid list slot.
+template <bool PACKED = false>
 ASTC_FN uint8_t* scatter_target(const GatherArgs& g, unsigned int i) {
 	unsigned int j;
-	const uint32_t index = staged_block(g, i, j);
+	const uint32_t index = staged_block<PACKED>(g, i, j);
 	return index == GATHER_INVALID ? nullptr : g.images[j].payload + (size_t)index * 16;
 }
 

@@ -28,10 +28,11 @@ struct RefineArgs {
 };
 
 // Staging block i of the chunk, by `lanes` lanes of one warp: its candidate value and decision (0 for an invalid list slot).
-template <int M>
+// PACKED: a packed table (astc_dev_gather.cuh).
+template <int M, bool PACKED = false>
 ASTC_FN void refine_decide_block(const GatherArgs& g, const RefineArgs& r, unsigned int i, int lane, int lanes) {
 	unsigned int j;
-	const uint32_t index = staged_block(g, i, j);
+	const uint32_t index = staged_block<PACKED>(g, i, j);
 	if (index == GATHER_INVALID) {
 		if (lane == 0) {
 			r.keep[i] = 0;
@@ -53,12 +54,13 @@ ASTC_FN void refine_decide_block(const GatherArgs& g, const RefineArgs& r, unsig
 
 // Staging block i of the chunk, by `lanes` lanes of one warp, when it was kept: its staged bytes (staged + 16 i) into the payload,
 // the texels of its footprint inside the image from the row into the decode (when the pair has one) and its value into the map.
+template <bool PACKED = false>
 ASTC_FN void refine_commit_block(const GatherArgs& g, const RefineArgs& r, const uint8_t* staged, unsigned int i, int lane, int lanes) {
 	if (ASTC_LDG(r.keep + i) == 0) {
 		return;      // (the whole warp)
 	}
 	unsigned int j;
-	const uint32_t index = staged_block(g, i, j);      // (a kept block is a valid slot)
+	const uint32_t index = staged_block<PACKED>(g, i, j);      // (a kept block is a valid slot)
 	const MetricEntry& e = r.pairs[j];
 	const GatherImage& im = g.images[j];
 	if (lane == 0) {
@@ -105,6 +107,24 @@ astc_refine_commit_kernel(const uint8_t* __restrict__ staged, const __grid_const
 	const unsigned int i = blockIdx.x * ASTC_REFINE_LIST_WARPS + (threadIdx.x >> 5);
 	if (i < g.n) {
 		refine_commit_block(g, r, staged, i, threadIdx.x & 31, ASTC_WARP);
+	}
+}
+
+// The same two kernels over a packed table (astc_dev_gather.cuh).
+template <int M>
+__global__ void __launch_bounds__(ASTC_REFINE_LIST_WARPS * 32)
+astc_refine_decide_packed_kernel(const __grid_constant__ GatherArgs g, const __grid_constant__ RefineArgs r) {
+	const unsigned int i = blockIdx.x * ASTC_REFINE_LIST_WARPS + (threadIdx.x >> 5);
+	if (i < g.n) {
+		refine_decide_block<M, true>(g, r, i, threadIdx.x & 31, ASTC_WARP);
+	}
+}
+
+__global__ void __launch_bounds__(ASTC_REFINE_LIST_WARPS * 32)
+astc_refine_commit_packed_kernel(const uint8_t* __restrict__ staged, const __grid_constant__ GatherArgs g, const __grid_constant__ RefineArgs r) {
+	const unsigned int i = blockIdx.x * ASTC_REFINE_LIST_WARPS + (threadIdx.x >> 5);
+	if (i < g.n) {
+		refine_commit_block<true>(g, r, staged, i, threadIdx.x & 31, ASTC_WARP);
 	}
 }
 #endif

@@ -24,6 +24,7 @@
 #include "astc_dev_gather.cuh"
 #include "astc_dev_metrics.cuh"
 #include "astc_dev_refine.cuh"
+#include "astc_dev_pack.cuh"
 #include "astc_dev_select.cuh"
 #include "astc_dev_totals.cuh"
 #include "astc_host_pack.h"
@@ -230,6 +231,29 @@ astc_scatter_blocks_kernel(const uint8_t* __restrict__ staged, const __grid_cons
 	uint8_t* dst = scatter_target(g, i);
 	if (dst == nullptr) {
 		return;      // (an invalid list slot)
+	}
+	store_block(dst, v);
+}
+
+// The same two kernels over a packed table (astc_dev_gather.cuh, astc_dev_pack.cuh).
+__global__ void __launch_bounds__(ASTC_GATHER_THREADS)
+astc_gather_blocks_packed_kernel(const __grid_constant__ GatherArgs g) {
+	const unsigned int warps = blockDim.x >> 5;
+	for (unsigned int i = blockIdx.x * warps + (threadIdx.x >> 5); i < g.n; i += gridDim.x * warps) {
+		gather_block<true>(g, i, (int)(threadIdx.x & 31), 32);
+	}
+}
+
+__global__ void __launch_bounds__(ASTC_GATHER_THREADS)
+astc_scatter_blocks_packed_kernel(const uint8_t* __restrict__ staged, const __grid_constant__ GatherArgs g) {
+	unsigned int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= g.n) {
+		return;
+	}
+	const uint4 v = __ldg(reinterpret_cast<const uint4*>(staged) + i);
+	uint8_t* dst = scatter_target<true>(g, i);
+	if (dst == nullptr) {
+		return;      // (an invalid slot)
 	}
 	store_block(dst, v);
 }
@@ -1735,16 +1759,20 @@ struct RefineSpec {
 // What launch_blocks compresses: a block-list table (astc_dev_gather.cuh). Entry j is table[j], lists[j] (no lists: every block
 // of each image), the block rows of its alpha-scale pre-pass (rows[j]) and, in a refine call, its pair (pairs[j]; no pairs: the
 // staged blocks are scattered). `words` go up behind the lists: a host list's count word and indices, at which its GatherList
-// (count and indices null here) is pointed.
+// (count and indices null here) is pointed. A packed call (astc_dev_pack.cuh) stages min(budget, blocks) slots, and its table's
+// firsts are rewritten on the device before the first gather.
 struct BlockCall {
 	std::vector<GatherImage> table;
 	std::vector<GatherList> lists;
 	std::vector<std::pair<unsigned int, unsigned int>> rows;
 	std::vector<MetricEntry> pairs;
 	std::vector<uint32_t> words;
-	size_t blocks = 0;                 // staging blocks of the whole call
+	size_t blocks = 0;                 // staging blocks of the whole call (a packed call: the sum of the capacities)
 	int data_type = 0;
 	RefineSpec refine;                 // (refine calls)
+	bool packed = false;               // (packed calls) the budget and the device word that receives the overflow, or null
+	unsigned int budget = 0;
+	uint32_t* overflow = nullptr;
 };
 
 // The staging call of checked `entries`: each owns the staging blocks and averages that follow those of the entries before it;
@@ -1779,22 +1807,23 @@ static astcenc_error plan_blocks(const std::vector<BlockEntry>& entries, astcenc
 // Staging calls (astc_dev_gather.cuh): gather -> one ordinary pass over the staging row -> scatter, chunk by chunk (a staging
 // row is one block row, which the batching of launch_slab_locked cannot split: a chunk holds at most knobs.batch_blocks
 // blocks). A chunk may span several entries. A refine call (astc_dev_refine.cuh) replaces each chunk's scatter by a decode of
-// the staged blocks into a staging decode row, the decisions and the commits. The whole call is one scratch turn
-// (launch_blocks), like a launch_slab.
+// the staged blocks into a staging decode row, the decisions and the commits. A packed call packs its table right after the
+// upload (astc_dev_pack.cuh) and runs the packed instantiations of the gather, scatter, decide and commit kernels; with a budget
+// of 0 the packing is all it does. The whole call is one scratch turn (launch_blocks), like a launch_slab.
 static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, cudaStream_t stream) {
 	const DevBsd& bsd = ctx->tables->bsd;
 	const bool volume = bsd.dim_z > 1;
 	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
-	const size_t n = call.blocks;
+	const size_t n = call.packed && call.budget < call.blocks ? call.budget : call.blocks;
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
 	const size_t avg_floats = call.table.back().avg_offset + (size_t)call.table.back().dim_x * call.table.back().dim_y;
 	const bool refine = !call.pairs.empty();
-	// in the table buffer: the table, its lists, a refine call's pairs and its two decode tables (a full chunk's decode row, the
-	// last chunk's), then the words
-	const size_t table_bytes = call.table.size() * sizeof(GatherImage);
+	// in the table buffer: the table (a packed call: and its sentinel), its lists, a refine call's pairs and its two decode tables
+	// (a full chunk's decode row, the last chunk's), then the words
+	const size_t table_bytes = (call.table.size() + (call.packed ? 1 : 0)) * sizeof(GatherImage);
 	const size_t lists_bytes = call.lists.size() * sizeof(GatherList);
 	const size_t pairs_bytes = call.pairs.size() * sizeof(MetricEntry);
-	const size_t rows_bytes = refine ? 2 * sizeof(GatherImage) : 0;
+	const size_t rows_bytes = refine && n != 0 ? 2 * sizeof(GatherImage) : 0;
 	const size_t words_at = table_bytes + lists_bytes + pairs_bytes + rows_bytes;
 	const size_t list_bytes = words_at + call.words.size() * sizeof(uint32_t);
 	// the refine buffer: the decode row of a chunk, then its values and decisions
@@ -1803,7 +1832,7 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * texel_bytes(call.data_type));
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
 	if (st == ASTCENC_SUCCESS && refine) st = ensure_buffer(ctx->refine, row_bytes + chunk * (sizeof(float) + 1));
-	if (st == ASTCENC_SUCCESS && radius != 0) {
+	if (st == ASTCENC_SUCCESS && radius != 0 && n != 0) {
 		st = ensure_buffer(ctx->list_alpha, avg_floats * sizeof(float));
 		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
@@ -1819,17 +1848,27 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 		}
 		// a decode row of m blocks is an image of m x 1 blocks: the staged candidates (list_out) decoded into the refine buffer
 		std::vector<GatherImage> rows;
-		for (size_t m : {chunk, n - (n - 1) / chunk * chunk}) {
-			if (refine) {
+		for (size_t m : {chunk, n - (n - 1) / (chunk != 0 ? chunk : 1) * chunk}) {
+			if (rows_bytes != 0) {
 				rows.push_back({ctx->refine.ptr, ctx->list_out.ptr, 0, 0, (unsigned int)(m * bsd.dim_x), bsd.dim_y, volume ? bsd.dim_z : 1u, (unsigned int)m, 1});
 			}
 		}
-		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(call.table.data()), reinterpret_cast<const uint8_t*>(call.table.data()) + table_bytes);
+		std::vector<GatherImage> table = call.table;
+		if (call.packed) {
+			table.push_back(GatherImage{});      // (the sentinel: astc_pack_lists_kernel writes the packed total there)
+		}
+		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
 		up.insert(up.end(), reinterpret_cast<const uint8_t*>(lists.data()), reinterpret_cast<const uint8_t*>(lists.data()) + lists_bytes);
 		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.pairs.data()), reinterpret_cast<const uint8_t*>(call.pairs.data()) + pairs_bytes);
 		up.insert(up.end(), reinterpret_cast<const uint8_t*>(rows.data()), reinterpret_cast<const uint8_t*>(rows.data()) + rows_bytes);
 		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.words.data()), reinterpret_cast<const uint8_t*>(call.words.data()) + call.words.size() * sizeof(uint32_t));
 		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+	}
+	if (st == ASTCENC_SUCCESS && call.packed) {
+		astc_pack_lists_kernel<<<1, 32, 0, stream>>>(ctx->list.as<GatherImage>(), reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes),
+		                                             (unsigned int)call.table.size(), call.budget, call.overflow);
+		ctx->launches++;
+		CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
 	// (refine calls) the decide and commit arguments and the decode tables
 	RefineArgs r{};
@@ -1846,7 +1885,7 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	// across the seams between unrelated blocks. A source's averages cover its window's rows, at their image positions, in the
 	// source's region of list_alpha. The threshold depends on the footprint and the radius alone: one value serves every source.
 	float threshold = 0.0f;
-	for (size_t k = 0; k < call.table.size() && st == ASTCENC_SUCCESS && radius != 0; k++) {
+	for (size_t k = 0; k < call.table.size() && st == ASTCENC_SUCCESS && radius != 0 && n != 0; k++) {
 		const GatherImage& e = call.table[k];
 		const DevImage src = pass_image(ctx, e.data, call.data_type, e.dim_x, e.dim_y, e.dim_z, swizzle);
 		st = alpha_prepass(ctx, src, call.rows[k].first, call.rows[k].second, ctx->list_alpha.as<float>() + e.avg_offset, stream, threshold);
@@ -1867,7 +1906,12 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 		g.base = first;
 		g.n = m;
 		const unsigned int warps = ASTC_GATHER_THREADS / 32;
-		astc_gather_blocks_kernel<<<(m + warps - 1) / warps < (unsigned int)ctx->plan.grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->plan.grid * 16, ASTC_GATHER_THREADS, 0, stream>>>(g);
+		const unsigned int gather_grid = (m + warps - 1) / warps < (unsigned int)ctx->plan.grid * 16 ? (m + warps - 1) / warps : (unsigned int)ctx->plan.grid * 16;
+		if (call.packed) {
+			astc_gather_blocks_packed_kernel<<<gather_grid, ASTC_GATHER_THREADS, 0, stream>>>(g);
+		} else {
+			astc_gather_blocks_kernel<<<gather_grid, ASTC_GATHER_THREADS, 0, stream>>>(g);
+		}
 		ctx->launches++;
 		// (the staging volume is one layer deep)
 		DevImage staged = pass_image(ctx, ctx->list_image.ptr, call.data_type, m * bsd.dim_x, bsd.dim_y, volume ? bsd.dim_z : 1, swizzle);
@@ -1877,18 +1921,34 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 		if (st == ASTCENC_SUCCESS && refine) {
 			enqueue_decode(ctx, d_rows + (m == chunk ? 0 : 1), 1, m, call.refine.decoded_type, call.refine.decode_swizzle, stream);
 			const unsigned int grid = (m + ASTC_REFINE_LIST_WARPS - 1) / ASTC_REFINE_LIST_WARPS;
-			if (call.refine.block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
-				astc_refine_decide_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-			} else if (call.refine.block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
-				astc_refine_decide_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+			if (call.packed) {
+				if (call.refine.block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
+					astc_refine_decide_packed_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				} else if (call.refine.block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
+					astc_refine_decide_packed_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				} else {
+					astc_refine_decide_packed_kernel<ASTCENC_B200_BLOCK_SQUARED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				}
+				astc_refine_commit_packed_kernel<<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(ctx->list_out.ptr, g, r);
 			} else {
-				astc_refine_decide_kernel<ASTCENC_B200_BLOCK_SQUARED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				if (call.refine.block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
+					astc_refine_decide_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				} else if (call.refine.block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
+					astc_refine_decide_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				} else {
+					astc_refine_decide_kernel<ASTCENC_B200_BLOCK_SQUARED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				}
+				astc_refine_commit_kernel<<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(ctx->list_out.ptr, g, r);
 			}
-			astc_refine_commit_kernel<<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(ctx->list_out.ptr, g, r);
 			ctx->launches += 2;
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 		} else if (st == ASTCENC_SUCCESS) {
-			astc_scatter_blocks_kernel<<<(m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g);
+			const unsigned int grid = (m + ASTC_GATHER_THREADS - 1) / ASTC_GATHER_THREADS;
+			if (call.packed) {
+				astc_scatter_blocks_packed_kernel<<<grid, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g);
+			} else {
+				astc_scatter_blocks_kernel<<<grid, ASTC_GATHER_THREADS, 0, stream>>>(ctx->list_out.ptr, g);
+			}
 			ctx->launches++;
 			CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 		}
@@ -1896,7 +1956,8 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	return st;
 }
 
-// A staging call on `cuda_stream` (null: the context's stream); a call of no staging blocks launches nothing.
+// A staging call on `cuda_stream` (null: the context's stream); a call of no staging blocks launches nothing (a packed call:
+// one whose capacities are all 0, whatever its budget).
 static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, void* cuda_stream) {
 	if (call.blocks == 0) {
 		return ASTCENC_SUCCESS;
@@ -2170,9 +2231,9 @@ astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* 
 
 // Device block lists: an image table whose entry j owns capacity[j] staging blocks, the slots of its device list (GatherList).
 // Checked whole before anything is enqueued, in the image-table order of astcenc_b200_compress_device_images; entries with a
-// capacity of 0 are checked and then left out of the call.
-astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count,
-                                                       astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
+// capacity of 0 are checked and then left out of the call. The unpacked and packed calls share this plan.
+static astcenc_error plan_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count,
+                                             astcenc_type data_type, const astcenc_swizzle* swizzle, BlockCall& call) {
 	astcenc_error status = check_compress_context(ctx);
 	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
 	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
@@ -2194,18 +2255,44 @@ astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, con
 		entries[i].list = &gather_lists[i];
 		entries[i].blocks = lists[i].capacity;
 	}
-	BlockCall call;
 	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	return status;
+}
+
+astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count,
+                                                       astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
+	BlockCall call;
+	const astcenc_error status = plan_device_block_lists(ctx, lists, list_count, data_type, swizzle, call);
+	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
+}
+
+// Packed calls (astc_dev_pack.cuh): the plan of the unpacked call, then the overflow pointer's alignment.
+static astcenc_error pack_call(BlockCall& call, unsigned int budget, uint32_t* overflow) {
+	if ((reinterpret_cast<uintptr_t>(overflow) & 3) != 0) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	call.packed = true;
+	call.budget = budget;
+	call.overflow = overflow;
+	return ASTCENC_SUCCESS;
+}
+
+astcenc_error astcenc_b200_compress_device_block_lists_packed(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count,
+                                                              unsigned int budget, uint32_t* overflow, astcenc_type data_type, const astcenc_swizzle* swizzle,
+                                                              void* cuda_stream) {
+	BlockCall call;
+	astcenc_error status = plan_device_block_lists(ctx, lists, list_count, data_type, swizzle, call);
+	if (status == ASTCENC_SUCCESS) status = pack_call(call, budget, overflow);
 	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
 }
 
 // Refine calls (astc_dev_refine.cuh): the block-list table of astcenc_b200_compress_device_block_lists, each entry with its pair
 // (original, decode and map). Checked whole before anything is enqueued, in the order include/astcenc.h gives; entries with a
-// capacity of 0 are checked and then left out of the call.
-astcenc_error astcenc_b200_refine_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_refine_list* lists, unsigned int list_count,
-                                                     astcenc_type data_type, const astcenc_swizzle* swizzle, astcenc_type decoded_type,
-                                                     const astcenc_swizzle* decode_swizzle, int input_components, astcenc_b200_block_metric block_metric,
-                                                     void* cuda_stream) {
+// capacity of 0 are checked and then left out of the call. The unpacked and packed calls share this plan.
+static astcenc_error plan_refine_lists(astcenc_context* ctx, const astcenc_b200_device_refine_list* lists, unsigned int list_count,
+                                       astcenc_type data_type, const astcenc_swizzle* swizzle, astcenc_type decoded_type,
+                                       const astcenc_swizzle* decode_swizzle, int input_components, astcenc_b200_block_metric block_metric,
+                                       BlockCall& call) {
 	astcenc_error status = check_compress_context(ctx);
 	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
 	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
@@ -2253,7 +2340,6 @@ astcenc_error astcenc_b200_refine_device_block_lists(astcenc_context* ctx, const
 		entries[i].blocks = l.capacity;
 		entries[i].pair = &pairs[i];
 	}
-	BlockCall call;
 	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
 	if (status != ASTCENC_SUCCESS) {
 		return status;
@@ -2262,7 +2348,26 @@ astcenc_error astcenc_b200_refine_device_block_lists(astcenc_context* ctx, const
 	call.refine.decode_swizzle = *decode_swizzle;
 	call.refine.block_metric = (int)block_metric;
 	call.refine.components = input_components;
-	return launch_blocks(ctx, call, *swizzle, cuda_stream);
+	return ASTCENC_SUCCESS;
+}
+
+astcenc_error astcenc_b200_refine_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_refine_list* lists, unsigned int list_count,
+                                                     astcenc_type data_type, const astcenc_swizzle* swizzle, astcenc_type decoded_type,
+                                                     const astcenc_swizzle* decode_swizzle, int input_components, astcenc_b200_block_metric block_metric,
+                                                     void* cuda_stream) {
+	BlockCall call;
+	const astcenc_error status = plan_refine_lists(ctx, lists, list_count, data_type, swizzle, decoded_type, decode_swizzle, input_components, block_metric, call);
+	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
+}
+
+astcenc_error astcenc_b200_refine_device_block_lists_packed(astcenc_context* ctx, const astcenc_b200_device_refine_list* lists, unsigned int list_count,
+                                                            unsigned int budget, uint32_t* overflow, astcenc_type data_type, const astcenc_swizzle* swizzle,
+                                                            astcenc_type decoded_type, const astcenc_swizzle* decode_swizzle, int input_components,
+                                                            astcenc_b200_block_metric block_metric, void* cuda_stream) {
+	BlockCall call;
+	astcenc_error status = plan_refine_lists(ctx, lists, list_count, data_type, swizzle, decoded_type, decode_swizzle, input_components, block_metric, call);
+	if (status == ASTCENC_SUCCESS) status = pack_call(call, budget, overflow);
+	return status == ASTCENC_SUCCESS ? launch_blocks(ctx, call, *swizzle, cuda_stream) : status;
 }
 
 // Decode calls over device block lists: the image table of astcenc_b200_decompress_device_images whose entry j owns capacity[j]

@@ -704,6 +704,46 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_refine_device_block_lists(struct 
                                                                         enum astcenc_b200_block_metric block_metric, void* cuda_stream);
 
 /**
+ * Packed block lists: astcenc_b200_compress_device_block_lists and astcenc_b200_refine_device_block_lists at a cost set by a
+ * budget the caller states rather than by the sum of the capacities. After astcenc_b200_select_blocks_pooled keeps the K worst
+ * blocks of a texture set, each image's list needs capacity min(K, n_j), because the split of K between the images is known
+ * only on the device; the unpacked calls stage every one of those slots, the packed calls stage at most `budget` of them.
+ * The descriptors are those of the unpacked calls, and so are the arguments after `overflow`.
+ * - Listed slots. Entry j lists v_j = min(*count_j, capacity_j) slots; the count is read on the device when the call runs. An
+ *   entry of capacity 0 lists none, and its count is not read.
+ * - Packing. Slot s < v_j of entry j gets the packed position P_j + s, P_j being the sum of v_i over the entries i < j in call
+ *   order (summed in 64 bits, without overflow). Packing reads only the count words, never the indices: a slot whose index is
+ *   out of range still takes a position, and the list rule then skips it.
+ * - Budget. A slot at a packed position below `budget` is processed exactly as the unpacked call processes it: the list rule,
+ *   skipped indices and duplicates, and for refine calls the candidate, its value v', the commit rule and the consistency of
+ *   payload, decode and map. A slot at or beyond `budget` is not processed, and its block keeps every byte. Truncation
+ *   therefore drops the trailing slots in entry order, deterministically.
+ * - Equivalence. When the sum of v_j is at most `budget`, the packed call writes the same payload bytes as the unpacked call
+ *   with the same table, byte for byte, and a refine call the same decoded texels and map values, bit for bit. With the lists
+ *   of astcenc_b200_select_blocks_pooled and `budget` the sum of the capacities of the pools that cover the entries, this
+ *   always holds.
+ * - overflow. A device word, or NULL, aligned to 4 bytes. It receives the sum of v_j minus `budget` when that is positive and 0
+ *   otherwise, saturated at 0xFFFFFFFF. Every successful call in which some entry has capacity > 0 writes it, budget == 0
+ *   included.
+ * Cost: the staging row has min(budget, sum of capacity_j) slots (the host knows both), so a packed call never stages more
+ * than the unpacked one. The call makes the unpacked call's launches over that many slots plus one, the packing kernel,
+ * launched after the table copy and before the first gather. A call whose capacities are all 0 launches nothing and writes
+ * nothing; a call with budget == 0 and some capacity is the packing launch alone. With a_scale_radius (2D block sizes) each
+ * entry gets its whole-image alpha-scale pre-pass, as in the unpacked call.
+ * Errors: those of the unpacked call, in its order; after them ASTCENC_ERR_BAD_PARAM for an overflow pointer not aligned to 4
+ * bytes. On error nothing is launched and nothing is written. Any budget is accepted.
+ */
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compress_device_block_lists_packed(
+    struct astcenc_context* context, const struct astcenc_b200_device_block_list* lists, unsigned int list_count,
+    unsigned int budget, uint32_t* overflow, enum astcenc_type data_type, const struct astcenc_swizzle* swizzle, void* cuda_stream);
+
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_refine_device_block_lists_packed(
+    struct astcenc_context* context, const struct astcenc_b200_device_refine_list* lists, unsigned int list_count,
+    unsigned int budget, uint32_t* overflow, enum astcenc_type data_type, const struct astcenc_swizzle* swizzle,
+    enum astcenc_type decoded_type, const struct astcenc_swizzle* decode_swizzle, int input_components,
+    enum astcenc_b200_block_metric block_metric, void* cuda_stream);
+
+/**
  * Totals of device-resident per-block maps, and from each total a selection weight that is zero once the image meets a target:
  * the device side of a per-image quality target ("every texture at 40 dB or better") in the refinement loop.
  * - Total. The sum of the entry's block_count map values, accumulated in double in a fixed order that depends only on
@@ -722,9 +762,10 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_refine_device_block_lists(struct 
  *   to the per-block float rounding of the map, so a target met within that rounding may be judged either way. limit
  *   = -INFINITY never meets the target.
  * - The closed loop. Compress, decode and map the set once; then enqueue every round up front, each one this call (then the
- *   weights are current), astcenc_b200_select_blocks_pooled with these weights, a threshold of 0 and the round's budget, and
- *   astcenc_b200_refine_device_block_lists, which keeps the maps current. Images that reach their target get no blocks in later
- *   rounds and the budget goes to those that still miss theirs, with no host synchronisation between rounds.
+ *   weights are current), astcenc_b200_select_blocks_pooled with these weights, a threshold of 0 and the round's budget K, and
+ *   astcenc_b200_refine_device_block_lists_packed with budget K, which keeps the maps current and stages K slots rather than
+ *   the sum of the capacities min(K, n_j). Images that reach their target get no blocks in later rounds and the budget goes
+ *   to those that still miss theirs, with no host synchronisation between rounds.
  *   ASTCENC_B200_WEIGHT_INVERSE_TOTAL gives the weights 1 / E_j (rule (d) of the pooled selection: a block ranks by its share
  *   of its image's error) with the same gate.
  * Enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in order with every other pass of the

@@ -32,6 +32,10 @@ ERR_OUT_OF_MEM, ERR_BAD_PARAM, ERR_BAD_BLOCK_SIZE, ERR_BAD_SWIZZLE, ERR_BAD_CONT
 BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR, BLOCK_LOG2_ERROR = 0, 1, 2
 # enum astcenc_b200_weight_rule: the selection weight of an image that misses its target
 WEIGHT_ONE, WEIGHT_INVERSE_TOTAL = 0, 1
+# the flags of struct astcenc_b200_block_summary
+BLOCK_IS_ERROR, BLOCK_IS_CONSTANT, BLOCK_IS_HDR, BLOCK_IS_DUAL_PLANE = 1, 2, 4, 8
+# sizeof(struct astcenc_block_info): the slot size of get_block_info_device_block_lists outputs
+BLOCK_INFO_BYTES = 2144
 
 
 class AstcencError(RuntimeError):
@@ -126,6 +130,32 @@ class DeviceRefineList(C.Structure):
     """struct astcenc_b200_device_refine_list (include/astcenc.h)."""
     _fields_ = [("data", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("payload", C.c_void_p), ("decoded", C.c_void_p),
                 ("block_error", C.c_void_p), ("indices", C.c_void_p), ("count", C.c_void_p), ("capacity", C.c_uint)]
+
+
+class BlockSummary(C.Structure):
+    """struct astcenc_b200_block_summary (include/astcenc.h): 16 bytes per block."""
+    _fields_ = [("flags", C.c_uint8), ("partition_count", C.c_uint8), ("partition_index", C.c_uint16), ("dual_plane_component", C.c_uint8),
+                ("weight_x", C.c_uint8), ("weight_y", C.c_uint8), ("weight_z", C.c_uint8), ("color_endpoint_modes", C.c_uint8 * 4),
+                ("color_level_count", C.c_uint16), ("weight_level_count", C.c_uint8), ("reserved", C.c_uint8)]
+
+
+# The same layout as a numpy structured dtype: a torch uint8 buffer of summaries, copied to the host as numpy, is read field by
+# field with buf.view(BLOCK_SUMMARY_DTYPE)["partition_count"].
+BLOCK_SUMMARY_DTYPE = np.dtype([("flags", np.uint8), ("partition_count", np.uint8), ("partition_index", "<u2"), ("dual_plane_component", np.uint8),
+                                ("weight_x", np.uint8), ("weight_y", np.uint8), ("weight_z", np.uint8), ("color_endpoint_modes", np.uint8, (4,)),
+                                ("color_level_count", "<u2"), ("weight_level_count", np.uint8), ("reserved", np.uint8)])
+assert BLOCK_SUMMARY_DTYPE.itemsize == C.sizeof(BlockSummary) == 16
+
+
+class DeviceBlockSummaryImage(C.Structure):
+    """struct astcenc_b200_device_block_summary_image (include/astcenc.h)."""
+    _fields_ = [("payload", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("summaries", C.c_void_p)]
+
+
+class DeviceBlockInfoList(C.Structure):
+    """struct astcenc_b200_device_block_info_list (include/astcenc.h)."""
+    _fields_ = [("payload", C.c_void_p), ("dim_x", C.c_uint), ("dim_y", C.c_uint), ("dim_z", C.c_uint), ("indices", C.c_void_p), ("count", C.c_void_p),
+                ("capacity", C.c_uint), ("infos", C.c_void_p)]
 
 
 class ErrorMetrics(C.Structure):
@@ -227,6 +257,10 @@ def lib():
         l.astcenc_b200_refine_device_block_lists_packed.argtypes = [C.c_void_p, C.POINTER(DeviceRefineList), C.c_uint, C.c_uint, C.c_void_p, C.c_int,
                                                                     C.POINTER(Swizzle), C.c_int, C.POINTER(Swizzle), C.c_int, C.c_int, C.c_void_p]
         l.astcenc_b200_refine_device_block_lists_packed.restype = C.c_int
+        l.astcenc_b200_get_block_summaries_device_images.argtypes = [C.c_void_p, C.POINTER(DeviceBlockSummaryImage), C.c_uint, C.c_void_p]
+        l.astcenc_b200_get_block_summaries_device_images.restype = C.c_int
+        l.astcenc_b200_get_block_info_device_block_lists.argtypes = [C.c_void_p, C.POINTER(DeviceBlockInfoList), C.c_uint, C.c_void_p]
+        l.astcenc_b200_get_block_info_device_block_lists.restype = C.c_int
         l.astcenc_b200_store_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t]
         l.astcenc_b200_store_cimage.restype = C.c_int
         l.astcenc_b200_load_cimage.argtypes = [C.c_char_p, C.POINTER(CImageHeader), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -623,6 +657,28 @@ class Context:
                                                                C.c_void_p(stream))
         if err:
             raise AstcencError(err, "astcenc_b200_decompress_device_block_lists")
+
+    def get_block_summaries_device_images(self, images, stream=0):
+        """Summaries of every block of device-resident payloads (astcenc_b200_get_block_summaries_device_images). images: a
+        sequence of (d_payload_ptr, dim_x, dim_y, dim_z, d_summaries_ptr); summaries[b] (16 bytes, BLOCK_SUMMARY_DTYPE) holds the
+        fields get_block_info reports for block b, narrowed. Enqueued on `stream`, no sync; works on decompress-only contexts."""
+        n = len(images)
+        table = (DeviceBlockSummaryImage * n)(*[DeviceBlockSummaryImage(C.c_void_p(p), x, y, z, C.c_void_p(q)) for p, x, y, z, q in images])
+        err = lib().astcenc_b200_get_block_summaries_device_images(self.handle, table if n else None, n, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_get_block_summaries_device_images")
+
+    def get_block_info_device_block_lists(self, lists, stream=0):
+        """The full astcenc_block_info of the blocks of device lists (astcenc_b200_get_block_info_device_block_lists). lists: a
+        sequence of (d_payload_ptr, dim_x, dim_y, dim_z, d_indices_ptr, d_count_ptr, capacity, d_infos_ptr); for each of the first
+        min(*count, capacity) slots whose index is in range, infos[s] (BLOCK_INFO_BYTES bytes) receives what get_block_info writes
+        for block indices[s]; other slots are left untouched. Enqueued on `stream`, no sync; works on decompress-only contexts."""
+        n = len(lists)
+        table = (DeviceBlockInfoList * n)(*[DeviceBlockInfoList(C.c_void_p(p), x, y, z, C.c_void_p(i or None), C.c_void_p(k or None), c, C.c_void_p(o or None))
+                                            for p, x, y, z, i, k, c, o in lists])
+        err = lib().astcenc_b200_get_block_info_device_block_lists(self.handle, table if n else None, n, C.c_void_p(stream))
+        if err:
+            raise AstcencError(err, "astcenc_b200_get_block_info_device_block_lists")
 
     def compute_block_errors_device_block_lists(self, lists, input_components=4, stream=0):
         """Refresh per-block error maps at device-resident block lists (astcenc_b200_compute_block_errors_device_block_lists).

@@ -6,6 +6,7 @@
 // One warp per block. The warp's slice of shared memory holds the symbolic block: weights[64], colour values
 // [4][8], the unpacked endpoints and a few scalars.
 #pragma once
+#include "../../include/astcenc.h"
 
 // decode slice layout (bytes from the slice base)
 enum { D_WEIGHTS = 0, D_COLORS = 64, D_ENDS = 96 /* int[4][8] + lns flags */, D_HDR = 96 + 128 + 16, D_SLICE = 304 };
@@ -79,22 +80,38 @@ ASTC_NOINLINE void decode_ise_mapped(int quant_level, unsigned int count, uint64
 	}
 }
 
-// physical_to_symbolic. Executed by lane 0; the result lands in the slice.
-ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi) {
+// The header stage of physical_to_symbolic (astcenc_symbolic_physical.cpp:291-556 without the two ISE decodes and the constant
+// colour), in registers: the block-type verdict (void extents 2D and 3D, reserved bits, the block-mode table, dual plane with
+// four partitions, partition-table validity, more than 18 colour integers, colour quant below QUANT_6) and the header fields.
+// An error block keeps the fields read before the rule it breaks; nothing reads them.
+struct BlockHeader {
+	int block_type, partition_count, partition_index, block_mode_packed, plane2_component, quant_mode;
+	int color_formats[4];
+	int weight_count;              // the weights of both planes
+	int weight_quant;
+	int color_integer_count;       // the colour values of all partitions
+	bool dual;
+};
+
+ASTC_FN BlockHeader block_header(uint64_t lo, uint64_t hi) {
 	const DevConstTables* ct = ASTC_CT;
-	DecodeHdr& h = *reinterpret_cast<DecodeHdr*>(astc_smem + slice + D_HDR);
+	BlockHeader h;
 	h.block_type = SYM_BTYPE_NONCONST;
 	h.partition_count = 0;
 	h.partition_index = 0;
 	h.block_mode_packed = 0;
 	h.plane2_component = -1;
 	h.quant_mode = 0;
+	for (int i = 0; i < 4; i++) {
+		h.color_formats[i] = 0;
+	}
+	h.weight_count = 0;
+	h.weight_quant = 0;
+	h.color_integer_count = 0;
+	h.dual = false;
 	int block_mode = (int)rd_bits(lo, hi, 11, 0);
 	if ((block_mode & 0x1FF) == 0x1FC) {
 		h.block_type = (block_mode & 0x200) ? SYM_BTYPE_CONST_F16 : SYM_BTYPE_CONST_U16;
-		for (int i = 0; i < 4; i++) {
-			h.constant_color[i] = (int)rd_bits(hi, 0, 16, 16 * (unsigned int)i);
-		}
 		if (BSD.dim_z > 1) {
 			// 3D void extent (astcenc_symbolic_physical.cpp:348-366): six 9-bit coordinates, no reserved bits
 			int v[6];
@@ -106,12 +123,12 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 			if ((v[0] >= v[1] || v[2] >= v[3] || v[4] >= v[5]) && !ones) {
 				h.block_type = SYM_BTYPE_ERROR;
 			}
-			return;
+			return h;
 		}
 		int rsvbits = (int)rd_bits(lo, hi, 2, 10);
 		if (rsvbits != 3) {
 			h.block_type = SYM_BTYPE_ERROR;
-			return;
+			return h;
 		}
 		int vx_low_s = (int)rd_bits(lo, hi, 13, 12);
 		int vx_high_s = (int)rd_bits(lo, hi, 13, 25);
@@ -121,34 +138,30 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 		if ((vx_low_s >= vx_high_s || vx_low_t >= vx_high_t) && !all_ones) {
 			h.block_type = SYM_BTYPE_ERROR;
 		}
-		return;
+		return h;
 	}
 	unsigned int packed_index = ASTC_LDG(&BSD.block_mode_packed_index[block_mode]);
 	if (packed_index == 0xFFFF) {
 		h.block_type = SYM_BTYPE_ERROR;
-		return;
+		return h;
 	}
 	const DevBlockMode* bm = BSD.block_modes + packed_index;
 	int weight_count = ASTC_LDG(&BSD.dec_modes[ASTC_LDG(&bm->decimation_mode)].weight_count);
-	int weight_quant_method = ASTC_LDG(&bm->quant_mode);
-	int is_dual_plane = ASTC_LDG(&bm->is_dual_plane);
-	int real_weight_count = is_dual_plane ? 2 * weight_count : weight_count;
+	h.weight_quant = ASTC_LDG(&bm->quant_mode);
+	h.dual = ASTC_LDG(&bm->is_dual_plane) != 0;
+	h.weight_count = h.dual ? 2 * weight_count : weight_count;
 	int partition_count = (int)rd_bits(lo, hi, 2, 11) + 1;
 	h.block_mode_packed = (int)packed_index;
 	h.partition_count = partition_count;
-	int bits_for_weights = (int)ise_sequence_bitcount((unsigned int)real_weight_count, weight_quant_method);
+	int bits_for_weights = (int)ise_sequence_bitcount((unsigned int)h.weight_count, h.weight_quant);
 	int below_weights_pos = 128 - bits_for_weights;
-	// the weight stream is read from the top of the block, bit-reversed (:404-407)
-	decode_ise_mapped(weight_quant_method, (unsigned int)real_weight_count, brev64(hi), brev64(lo), 0, ct->wq_unscramble_and_unquant[weight_quant_method],
-	                  slice + D_WEIGHTS, is_dual_plane);
-	if (is_dual_plane && partition_count == 4) {
+	if (h.dual && partition_count == 4) {
 		h.block_type = SYM_BTYPE_ERROR;
-		return;
+		return h;
 	}
-	int color_formats[4] = {0, 0, 0, 0};
 	int encoded_type_highpart_size = 0;
 	if (partition_count == 1) {
-		color_formats[0] = (int)rd_bits(lo, hi, 4, 13);
+		h.color_formats[0] = (int)rd_bits(lo, hi, 4, 13);
 	} else {
 		encoded_type_highpart_size = (3 * partition_count) - 4;
 		below_weights_pos -= encoded_type_highpart_size;
@@ -156,7 +169,7 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 		int baseclass = encoded_type & 0x3;
 		if (baseclass == 0) {
 			for (int i = 0; i < 4; i++) {
-				if (i < partition_count) color_formats[i] = (encoded_type >> 2) & 0xF;
+				if (i < partition_count) h.color_formats[i] = (encoded_type >> 2) & 0xF;
 			}
 			below_weights_pos += encoded_type_highpart_size;
 			encoded_type_highpart_size = 0;
@@ -165,13 +178,13 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 			baseclass--;
 			for (int i = 0; i < 4; i++) {
 				if (i < partition_count) {
-					color_formats[i] = (((encoded_type >> bitpos) & 1) + baseclass) << 2;
+					h.color_formats[i] = (((encoded_type >> bitpos) & 1) + baseclass) << 2;
 					bitpos++;
 				}
 			}
 			for (int i = 0; i < 4; i++) {
 				if (i < partition_count) {
-					color_formats[i] |= (encoded_type >> bitpos) & 3;
+					h.color_formats[i] |= (encoded_type >> bitpos) & 3;
 					bitpos += 2;
 				}
 			}
@@ -179,22 +192,22 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 		h.partition_index = (int)rd_bits(lo, hi, 10, 13);
 		if (ASTC_LDG(&BSD.partitioning_packed_index[partition_count - 2][h.partition_index]) == 0xFFFF) {
 			h.block_type = SYM_BTYPE_ERROR;
-			return;
+			return h;
 		}
 	}
 	int color_integer_count = 0;
 	for (int i = 0; i < 4; i++) {
-		h.color_formats[i] = color_formats[i];
 		if (i < partition_count) {
-			color_integer_count += ((color_formats[i] >> 2) + 1) * 2;
+			color_integer_count += ((h.color_formats[i] >> 2) + 1) * 2;
 		}
 	}
+	h.color_integer_count = color_integer_count;
 	if (color_integer_count > 18) {
 		h.block_type = SYM_BTYPE_ERROR;
-		return;
+		return h;
 	}
 	int color_bits = (partition_count == 1 ? 115 - 4 : 113 - 4 - 10) - bits_for_weights - encoded_type_highpart_size;
-	if (is_dual_plane) {
+	if (h.dual) {
 		color_bits -= 2;
 	}
 	if (color_bits < 0) {
@@ -203,18 +216,51 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 	int color_quant_level = ASTC_LDG(&ct->quant_mode_table[color_integer_count >> 1][color_bits]);
 	if (color_quant_level < QUANT_6) {
 		h.block_type = SYM_BTYPE_ERROR;
-		return;
+		return h;
 	}
 	h.quant_mode = color_quant_level;
+	if (h.dual) {
+		h.plane2_component = (int)rd_bits(lo, hi, 2, (unsigned int)(below_weights_pos - 2));
+	}
+	return h;
+}
+
+// physical_to_symbolic: the header stage, then the weight and colour ISE decodes and the constant colour. Executed by lane 0;
+// the result lands in the slice.
+ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi) {
+	const DevConstTables* ct = ASTC_CT;
+	DecodeHdr& h = *reinterpret_cast<DecodeHdr*>(astc_smem + slice + D_HDR);
+	const BlockHeader b = block_header(lo, hi);
+	h.block_type = b.block_type;
+	h.partition_count = b.partition_count;
+	h.partition_index = b.partition_index;
+	h.block_mode_packed = b.block_mode_packed;
+	h.plane2_component = b.plane2_component;
+	h.quant_mode = b.quant_mode;
+	for (int i = 0; i < 4; i++) {
+		h.color_formats[i] = b.color_formats[i];
+	}
+	if (b.block_type == SYM_BTYPE_CONST_F16 || b.block_type == SYM_BTYPE_CONST_U16) {
+		for (int i = 0; i < 4; i++) {
+			h.constant_color[i] = (int)rd_bits(hi, 0, 16, 16 * (unsigned int)i);
+		}
+		return;
+	}
+	if (b.block_type != SYM_BTYPE_NONCONST) {
+		return;
+	}
+	// the weight stream is read from the top of the block, bit-reversed (:404-407)
+	decode_ise_mapped(b.weight_quant, (unsigned int)b.weight_count, brev64(hi), brev64(lo), 0, ct->wq_unscramble_and_unquant[b.weight_quant],
+	                  slice + D_WEIGHTS, b.dual ? 1 : 0);
 	// the colour values of all partitions are one sequence; partition p's values start at 8 * p in the slice
 	SPtr<uint8_t> colors = sptr<uint8_t>(slice + D_COLORS);
 	SPtr<uint8_t> tmp = sptr<uint8_t>(slice + D_ENDS);      // staging (the endpoints are unpacked afterwards)
-	decode_ise_mapped(color_quant_level, (unsigned int)color_integer_count, lo, hi, partition_count == 1 ? 17u : 19u + 10u,
-	                  ct->color_scrambled_pquant_to_uquant[color_quant_level - QUANT_6], slice + D_ENDS, 0);
+	decode_ise_mapped(b.quant_mode, (unsigned int)b.color_integer_count, lo, hi, b.partition_count == 1 ? 17u : 19u + 10u,
+	                  ct->color_scrambled_pquant_to_uquant[b.quant_mode - QUANT_6], slice + D_ENDS, 0);
 	int k = 0;
 	for (int i = 0; i < 4; i++) {
-		if (i < partition_count) {
-			int vals = 2 * (color_formats[i] >> 2) + 2;
+		if (i < b.partition_count) {
+			int vals = 2 * (b.color_formats[i] >> 2) + 2;
 			for (int j = 0; j < 8; j++) {
 				if (j < vals) {
 					colors[i * 8 + j] = tmp[k + j];
@@ -222,9 +268,6 @@ ASTC_NOINLINE void physical_to_symbolic(uint32_t slice, uint64_t lo, uint64_t hi
 			}
 			k += vals;
 		}
-	}
-	if (is_dual_plane) {
-		h.plane2_component = (int)rd_bits(lo, hi, 2, (unsigned int)(below_weights_pos - 2));
 	}
 }
 
@@ -443,28 +486,35 @@ ASTC_COOP void decompress_block(int lane, uint32_t slice, const uint8_t* pcb, un
 }
 
 // ---------------------------------------------------------------------------------------------
-// astcenc_get_block_info (astcenc_entry.cpp:1401-1517): the decoded view of one block. Filled by one warp.
+// astcenc_get_block_info (astcenc_entry.cpp:1401-1517): the decoded view of one block, written straight into the public
+// astcenc_block_info layout by one warp (astcenc_get_block_info, astcenc_b200_get_block_info_device_block_lists).
 // ---------------------------------------------------------------------------------------------
-struct DevBlockInfo {
-	int is_error_block, is_constant_block, is_hdr_block, is_dual_plane_block;
-	unsigned int partition_count, partition_index, dual_plane_component;
-	unsigned int color_endpoint_modes[4];
-	unsigned int color_level_count, weight_level_count, weight_x, weight_y, weight_z;
-	float color_endpoints[4][2][4];
-	float weight_values_plane1[ASTC_MAX_TEXELS];
-	float weight_values_plane2[ASTC_MAX_TEXELS];
-	uint8_t partition_assignment[ASTC_MAX_TEXELS];
+// The fields astcenc_get_block_info takes from the context rather than from the block.
+struct BlockInfoHead {
+	int profile;
+	unsigned int block_x, block_y, block_z, texel_count;
 };
 
-ASTC_COOP void block_info(int lane, uint32_t slice, uint64_t lo, uint64_t hi, DevBlockInfo* out) {
+// Every byte of *out (4-byte aligned): zeros where the reference leaves its memset's zeros. The lanes zero the struct word by
+// word; the barrier after the parse orders those stores before the fields'.
+ASTC_COOP void block_info(int lane, uint32_t slice, uint64_t lo, uint64_t hi, const BlockInfoHead& head, astcenc_block_info* out) {
 	int T = BSD.texel_count;
 	DecodeHdr& h = *reinterpret_cast<DecodeHdr*>(astc_smem + slice + D_HDR);
+	uint32_t* words = reinterpret_cast<uint32_t*>(out);
+	for (int k = lane; k < (int)(sizeof(astcenc_block_info) / 4); k += ASTC_WARP) {
+		words[k] = 0;
+	}
 	if (lane == 0) {
 		physical_to_symbolic(slice, lo, hi);
 	}
 	wsync();
 	int block_type = h.block_type;
 	if (lane == 0) {
+		out->profile = (astcenc_profile)head.profile;
+		out->block_x = head.block_x;
+		out->block_y = head.block_y;
+		out->block_z = head.block_z;
+		out->texel_count = head.texel_count;
 		out->is_error_block = block_type == SYM_BTYPE_ERROR;
 		out->is_constant_block = block_type == SYM_BTYPE_CONST_F16 || block_type == SYM_BTYPE_CONST_U16;
 	}
@@ -481,13 +531,13 @@ ASTC_COOP void block_info(int lane, uint32_t slice, uint64_t lo, uint64_t hi, De
 		out->weight_x = ASTC_LDG(&BSD.dec_modes[d].weight_x);
 		out->weight_y = ASTC_LDG(&BSD.dec_modes[d].weight_y);
 		out->weight_z = ASTC_LDG(&BSD.dec_modes[d].weight_z);
-		out->is_dual_plane_block = dual ? 1 : 0;
+		out->is_dual_plane_block = dual;
 		out->partition_count = (unsigned int)pc;
 		out->partition_index = (unsigned int)h.partition_index;
 		out->dual_plane_component = (unsigned int)h.plane2_component;
 		out->color_level_count = quant_level_count(h.quant_mode);
 		out->weight_level_count = quant_level_count(ASTC_LDG(&bm->quant_mode));
-		int is_hdr = 0;
+		bool is_hdr = false;
 		for (int p = 0; p < 4; p++) {
 			if (p >= pc) {
 				break;
@@ -527,4 +577,72 @@ ASTC_COOP void block_info(int lane, uint32_t slice, uint64_t lo, uint64_t hi, De
 		}
 		out->partition_assignment[t] = ASTC_LDG(&pi.partition_of_texel[t]);
 	}
+}
+
+// ---------------------------------------------------------------------------------------------
+// astcenc_b200_get_block_summaries_device_images: the 16-byte summary of one block (struct astcenc_b200_block_summary) from the
+// header stage alone, by one lane. Each field is the same-named field block_info writes, narrowed; error and constant blocks
+// get their flag and zeros, as block_info returns early for them.
+// ---------------------------------------------------------------------------------------------
+// The 16 bytes of a block as two little-endian halves. A 16-byte aligned block is one vector load on the device.
+ASTC_FN void load_block_bits(const uint8_t* pcb, uint64_t& lo, uint64_t& hi) {
+#if !defined(ASTC_HOSTSIM)
+	if ((reinterpret_cast<uintptr_t>(pcb) & 15) == 0) {
+		const uint4 v = __ldg(reinterpret_cast<const uint4*>(pcb));
+		lo = (uint64_t)v.x | ((uint64_t)v.y << 32);
+		hi = (uint64_t)v.z | ((uint64_t)v.w << 32);
+		return;
+	}
+#endif
+	const uint32_t* p32 = reinterpret_cast<const uint32_t*>(pcb);
+	lo = (uint64_t)ASTC_LDG(p32) | ((uint64_t)ASTC_LDG(p32 + 1) << 32);
+	hi = (uint64_t)ASTC_LDG(p32 + 2) | ((uint64_t)ASTC_LDG(p32 + 3) << 32);
+}
+
+// *out (16-byte aligned) from four little-endian words in the struct's byte order: one vector store on the device.
+ASTC_FN void store_summary(astcenc_b200_block_summary* out, uint32_t x, uint32_t y, uint32_t z, uint32_t w) {
+#if defined(ASTC_HOSTSIM)
+	uint32_t* p = reinterpret_cast<uint32_t*>(out);
+	p[0] = x;
+	p[1] = y;
+	p[2] = z;
+	p[3] = w;
+#else
+	*reinterpret_cast<uint4*>(out) = make_uint4(x, y, z, w);
+#endif
+}
+
+ASTC_FN void block_summary(uint64_t lo, uint64_t hi, astcenc_b200_block_summary* out) {
+	const BlockHeader h = block_header(lo, hi);
+	if (h.block_type == SYM_BTYPE_ERROR) {
+		store_summary(out, ASTCENC_B200_BLOCK_IS_ERROR, 0u, 0u, 0u);
+		return;
+	}
+	if (h.block_type != SYM_BTYPE_NONCONST) {
+		store_summary(out, ASTCENC_B200_BLOCK_IS_CONSTANT, 0u, 0u, 0u);
+		return;
+	}
+	const DevBlockMode* bm = BSD.block_modes + h.block_mode_packed;
+	const unsigned int d = ASTC_LDG(&bm->decimation_mode);
+	// is_hdr_block is rgb_hdr || alpha_hdr of unpack_color_endpoints under the context's profile. The flags depend on the
+	// endpoint mode and the profile alone, never on the colour values, so the modes are unpacked from zeros and the values are
+	// not decoded. The LDR_ONLY form leaves out the HDR unpackers (and their local arrays); it sets rgb_hdr for every HDR mode,
+	// as the general form does, so the disjunction is the same under every profile.
+	bool is_hdr = false;
+	unsigned int modes = 0;
+	for (int p = 0; p < 4; p++) {
+		if (p < h.partition_count) {
+			const uint8_t zeros[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+			bool rgb_hdr, a_hdr;
+			i4 e0, e1;
+			unpack_color_endpoints_inl<true>(CFG.profile, h.color_formats[p], zeros, rgb_hdr, a_hdr, e0, e1);
+			is_hdr = is_hdr || rgb_hdr || a_hdr;
+			modes |= (unsigned int)h.color_formats[p] << (8 * p);
+		}
+	}
+	const unsigned int flags = (is_hdr ? ASTCENC_B200_BLOCK_IS_HDR : 0u) | (h.dual ? ASTCENC_B200_BLOCK_IS_DUAL_PLANE : 0u);
+	store_summary(out, flags | ((unsigned int)h.partition_count << 8) | ((unsigned int)h.partition_index << 16),
+	              ((unsigned int)h.plane2_component & 0xFFu) | ((unsigned int)ASTC_LDG(&BSD.dec_modes[d].weight_x) << 8) |
+	                  ((unsigned int)ASTC_LDG(&BSD.dec_modes[d].weight_y) << 16) | ((unsigned int)ASTC_LDG(&BSD.dec_modes[d].weight_z) << 24),
+	              modes, quant_level_count(h.quant_mode) | (quant_level_count(h.weight_quant) << 16));
 }

@@ -266,3 +266,37 @@ ASTC_FN void decode_list_blocks(const GatherImage* images, const GatherList* lis
 		decompress_block(lane, slice, im.payload + (size_t)index * 16, k - by * im.blocks_x, by);
 	}
 }
+
+// ---- block info of device payloads (astcenc_b200_get_block_summaries_device_images, astcenc_b200_get_block_info_device_block_lists) ----
+// Both walk an image table whose entry j holds a payload and, in GatherImage::data, the output: the summaries of every block of
+// the image (call blocks [first[j], first[j + 1])), or the structs of the slots of list j (call slots [first[j], first[j + 1]),
+// the capacity[j] slots of its list, resolved as decode_list_blocks resolves them).
+//
+// Summaries of call blocks c0, c0 + step, ... below c1: one lane per block (the device takes one block per thread, grid-stride;
+// the host simulation runs lane-strided).
+ASTC_FN void summarize_table_blocks(const GatherImage* images, unsigned int image_count, size_t c0, size_t c1, size_t step) {
+	for (size_t c = c0; c < c1; c += step) {
+		const GatherImage& im = images[find_image(images, image_count, c)];
+		const size_t b = c - im.first;
+		uint64_t lo, hi;
+		load_block_bits(im.payload + b * 16, lo, hi);
+		block_summary(lo, hi, static_cast<astcenc_b200_block_summary*>(const_cast<void*>(im.data)) + b);
+	}
+}
+
+// Call slot c by one warp (lane `lane`, slice = the warp's decode slice): infos[s] of its entry for a valid slot s, nothing for
+// an invalid one (the whole warp: every lane reads the same slot).
+ASTC_FN void info_list_slot(const GatherImage* images, const GatherList* lists, unsigned int image_count, size_t c, int lane, uint32_t slice,
+                            const BlockInfoHead& head) {
+	const unsigned int j = find_image(images, image_count, c);
+	const GatherImage& im = images[j];
+	const size_t s = c - im.first;
+	const uint32_t index = list_slot(lists[j], s);
+	if (index == GATHER_INVALID) {
+		return;
+	}
+	uint64_t lo, hi;
+	load_block_bits(im.payload + (size_t)index * 16, lo, hi);
+	block_info(lane, slice, lo, hi, head, static_cast<astcenc_block_info*>(const_cast<void*>(im.data)) + s);
+	wsync();      // every lane is done with the slice before lane 0 parses the warp's next block into it
+}

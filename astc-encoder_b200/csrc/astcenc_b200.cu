@@ -287,9 +287,31 @@ astc_decompress_block_lists_kernel(const __grid_constant__ DevBsd bsd, const __g
 
 __global__ void __launch_bounds__(32, 1)
 astc_block_info_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
-                       unsigned long long lo, unsigned long long hi, DevBlockInfo* out) {
+                       unsigned long long lo, unsigned long long hi, const __grid_constant__ BlockInfoHead head, astcenc_block_info* out) {
 	stage_launch_constants(bsd, cfg, img);
-	block_info(threadIdx.x & 31, ASTC_SMEM_HDR, lo, hi, out);
+	block_info(threadIdx.x & 31, ASTC_SMEM_HDR, lo, hi, head, out);
+}
+
+// ---- block info of device payloads (astc_dev_gather.cuh): summaries one thread per block, grid-stride; list structs one warp
+// per slot, grid-stride ----
+#define ASTC_SUMMARY_THREADS 256
+__global__ void __launch_bounds__(ASTC_SUMMARY_THREADS)
+astc_block_summaries_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
+                            const GatherImage* __restrict__ images, unsigned int image_count, size_t total) {
+	stage_launch_constants(bsd, cfg, img);
+	summarize_table_blocks(images, image_count, (size_t)blockIdx.x * blockDim.x + threadIdx.x, total, (size_t)gridDim.x * blockDim.x);
+}
+
+#define ASTC_INFO_LIST_THREADS 256
+__global__ void __launch_bounds__(ASTC_INFO_LIST_THREADS)
+astc_block_info_lists_kernel(const __grid_constant__ DevBsd bsd, const __grid_constant__ DevConfig cfg, const __grid_constant__ DevImage img,
+                             const GatherImage* __restrict__ images, const GatherList* __restrict__ lists, unsigned int image_count, size_t total,
+                             const __grid_constant__ BlockInfoHead head) {
+	stage_launch_constants(bsd, cfg, img);
+	const unsigned int warps = blockDim.x >> 5, warp = threadIdx.x >> 5;
+	for (size_t c = (size_t)blockIdx.x * warps + warp; c < total; c += (size_t)gridDim.x * warps) {
+		info_list_slot(images, lists, image_count, c, (int)(threadIdx.x & 31), ASTC_SMEM_HDR + warp * D_SLICE, head);
+	}
 }
 
 // ---- the single-kernel drivers (kept for A/B measurements: ASTCENC_B200_DRIVER=lockstep|warp) ----
@@ -1500,28 +1522,34 @@ astcenc_error astcenc_decompress_reset(astcenc_context* ctx) {
 	return ASTCENC_SUCCESS;
 }
 
-// astcenc_get_block_info (astcenc_entry.cpp:1401-1517). A query for tools: one 32-thread launch per call.
+// The fields of astcenc_block_info that come from the context.
+static BlockInfoHead block_info_head(const astcenc_context* ctx) {
+	return {(int)ctx->config.profile, ctx->config.block_x, ctx->config.block_y, ctx->config.block_z, ctx->tables->bsd.texel_count};
+}
+
+// astcenc_get_block_info (astcenc_entry.cpp:1401-1517). A query for tools: one 32-thread launch per call, which writes the whole
+// struct (block_info, astc_dev_decode.cuh).
 astcenc_error astcenc_get_block_info(astcenc_context* ctx, const uint8_t data[16], astcenc_block_info* info) {
 	memset(info, 0, sizeof(*info));
+	const BlockInfoHead head = block_info_head(ctx);
 	info->profile = ctx->config.profile;
-	info->block_x = ctx->config.block_x;
-	info->block_y = ctx->config.block_y;
-	info->block_z = ctx->config.block_z;
-	info->texel_count = ctx->tables->bsd.texel_count;
+	info->block_x = head.block_x;
+	info->block_y = head.block_y;
+	info->block_z = head.block_z;
+	info->texel_count = head.texel_count;
 	DeviceGuard guard(ctx->device);
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	DevBlockInfo* d_info = nullptr;
-	CUDA_TRY(cudaMalloc(&d_info, sizeof(DevBlockInfo)), return ASTCENC_ERR_OUT_OF_MEM);
-	cudaMemsetAsync(d_info, 0, sizeof(DevBlockInfo), ctx->stream);
+	astcenc_block_info* d_info = nullptr;
+	CUDA_TRY(cudaMalloc(&d_info, sizeof(astcenc_block_info)), return ASTCENC_ERR_OUT_OF_MEM);
 	unsigned long long lo, hi;
 	memcpy(&lo, data, 8);
 	memcpy(&hi, data + 8, 8);
 	DevImage img{};
-	astc_block_info_kernel<<<1, 32, ASTC_SMEM_HDR + D_SLICE, ctx->stream>>>(ctx->tables->bsd, ctx->dcfg, img, lo, hi, d_info);
+	astc_block_info_kernel<<<1, 32, ASTC_SMEM_HDR + D_SLICE, ctx->stream>>>(ctx->tables->bsd, ctx->dcfg, img, lo, hi, head, d_info);
 	ctx->launches++;
-	DevBlockInfo h;
+	astcenc_block_info h;
 	cudaError_t e = cudaMemcpyAsync(&h, d_info, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream);
 	if (e == cudaSuccess) {
 		e = cudaStreamSynchronize(ctx->stream);
@@ -1530,35 +1558,7 @@ astcenc_error astcenc_get_block_info(astcenc_context* ctx, const uint8_t data[16
 	if (e != cudaSuccess) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	info->is_error_block = h.is_error_block != 0;
-	if (info->is_error_block) {
-		return ASTCENC_SUCCESS;
-	}
-	info->is_constant_block = h.is_constant_block != 0;
-	if (info->is_constant_block) {
-		return ASTCENC_SUCCESS;
-	}
-	info->is_hdr_block = h.is_hdr_block != 0;
-	info->is_dual_plane_block = h.is_dual_plane_block != 0;
-	info->partition_count = h.partition_count;
-	info->partition_index = h.partition_index;
-	info->dual_plane_component = h.dual_plane_component;
-	info->color_level_count = h.color_level_count;
-	info->weight_level_count = h.weight_level_count;
-	info->weight_x = h.weight_x;
-	info->weight_y = h.weight_y;
-	info->weight_z = h.weight_z;
-	for (unsigned int p = 0; p < h.partition_count && p < 4; p++) {
-		info->color_endpoint_modes[p] = h.color_endpoint_modes[p];
-		memcpy(info->color_endpoints[p], h.color_endpoints[p], sizeof(h.color_endpoints[p]));
-	}
-	for (unsigned int i = 0; i < info->texel_count; i++) {
-		info->weight_values_plane1[i] = h.weight_values_plane1[i];
-		if (info->is_dual_plane_block) {
-			info->weight_values_plane2[i] = h.weight_values_plane2[i];
-		}
-		info->partition_assignment[i] = h.partition_assignment[i];
-	}
+	memcpy(info, &h, sizeof(h));
 	return ASTCENC_SUCCESS;
 }
 
@@ -2768,3 +2768,112 @@ astcenc_error astcenc_b200_last_timing(astcenc_context* ctx, float* kernel_ms, s
 }
 
 }  // extern "C"
+
+// Block info calls (astc_dev_gather.cuh): the image table of astcenc_b200_decompress_device_images, checked whole before anything
+// is enqueued, in the order include/astcenc.h gives; table_entry gives the block counts. The table (and a list call's lists)
+// go up in one copy and one launch does the call, in one scratch turn.
+static astcenc_error launch_block_info_table(astcenc_context* ctx, const std::vector<GatherImage>& table, const std::vector<GatherList>& lists, size_t total,
+                                             cudaStream_t s) {
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	return scratch_turn(ctx, s, [&]() -> astcenc_error {
+		const size_t table_bytes = table.size() * sizeof(GatherImage);
+		const size_t lists_bytes = lists.size() * sizeof(GatherList);
+		astcenc_error r = ensure_buffer(ctx->list, table_bytes + lists_bytes);
+		if (r != ASTCENC_SUCCESS) {
+			return r;
+		}
+		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
+		up.insert(up.end(), reinterpret_cast<const uint8_t*>(lists.data()), reinterpret_cast<const uint8_t*>(lists.data()) + lists_bytes);
+		// (from pageable memory: staged by the driver before the call returns)
+		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
+		const DevImage img{};
+		if (lists.empty()) {
+			const size_t ctas = (total + ASTC_SUMMARY_THREADS - 1) / ASTC_SUMMARY_THREADS;
+			const size_t cap = (size_t)ctx->sm_count * (2048 / ASTC_SUMMARY_THREADS);
+			astc_block_summaries_kernel<<<(unsigned int)(ctas < cap ? ctas : cap), ASTC_SUMMARY_THREADS, ASTC_SMEM_HDR, s>>>(
+			    ctx->tables->bsd, ctx->dcfg, img, ctx->list.as<const GatherImage>(), (unsigned int)table.size(), total);
+		} else {
+			const unsigned int warps = ASTC_INFO_LIST_THREADS / 32;
+			const size_t ctas = (total + warps - 1) / warps;
+			const size_t cap = (size_t)ctx->sm_count * 8;
+			astc_block_info_lists_kernel<<<(unsigned int)(ctas < cap ? ctas : cap), ASTC_INFO_LIST_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, s>>>(
+			    ctx->tables->bsd, ctx->dcfg, img, ctx->list.as<const GatherImage>(), reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes),
+			    (unsigned int)table.size(), total, block_info_head(ctx));
+		}
+		ctx->launches++;
+		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
+		return ASTCENC_SUCCESS;
+	});
+}
+
+static bool aligned_to(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+astcenc_error astcenc_b200_get_block_summaries_device_images(astcenc_context* ctx, const astcenc_b200_device_block_summary_image* images,
+                                                             unsigned int image_count, void* cuda_stream) {
+	if (!ctx || (image_count != 0 && !images)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	for (unsigned int i = 0; i < image_count; i++) {
+		const astcenc_b200_device_block_summary_image& im = images[i];
+		if (!im.payload || !im.summaries || !aligned_to(im.summaries, 16) || check_texel_count(im.dim_x, im.dim_y, im.dim_z) != ASTCENC_SUCCESS) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+	}
+	std::vector<GatherImage> table(image_count);
+	size_t blocks = 0;
+	for (unsigned int i = 0; i < image_count; i++) {
+		const astcenc_b200_device_block_summary_image& im = images[i];
+		// (the payload is read, never written; data holds the summaries)
+		const astcenc_error status = table_entry(ctx, ASTCENC_TYPE_U8, im.dim_x, im.dim_y, im.dim_z, im.summaries, const_cast<uint8_t*>(im.payload), blocks, table[i]);
+		if (status != ASTCENC_SUCCESS) {
+			return status;
+		}
+	}
+	if (blocks == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	return launch_block_info_table(ctx, table, {}, blocks, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream);
+}
+
+astcenc_error astcenc_b200_get_block_info_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_info_list* lists, unsigned int list_count,
+                                                             void* cuda_stream) {
+	if (!ctx || (list_count != 0 && !lists)) {
+		return ASTCENC_ERR_BAD_PARAM;
+	}
+	for (unsigned int i = 0; i < list_count; i++) {
+		const astcenc_b200_device_block_info_list& l = lists[i];
+		if (!l.payload || (l.capacity != 0 && (!l.indices || !l.count || !l.infos)) || !aligned_to(l.indices, 4) || !aligned_to(l.count, 4) ||
+		    !aligned_to(l.infos, 4) || check_texel_count(l.dim_x, l.dim_y, l.dim_z) != ASTCENC_SUCCESS) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+	}
+	std::vector<GatherImage> table;
+	std::vector<GatherList> gather_lists;
+	size_t slots = 0;
+	for (unsigned int i = 0; i < list_count; i++) {
+		const astcenc_b200_device_block_info_list& l = lists[i];
+		GatherImage e;
+		size_t blocks = 0;
+		// (the payload is read, never written; data holds the structs)
+		astcenc_error status = table_entry(ctx, ASTCENC_TYPE_U8, l.dim_x, l.dim_y, l.dim_z, l.infos, const_cast<uint8_t*>(l.payload), blocks, e);
+		if (status == ASTCENC_SUCCESS && l.capacity > SIZE_MAX - slots) {
+			status = ASTCENC_ERR_BAD_PARAM;
+		}
+		if (status != ASTCENC_SUCCESS) {
+			return status;
+		}
+		if (l.capacity != 0) {
+			e.first = slots;
+			table.push_back(e);
+			gather_lists.push_back({l.indices, l.count, l.capacity, (unsigned int)blocks});
+			slots += l.capacity;
+		}
+	}
+	if (slots == 0) {
+		return ASTCENC_SUCCESS;
+	}
+	return launch_block_info_table(ctx, table, gather_lists, slots, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream);
+}

@@ -796,6 +796,78 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_total_block_maps(struct astcenc_c
                                                                 unsigned int entry_count, enum astcenc_b200_weight_rule rule, void* cuda_stream);
 
 /**
+ * Block info of device-resident payloads on the device: what astcenc_get_block_info reports, for whole payloads or for the
+ * blocks of device lists, without copying a block to the host. For callers who want to see what a refinement round did to an
+ * encoding (which blocks now use two partitions or dual planes, which are constant, which weight grids a mip chain's small
+ * levels use), or whether a payload loaded from a file holds error blocks, and where, before it is decoded or shipped.
+ *
+ * astcenc_b200_get_block_summaries_device_images: a 16-byte summary of every block of whole payloads.
+ * images[i] describes a payload ALREADY RESIDENT in device memory (astcenc_compress_image's block order, 16 bytes per block, of
+ * an image of dim_x * dim_y * dim_z texels in the context's footprint) and a device array of one summary per block, in the
+ * same order. Every field of summaries[b] equals the same-named field astcenc_get_block_info on this context writes for block
+ * b's 16 bytes, narrowed to the field's width (every value fits): flags holds its four is_* fields as the bits below, and
+ * dual_plane_component is 0xFF where astcenc_get_block_info reports 0xFFFFFFFF (a block with one plane). An error or constant
+ * block therefore gets its flag and zeros, as astcenc_get_block_info returns early for them. reserved is written as 0.
+ *
+ * astcenc_b200_get_block_info_device_block_lists: the full astcenc_block_info of the blocks of device lists, for drilling into
+ * the blocks a selection picked. lists[i] describes a payload ALREADY RESIDENT in device memory, a device index list with a
+ * device count, and a device array of capacity structs. The list rule is that of astcenc_b200_decompress_device_block_lists:
+ * the call reads the first min(*count, capacity) slots, and a slot whose index is at or beyond the image's block count is
+ * skipped. The output is indexed by slot, not by block: each read slot s receives in infos[s], byte for byte, the whole struct
+ * astcenc_get_block_info on this context writes for block indices[s], its zeros included. Skipped slots and slots past the
+ * count are left untouched; duplicate indices write the same bytes.
+ *
+ * Both calls:
+ * - Take 2D images, texture arrays (2D block sizes; z counts the slices) and volumes of 3D block sizes, and work on
+ *   decompress-only contexts. Outputs must not overlap each other or any payload (not checked).
+ * - Are enqueued on `cuda_stream` (0 = the context's own stream) without synchronising, in order with every other pass of the
+ *   context: the counts and the indices are read on the device when the call runs. The descriptor array is copied.
+ * - Cost one table copy and one kernel launch (one lane per block for summaries, one warp per slot for lists, over the sum of
+ *   the capacities). A call with nothing to do (no images, or capacities all zero) launches nothing.
+ * - Errors, in this order; on error nothing is launched and nothing is written:
+ *     1. ASTCENC_ERR_BAD_PARAM for a NULL context;
+ *     2. ASTCENC_ERR_BAD_PARAM for a NULL table with a non-zero count;
+ *     3. ASTCENC_ERR_BAD_PARAM for an entry with a NULL payload or output (summaries; for lists, infos, indices or count with
+ *        capacity > 0), or an output not aligned: summaries to 16 bytes, indices, count and infos to 4;
+ *     4. ASTCENC_ERR_BAD_PARAM for a zero or overflowing dimension;
+ *     5. ASTCENC_ERR_BAD_PARAM for an image of 2^32 blocks or more, or a call whose block or slot total overflows.
+ *   Every entry is checked before anything is enqueued.
+ */
+static const unsigned int ASTCENC_B200_BLOCK_IS_ERROR = 1, ASTCENC_B200_BLOCK_IS_CONSTANT = 2, ASTCENC_B200_BLOCK_IS_HDR = 4,
+                          ASTCENC_B200_BLOCK_IS_DUAL_PLANE = 8;
+struct astcenc_b200_block_summary {    /* 16 bytes */
+	uint8_t flags;                     /* ASTCENC_B200_BLOCK_IS_* */
+	uint8_t partition_count;
+	uint16_t partition_index;
+	uint8_t dual_plane_component;      /* 0xFF for a block with one plane */
+	uint8_t weight_x, weight_y, weight_z;
+	uint8_t color_endpoint_modes[4];
+	uint16_t color_level_count;
+	uint8_t weight_level_count;
+	uint8_t reserved;                  /* written as 0 */
+};
+struct astcenc_b200_device_block_summary_image {
+	const uint8_t* payload;            /* device: the whole payload, astcenc_compress_image's block order */
+	unsigned int dim_x, dim_y, dim_z;
+	struct astcenc_b200_block_summary* summaries;   /* device: one per block, same order; 16-byte aligned */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_get_block_summaries_device_images(struct astcenc_context* context,
+                                                                                 const struct astcenc_b200_device_block_summary_image* images,
+                                                                                 unsigned int image_count, void* cuda_stream);
+
+struct astcenc_b200_device_block_info_list {
+	const uint8_t* payload;            /* device: the whole payload, astcenc_compress_image's block order */
+	unsigned int dim_x, dim_y, dim_z;
+	const uint32_t* indices;           /* device: block positions in that order */
+	const uint32_t* count;             /* device: how many are listed */
+	unsigned int capacity;             /* at most this many are read; the call's cost */
+	struct astcenc_block_info* infos;  /* device: capacity structs; slot s describes block indices[s] */
+};
+ASTCENC_PUBLIC enum astcenc_error astcenc_b200_get_block_info_device_block_lists(struct astcenc_context* context,
+                                                                                 const struct astcenc_b200_device_block_info_list* lists,
+                                                                                 unsigned int list_count, void* cuda_stream);
+
+/**
  * The .astc container (Docs/FileFormat.md; Source/astcenccli_image_load_store.cpp:2573-2760, load_cimage / store_cimage):
  * a 16-byte header - magic 13 AB A1 5C, block dimensions (one byte each), image dimensions (24 bits each, little endian)
  * - followed by the blocks as astcenc_compress_image() wrote them.

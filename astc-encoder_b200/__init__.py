@@ -30,6 +30,8 @@ ERROR_NAMES = ["ASTCENC_SUCCESS", "ASTCENC_ERR_OUT_OF_MEM", "ASTCENC_ERR_BAD_CPU
 ERR_OUT_OF_MEM, ERR_BAD_PARAM, ERR_BAD_BLOCK_SIZE, ERR_BAD_SWIZZLE, ERR_BAD_CONTEXT, ERR_NOT_IMPLEMENTED = 1, 3, 4, 7, 9, 10
 # enum astcenc_b200_block_metric: what a per-block error map measures
 BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR, BLOCK_LOG2_ERROR = 0, 1, 2
+# normal maps: the sum of each texel's angle in degrees, and the largest one (3 is not assigned)
+BLOCK_ANGULAR_ERROR, BLOCK_WORST_ANGULAR_ERROR = 4, 5
 # enum astcenc_b200_weight_rule: the selection weight of an image that misses its target
 WEIGHT_ONE, WEIGHT_INVERSE_TOTAL = 0, 1
 # the flags of struct astcenc_b200_block_summary
@@ -571,8 +573,11 @@ class Context:
     def compute_block_metric_device_images(self, images, block_metric, hdr=False, normal=False, input_components=4, fstop_lo=-10, fstop_hi=10,
                                            stream=0):
         """compute_error_metrics_device_images with maps of `block_metric` (astcenc_b200_compute_block_metric_device_images):
-        BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR (each block's share of alpha_psnr's error sum) or BLOCK_LOG2_ERROR (each
-        block's share of log_rmse's). Same tuples, same figures; enqueued on `stream`, no sync."""
+        BLOCK_SQUARED_ERROR, BLOCK_ALPHA_WEIGHTED_ERROR (each block's share of alpha_psnr's error sum), BLOCK_LOG2_ERROR (each
+        block's share of log_rmse's), BLOCK_ANGULAR_ERROR (the sum of its texels' normal angles in degrees: the block's share of
+        mean_angular_error times the pixel count) or BLOCK_WORST_ANGULAR_ERROR (its largest texel angle: the map's maximum is
+        worst_angular_error). The angular maps read RGB whatever input_components is and need no `normal`. Same tuples, same
+        figures; enqueued on `stream`, no sync."""
         n = len(images)
         table = _metrics_table(images)
         err = lib().astcenc_b200_compute_block_metric_device_images(self.handle, int(hdr), int(normal), input_components, block_metric, table if n else None,
@@ -694,7 +699,7 @@ class Context:
     def compute_block_metric_device_block_lists(self, lists, block_metric, input_components=4, stream=0):
         """compute_block_errors_device_block_lists for maps of `block_metric` (astcenc_b200_compute_block_metric_device_block_lists):
         each listed map value receives what compute_block_metric_device_images writes for that block with the same metric, and no
-        other value changes. Same tuples; enqueued on `stream`, no sync."""
+        other value changes; any metric compute_block_metric_device_images takes. Same tuples; enqueued on `stream`, no sync."""
         n = len(lists)
         table = _block_error_list_table(lists)
         err = lib().astcenc_b200_compute_block_metric_device_block_lists(self.handle, input_components, block_metric, table if n else None, n,
@@ -709,7 +714,9 @@ class Context:
         d_decoded_ptr or 0, d_block_error_ptr, d_indices_ptr, d_count_ptr, capacity). For the first min(*count, capacity) indices
         in range, the candidate (what compress_device_block_lists would write) is decoded by this context to decoded_type with
         decode_swizzle and measured in block_metric over input_components; where that value is below the map's, the payload
-        bytes, the decoded texels and the map value are replaced. Enqueued on `stream`, no sync."""
+        bytes, the decoded texels and the map value are replaced. block_metric is any metric of compute_block_metric_device_images;
+        for a normal map encoded with the rrrg swizzle, decode with decode_swizzle (0, 3, 6, 5), (R, A, Z, 1), and measure in
+        BLOCK_ANGULAR_ERROR or BLOCK_WORST_ANGULAR_ERROR. Enqueued on `stream`, no sync."""
         n = len(lists)
         table = (DeviceRefineList * n)(*[DeviceRefineList(C.c_void_p(p), x, y, z, C.c_void_p(q), C.c_void_p(d or None), C.c_void_p(b or None),
                                                           C.c_void_p(i or None), C.c_void_p(k or None), c)

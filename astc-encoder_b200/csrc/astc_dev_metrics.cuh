@@ -18,7 +18,7 @@
 // block order; it compiles for the host simulation too (tests/hostsim/hostsim_metrics.cpp). A list refresh
 // (astcenc_b200_compute_block_errors_device_block_lists) runs the same function at the slots of device block lists, one warp per
 // slot (tests/hostsim/hostsim_map_lists.cpp). A map measures one enum astcenc_b200_block_metric (metric_block_terms): the
-// squared error on astc_block_error_kernel / astc_block_error_lists_kernel, the alpha-weighted and log2 errors on
+// squared error on astc_block_error_kernel / astc_block_error_lists_kernel, the alpha-weighted, log2 and angular errors on
 // astc_block_metric_kernel<M> / astc_block_metric_lists_kernel<M>, all through block_error_sum<M>.
 #pragma once
 #include <vector>
@@ -227,21 +227,57 @@ ASTC_FN float metric_log2(float x) {
 	return p + e;
 }
 
+// (c - 0.5) * 2, normalize_safe(xyz, unit3) (:269-275; astcenc_vecmathlib.h:362-371), dot in DPPS order; w is 0
+ASTC_FN f4 metric_normal(f4 c) {
+	float x = (c.x - 0.5f) * 2.0f, y = (c.y - 0.5f) * 2.0f, z = (c.z - 0.5f) * 2.0f;
+	float len = (x * x + y * y) + (z * z + 0.0f);
+	if (len != 0.0f) {
+		float s = sqrtf(len);
+		return mk4(x / s, y / s, z / s, 0.0f);
+	}
+	float u = 0.57735026918962576451f;      // unit3()
+	return mk4(u, u, u, 0.0f);
+}
+
+// The angle in degrees between the normals of the RGB of c1 and c2 (:276-281): the float dot product in DPPS order clamped to
+// [-1, 1] (a NaN dot gives -1: 180 degrees), acos in double. The per-texel term of mean_angular_error and worst_angular_error.
+ASTC_FN double metric_angle(f4 c1, f4 c2) {
+	f4 n1 = metric_normal(c1);
+	f4 n2 = metric_normal(c2);
+	float d = (n1.x * n2.x + n1.y * n2.y) + (n1.z * n2.z + 0.0f);
+	d = fminf(fmaxf(d, -1.0f), 1.0f);
+	float rad_to_degrees = 180.0f / 3.14159265358979323846f;
+	return acos((double)d) * (double)rad_to_degrees;
+}
+
 // ---- the per-block error map ----
 
+// How a map of metric M combines its terms, within a lane and across lanes: the largest for WORST_ANGULAR_ERROR (fmax does not
+// depend on the order), the double sum for every other metric.
+template <int M>
+ASTC_FN double metric_combine(double acc, double term) {
+	return M == ASTCENC_B200_BLOCK_WORST_ANGULAR_ERROR ? fmax(acc, term) : acc + term;
+}
+
 // The terms of one texel of a map of metric M (enum astcenc_b200_block_metric) over the channels in `mask`, c1 the original and
-// c2 the decoded texel, added to acc in channel order. Each term is a float square of float values, added in double:
+// c2 the decoded texel, combined into acc (metric_combine) in channel order. Each term but the angle is a float square of float
+// values, combined in double:
 //   SQUARED_ERROR         (c1 - c2)^2 per channel, the MS_ERR terms of the sums
 //   ALPHA_WEIGHTED_ERROR  ((c1 - c2) * c1.w)^2 per RGB channel and (c1.w - c2.w)^2 for alpha, the MS_AERR terms
 //   LOG2_ERROR            (log2(c1) - log2(c2))^2 per RGB channel, the MS_LOG terms
+//   ANGULAR_ERROR and WORST_ANGULAR_ERROR  metric_angle of the RGB whatever the mask, the MS_ANG_MEAN / MS_ANG_WORST term
 template <int M>
 ASTC_FN void metric_block_terms(const f4& c1, const f4& c2, int mask, double& acc) {
+	if (M == ASTCENC_B200_BLOCK_ANGULAR_ERROR || M == ASTCENC_B200_BLOCK_WORST_ANGULAR_ERROR) {
+		acc = metric_combine<M>(acc, metric_angle(c1, c2));
+		return;
+	}
 	if (M == ASTCENC_B200_BLOCK_LOG2_ERROR) {
 		const float o[3] = {c1.x, c1.y, c1.z}, q[3] = {c2.x, c2.y, c2.z};
 		for (int k = 0; k < 3; k++) {
 			if (mask & (1 << k)) {
 				const float l = metric_log2(o[k]) - metric_log2(q[k]);
-				acc += (double)(l * l);
+				acc = metric_combine<M>(acc, (double)(l * l));
 			}
 		}
 		return;
@@ -250,17 +286,18 @@ ASTC_FN void metric_block_terms(const f4& c1, const f4& c2, int mask, double& ac
 	for (int k = 0; k < 4; k++) {
 		if (mask & (1 << k)) {
 			const float v = M == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR && k < 3 ? d[k] * c1.w : d[k];
-			acc += (double)(v * v);
+			acc = metric_combine<M>(acc, (double)(v * v));
 		}
 	}
 }
 
 // Map block `index` of entry e (astcenc_compress_image's block order for the footprint bx x by x bz; a 2D footprint's index
-// counts the slices of a texture array), by `lanes` lanes of one warp, against the decoded texels `decoded` gives: the sum, over
-// the block's texels inside the image, of the terms of metric M (metric_block_terms) of the channels in `mask`, added in double.
-// decoded(t, x, y, z) is the decoded texel of footprint texel t at image position (x, y, z). Lane l takes texels l, l + lanes, ...
-// in footprint order, then the lanes are summed in a fixed xor-shuffle order. Every lane returns the sum. So a value depends on
-// where the decoded texels live only through what `decoded` returns.
+// counts the slices of a texture array), by `lanes` lanes of one warp, against the decoded texels `decoded` gives: the terms of
+// metric M (metric_block_terms) of the channels in `mask` over the block's texels inside the image, combined in double
+// (metric_combine: a sum, or the largest for WORST_ANGULAR_ERROR). decoded(t, x, y, z) is the decoded texel of footprint texel t
+// at image position (x, y, z). Lane l takes texels l, l + lanes, ... in footprint order, then the lanes are combined in a fixed
+// xor-shuffle order. Every lane returns the value. So a value depends on where the decoded texels live only through what
+// `decoded` returns.
 template <int M, typename Decoded>
 ASTC_FN double block_error_sum_of(const MetricEntry& e, unsigned int bx, unsigned int by, unsigned int bz, uint32_t index, int mask, int lane, int lanes,
                                   const Decoded& decoded) {
@@ -277,7 +314,7 @@ ASTC_FN double block_error_sum_of(const MetricEntry& e, unsigned int bx, unsigne
 	}
 #if !defined(ASTC_ONE_LANE)
 	for (int o = lanes / 2; o > 0; o >>= 1) {
-		acc += __shfl_xor_sync(0xffffffffu, acc, o);
+		acc = metric_combine<M>(acc, __shfl_xor_sync(0xffffffffu, acc, o));
 	}
 #endif
 	return acc;
@@ -370,18 +407,6 @@ static __device__ __forceinline__ float metric_mpsnr_sumdiff(float v1, float v2,
 	return summa;
 }
 
-// (c - 0.5) * 2, normalize_safe(xyz, unit3) (:269-275; astcenc_vecmathlib.h:362-371), dot in DPPS order
-static __device__ __forceinline__ float3 metric_normal(f4 c) {
-	float x = (c.x - 0.5f) * 2.0f, y = (c.y - 0.5f) * 2.0f, z = (c.z - 0.5f) * 2.0f;
-	float len = (x * x + y * y) + (z * z + 0.0f);
-	if (len != 0.0f) {
-		float s = sqrtf(len);
-		return make_float3(x / s, y / s, z / s);
-	}
-	float u = 0.57735026918962576451f;      // unit3()
-	return make_float3(u, u, u);
-}
-
 // CTA b of the launch is virtual CTA b - first of its entry: slice z, CTA v of that slice's `ctas`.
 __global__ void __launch_bounds__(ASTC_METRIC_THREADS)
 astc_error_metrics_kernel(const __grid_constant__ MetricArgs a) {
@@ -428,12 +453,7 @@ astc_error_metrics_kernel(const __grid_constant__ MetricArgs a) {
 			acc[MS_MPSNR + 2] += (double)metric_mpsnr_sumdiff(c1.z, c2.z, a.fstop_lo, a.fstop_hi);
 		}
 		if (a.normal) {
-			float3 n1 = metric_normal(c1);
-			float3 n2 = metric_normal(c2);
-			float d = (n1.x * n2.x + n1.y * n2.y) + (n1.z * n2.z + 0.0f);
-			d = fminf(fmaxf(d, -1.0f), 1.0f);
-			float rad_to_degrees = 180.0f / 3.14159265358979323846f;
-			double deg = acos((double)d) * (double)rad_to_degrees;
+			double deg = metric_angle(c1, c2);
 			acc[MS_ANG_MEAN] += deg * inv_pixels;
 			acc[MS_ANG_WORST] = fmax(acc[MS_ANG_WORST], deg);
 		}
@@ -514,7 +534,7 @@ astc_block_error_kernel(const __grid_constant__ MetricArgs a) {
 	block_map_warp<ASTCENC_B200_BLOCK_SQUARED_ERROR>(a);
 }
 
-// The maps of the other metrics: one instantiation each (ALPHA_WEIGHTED_ERROR, LOG2_ERROR).
+// The maps of the other metrics: one instantiation each (ALPHA_WEIGHTED_ERROR, LOG2_ERROR, ANGULAR_ERROR, WORST_ANGULAR_ERROR).
 template <int M>
 __global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
 astc_block_metric_kernel(const __grid_constant__ MetricArgs a) {
@@ -530,7 +550,7 @@ astc_block_error_lists_kernel(const __grid_constant__ MetricListArgs a) {
 	}
 }
 
-// A list refresh of maps of metric M (ALPHA_WEIGHTED_ERROR, LOG2_ERROR).
+// A list refresh of maps of metric M (every metric but SQUARED_ERROR).
 template <int M>
 __global__ void __launch_bounds__(ASTC_METRIC_MAP_WARPS * 32)
 astc_block_metric_lists_kernel(const __grid_constant__ MetricListArgs a) {

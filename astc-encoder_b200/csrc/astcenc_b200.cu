@@ -19,6 +19,7 @@
 #include <new>
 #include <thread>
 #include <chrono>
+#include <type_traits>
 
 #include "astc_dev_search.cuh"
 #include "astc_dev_gather.cuh"
@@ -583,6 +584,21 @@ static void release_tables(DeviceTables* t) {
 		cudaFree(t->d_blob);
 		astc_host::free_block_size_tables(t->host_tables);
 		delete t;
+	}
+}
+
+// The metrics a map may measure (enum astcenc_b200_block_metric), in one place: with_block_metric runs
+// f(std::integral_constant<int, M>()) for block_metric's M and returns true, or returns false and runs nothing for any other
+// value (it arrives through the C ABI as any int). Every launch site that picks a kernel by metric goes through it.
+template <class F>
+static bool with_block_metric(int block_metric, F&& f) {
+	switch (block_metric) {
+	case ASTCENC_B200_BLOCK_SQUARED_ERROR: f(std::integral_constant<int, ASTCENC_B200_BLOCK_SQUARED_ERROR>()); return true;
+	case ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR: f(std::integral_constant<int, ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR>()); return true;
+	case ASTCENC_B200_BLOCK_LOG2_ERROR: f(std::integral_constant<int, ASTCENC_B200_BLOCK_LOG2_ERROR>()); return true;
+	case ASTCENC_B200_BLOCK_ANGULAR_ERROR: f(std::integral_constant<int, ASTCENC_B200_BLOCK_ANGULAR_ERROR>()); return true;
+	case ASTCENC_B200_BLOCK_WORST_ANGULAR_ERROR: f(std::integral_constant<int, ASTCENC_B200_BLOCK_WORST_ANGULAR_ERROR>()); return true;
+	default: return false;
 	}
 }
 
@@ -1562,6 +1578,11 @@ astcenc_error astcenc_get_block_info(astcenc_context* ctx, const uint8_t data[16
 	return ASTCENC_SUCCESS;
 }
 
+// A map's metric is one of those with_block_metric runs.
+static bool check_block_metric(astcenc_b200_block_metric block_metric) {
+	return with_block_metric((int)block_metric, [](auto) {});
+}
+
 // One metrics call of a planned table (plan_metrics) on `stream`, inside a scratch turn: the table and the map list go up into
 // the context's table buffer (ctx->list) in one copy, the metrics kernel and the finish kernel run, then the map kernel of
 // block_metric when an entry asks for a map. The sums of entry j are left at ctx->metric_partials + (plan.ctas + j) * ASTC_METRIC_SUMS doubles.
@@ -1603,13 +1624,13 @@ static astcenc_error launch_metrics(astcenc_context* ctx, const std::vector<Metr
 	ctx->launches++;
 	if (plan.map_grid != 0) {
 		const dim3 grid(plan.map_grid), cta(ASTC_METRIC_MAP_WARPS * 32);
-		if (block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
-			astc_block_metric_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, cta, 0, stream>>>(a);
-		} else if (block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
-			astc_block_metric_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, cta, 0, stream>>>(a);
-		} else {
-			astc_block_error_kernel<<<grid, cta, 0, stream>>>(a);
-		}
+		with_block_metric(block_metric, [&](auto m) {
+			if constexpr (decltype(m)::value == ASTCENC_B200_BLOCK_SQUARED_ERROR) {
+				astc_block_error_kernel<<<grid, cta, 0, stream>>>(a);
+			} else {
+				astc_block_metric_kernel<decltype(m)::value><<<grid, cta, 0, stream>>>(a);
+			}
+		});
 		ctx->launches++;
 	}
 	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
@@ -1922,22 +1943,14 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 			enqueue_decode(ctx, d_rows + (m == chunk ? 0 : 1), 1, m, call.refine.decoded_type, call.refine.decode_swizzle, stream);
 			const unsigned int grid = (m + ASTC_REFINE_LIST_WARPS - 1) / ASTC_REFINE_LIST_WARPS;
 			if (call.packed) {
-				if (call.refine.block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
-					astc_refine_decide_packed_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-				} else if (call.refine.block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
-					astc_refine_decide_packed_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-				} else {
-					astc_refine_decide_packed_kernel<ASTCENC_B200_BLOCK_SQUARED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-				}
+				with_block_metric(call.refine.block_metric, [&](auto mt) {
+					astc_refine_decide_packed_kernel<decltype(mt)::value><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				});
 				astc_refine_commit_packed_kernel<<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(ctx->list_out.ptr, g, r);
 			} else {
-				if (call.refine.block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
-					astc_refine_decide_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-				} else if (call.refine.block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
-					astc_refine_decide_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-				} else {
-					astc_refine_decide_kernel<ASTCENC_B200_BLOCK_SQUARED_ERROR><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
-				}
+				with_block_metric(call.refine.block_metric, [&](auto mt) {
+					astc_refine_decide_kernel<decltype(mt)::value><<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(g, r);
+				});
 				astc_refine_commit_kernel<<<grid, ASTC_REFINE_LIST_WARPS * 32, 0, stream>>>(ctx->list_out.ptr, g, r);
 			}
 			ctx->launches += 2;
@@ -2156,12 +2169,6 @@ astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const 
 	}
 	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
 	return scratch_turn(ctx, s, [&] { return launch_decode(ctx, table.data(), image_count, blocks, (int)data_type, *swizzle, s); });
-}
-
-// A map's metric is one of enum astcenc_b200_block_metric (the value arrives through the C ABI as any int).
-static bool check_block_metric(astcenc_b200_block_metric block_metric) {
-	const int m = (int)block_metric;
-	return m >= ASTCENC_B200_BLOCK_SQUARED_ERROR && m <= ASTCENC_B200_BLOCK_LOG2_ERROR;
 }
 
 // Metrics calls: every pair is checked before anything is enqueued; the table goes up in one copy and the call is two
@@ -2519,13 +2526,13 @@ astcenc_error astcenc_b200_compute_block_metric_device_block_lists(astcenc_conte
 		a.bz = bz;
 		a.components = input_components;
 		const dim3 grid(plan.grid), cta(ASTC_METRIC_MAP_WARPS * 32);
-		if (block_metric == ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR) {
-			astc_block_metric_lists_kernel<ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR><<<grid, cta, 0, s>>>(a);
-		} else if (block_metric == ASTCENC_B200_BLOCK_LOG2_ERROR) {
-			astc_block_metric_lists_kernel<ASTCENC_B200_BLOCK_LOG2_ERROR><<<grid, cta, 0, s>>>(a);
-		} else {
-			astc_block_error_lists_kernel<<<grid, cta, 0, s>>>(a);
-		}
+		with_block_metric(block_metric, [&](auto m) {
+			if constexpr (decltype(m)::value == ASTCENC_B200_BLOCK_SQUARED_ERROR) {
+				astc_block_error_lists_kernel<<<grid, cta, 0, s>>>(a);
+			} else {
+				astc_block_metric_lists_kernel<decltype(m)::value><<<grid, cta, 0, s>>>(a);
+			}
+		});
 		ctx->launches++;
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		return ASTCENC_SUCCESS;

@@ -423,18 +423,33 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_error_metrics_device_imag
  *   block's share of the error sum behind log_rmse, measured whether or not HDR figures are asked for: errors in dark and mid
  *   tones weigh as much as errors in the brightest blocks. Summed over the image and divided by the pixel count, log_rmse^2.
  * The image sums agree with the figures up to the per-block float rounding.
+ * The normal-map metrics measure the angle theta(o, d) in degrees of each texel, the per-texel term of mean_angular_error and
+ * worst_angular_error: each texel's RGB becomes a normal (c - 0.5) * 2, normalised (a zero-length vector becomes the unit
+ * vector (1, 1, 1) / sqrt(3)); the dot product of the two normals is taken in float in DPPS order ((x1 x2 + y1 y2) + (z1 z2 + 0))
+ * and clamped to [-1, 1] with fminf(fmaxf(dot, -1), 1), so a NaN dot gives -1, 180 degrees; theta is acos of it in double
+ * times (double)(180.0f / pi). Both read R, G and B whatever input_components selects (input_components is still checked to be
+ * 1-4), and neither depends on compute_normal_metrics or compute_hdr_metrics.
+ * ASTCENC_B200_BLOCK_ANGULAR_ERROR: the sum of theta over the block's texels inside the image, added in double and rounded to
+ *   float once. Summed over the image and divided by the pixel count, mean_angular_error.
+ * ASTCENC_B200_BLOCK_WORST_ANGULAR_ERROR: the largest theta over the same texels, combined with fmax in double (the order does
+ *   not matter) and rounded to float once. The largest value of the map is exactly (float)worst_angular_error, as rounding to
+ *   float is monotone. Its total over the image is a sum of maxima, not a figure.
+ * Valid values are 0, 1, 2, 4 and 5. Any other value, 3 included, is ASTCENC_ERR_BAD_PARAM wherever a call takes a block_metric.
  */
 enum astcenc_b200_block_metric {
 	ASTCENC_B200_BLOCK_SQUARED_ERROR = 0,
 	ASTCENC_B200_BLOCK_ALPHA_WEIGHTED_ERROR = 1,
-	ASTCENC_B200_BLOCK_LOG2_ERROR = 2
+	ASTCENC_B200_BLOCK_LOG2_ERROR = 2,
+	/* 3 is not assigned */
+	ASTCENC_B200_BLOCK_ANGULAR_ERROR = 4,        /* sum over the block's texels of the angle, in degrees */
+	ASTCENC_B200_BLOCK_WORST_ANGULAR_ERROR = 5   /* the largest angle over the block's texels, in degrees */
 };
 
 /**
  * astcenc_b200_compute_error_metrics_device_images with a chosen per-block error map: every block_error map receives
  * block_metric (enum astcenc_b200_block_metric) instead of the squared error. Everything else is that call's: the figures (bit for
  * bit the same), the stream, the descriptor table, decompress-only contexts, the launch count (two kernel launches, three when any
- * entry asks for a map) and the error order, into which one check is inserted: ASTCENC_ERR_BAD_PARAM for block_metric outside 0-2
+ * entry asks for a map) and the error order, into which one check is inserted: ASTCENC_ERR_BAD_PARAM for block_metric not one of 0, 1, 2, 4, 5
  * comes right after the check of input_components. With ASTCENC_B200_BLOCK_SQUARED_ERROR the call is
  * astcenc_b200_compute_error_metrics_device_images.
  */
@@ -633,7 +648,7 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_errors_device_block
  * value receives bit for bit what astcenc_b200_compute_block_metric_device_images writes for that block with the same
  * input_components and block_metric, and every other value is left untouched. Everything else is that call's: the list rule, the
  * stream, decompress-only contexts, one kernel launch (none when the capacities are all zero) and the error order, into which one
- * check is inserted: ASTCENC_ERR_BAD_PARAM for block_metric outside 0-2 comes right after the check of input_components. With
+ * check is inserted: ASTCENC_ERR_BAD_PARAM for block_metric not one of 0, 1, 2, 4, 5 comes right after the check of input_components. With
  * ASTCENC_B200_BLOCK_SQUARED_ERROR the call is astcenc_b200_compute_block_errors_device_block_lists.
  */
 ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_metric_device_block_lists(struct astcenc_context* context, int input_components,
@@ -678,7 +693,7 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_compute_block_metric_device_block
  *   2. ASTCENC_ERR_BAD_PARAM for a NULL swizzle, then ASTCENC_ERR_BAD_SWIZZLE for a swizzle with a selector beyond
  *      ASTCENC_SWZ_1; then the same two for decode_swizzle, whose selectors may go up to ASTCENC_SWZ_Z;
  *   3. ASTCENC_ERR_BAD_PARAM for input_components outside 1-4;
- *   4. ASTCENC_ERR_BAD_PARAM for block_metric outside 0-2;
+ *   4. ASTCENC_ERR_BAD_PARAM for block_metric not one of 0, 1, 2, 4, 5;
  *   5. ASTCENC_ERR_BAD_PARAM for lists == NULL with a non-zero count, then for a bad data_type, then for a bad decoded_type,
  *      then for an entry with a NULL data or payload, a NULL indices, count or block_error with capacity > 0, indices, count or
  *      block_error not aligned to 4 bytes, or data or decoded not aligned to its texel (4 / 8 / 16 bytes for U8 / F16 / F32:
@@ -758,9 +773,13 @@ ASTCENC_PUBLIC enum astcenc_error astcenc_b200_refine_device_block_lists_packed(
  *     SQUARED_ERROR, PSNR of at least P dB:               limit = samples * 10^(-P / 10);
  *     ALPHA_WEIGHTED_ERROR, alpha_psnr of at least P dB:  limit = samples * 10^(-P / 10), input_components == 4;
  *     LOG2_ERROR, log_rmse of at most R:                  limit = R^2 * pixels;
+ *     ANGULAR_ERROR, mean_angular_error of at most D deg: limit = D * pixels;
  *   samples being pixels times the number of channels input_components selects. A total agrees with the figure's error sum up
  *   to the per-block float rounding of the map, so a target met within that rounding may be judged either way. limit
- *   = -INFINITY never meets the target.
+ *   = -INFINITY never meets the target. The total of a WORST_ANGULAR_ERROR map is a sum of maxima and is not a target. For "no
+ *   texel worse than T degrees", call astcenc_b200_select_blocks (or astcenc_b200_select_blocks_pooled with no weight) on that
+ *   map with threshold T and a capacity, then refine with the same metric: the candidates are exactly the blocks that still
+ *   have a texel beyond T, so a round in which none is left lists nothing.
  * - The closed loop. Compress, decode and map the set once; then enqueue every round up front, each one this call (then the
  *   weights are current), astcenc_b200_select_blocks_pooled with these weights, a threshold of 0 and the round's budget K, and
  *   astcenc_b200_refine_device_block_lists_packed with budget K, which keeps the maps current and stages K slots rather than

@@ -556,6 +556,67 @@ static astcenc_error scratch_turn(astcenc_context* ctx, cudaStream_t stream, F w
 	return st;
 }
 
+// The stream of a call: the caller's, or the context's when the caller passes null.
+static cudaStream_t call_stream(const astcenc_context* ctx, void* cuda_stream) {
+	return cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
+}
+
+// A device-table call once its arguments are checked: `work(stream)` enqueues it on call_stream, on the context's device, in
+// one scratch turn.
+template <typename F>
+static astcenc_error device_turn(astcenc_context* ctx, void* cuda_stream, F work) {
+	DeviceGuard guard(ctx->device);
+	if (!guard.ok) {
+		return ASTCENC_ERR_BAD_CONTEXT;
+	}
+	const cudaStream_t stream = call_stream(ctx, cuda_stream);
+	return scratch_turn(ctx, stream, [&] { return work(stream); });
+}
+
+// The tables of one call, sent to a device buffer in one copy. add() puts an array behind the previous ones, at an offset aligned
+// for its type, and returns that offset; reserve() lays out device space behind the last array that the copy does not fill.
+// Device pointers (at) exist from place() on: it grows the buffer, which may move it.
+class TableUpload {
+public:
+	template <typename T> size_t add(const T* p, size_t n) {
+		static_assert(std::is_trivially_copyable<T>::value, "a table is copied byte for byte");
+		const size_t at = reserve<T>(n);
+		bytes_.resize(end_);
+		if (n != 0) {
+			memcpy(bytes_.data() + at, p, n * sizeof(T));
+		}
+		return at;
+	}
+	template <typename T> size_t add(const std::vector<T>& v) { return add(v.data(), v.size()); }
+	template <typename T> size_t reserve(size_t n) {
+		const size_t at = (end_ + alignof(T) - 1) & ~(alignof(T) - 1);
+		end_ = at + n * sizeof(T);
+		return at;
+	}
+	astcenc_error place(DevBuffer& buf) {
+		const astcenc_error st = ensure_buffer(buf, end_);
+		device_ = st == ASTCENC_SUCCESS ? buf.ptr : nullptr;
+		return st;
+	}
+	// place(buf), then the arrays in one copy on `stream`, from pageable memory: staged by the driver before the call returns, so
+	// the host arrays (a host list's indices among them) may go when the caller does.
+	astcenc_error send(DevBuffer& buf, cudaStream_t stream) {
+		astcenc_error st = place(buf);
+		if (st == ASTCENC_SUCCESS) {
+			CUDA_TRY(cudaMemcpyAsync(device_, bytes_.data(), bytes_.size(), cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+		}
+		return st;
+	}
+	template <typename T> T* at(size_t offset) const { return reinterpret_cast<T*>(device_ + offset); }
+	// the host copy of an added array, for fields that point into the buffer itself (set after place, before the copy)
+	template <typename T> T* host(size_t offset) { return reinterpret_cast<T*>(bytes_.data() + offset); }
+
+private:
+	std::vector<uint8_t> bytes_;
+	size_t end_ = 0;
+	uint8_t* device_ = nullptr;
+};
+
 static std::mutex g_const_mtx;
 static DevConstTables* g_d_consts[64];
 
@@ -1424,6 +1485,56 @@ astcenc_error astcenc_compress_cancel(astcenc_context* ctx) {
 	return ASTCENC_SUCCESS;
 }
 
+// p is aligned to `a` bytes, a power of two (null is aligned to anything).
+static bool aligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+// The metrics entry of a pair of images of one geometry, dim_z slices of dim_x * dim_y texels: the original of original_type and
+// the decoded image of decoded_type, with the figures and map they receive (either may be null). blocks_x and blocks_y are the
+// footprint's block grid, which a refine call's pairs are read with; the metric planners fill in the rest (and set those two
+// again).
+static MetricEntry metric_pair(const astcenc_context* ctx, const void* original, astcenc_type original_type, const void* decoded, astcenc_type decoded_type,
+                               unsigned int dim_x, unsigned int dim_y, unsigned int dim_z, astcenc_b200_error_metrics* metrics, float* block_error) {
+	MetricEntry e{};
+	e.img1 = original;
+	e.img2 = decoded;
+	e.type1 = (int)original_type;
+	e.type2 = (int)decoded_type;
+	e.pitch1 = e.pitch2 = dim_x;
+	e.stride1 = e.stride2 = (size_t)dim_x * dim_y;
+	e.dim_x = dim_x;
+	e.dim_y = dim_y;
+	e.dim_z = dim_z;
+	e.blocks_x = (unsigned int)block_count_axis(dim_x, ctx->tables->bsd.dim_x);
+	e.blocks_y = (unsigned int)block_count_axis(dim_y, ctx->tables->bsd.dim_y);
+	e.metrics = metrics;
+	e.block_error = block_error;
+	return e;
+}
+
+// A block-list table (astc_dev_gather.cuh): entry j is table[j] with lists[j] (no lists: every block of each image), and owns
+// the call slots [table[j].first, table[j].first + its slots); `slots` is their total.
+struct ListTable {
+	std::vector<GatherImage> table;
+	std::vector<GatherList> lists;
+	size_t slots = 0;
+	// Appends image entry e (of table_entry) with its list, or with none for a null list, owning n slots: the list's capacity, or
+	// the image's blocks. An entry of no slots is left out. ASTCENC_ERR_BAD_PARAM when the total does not fit a size_t.
+	astcenc_error add(GatherImage e, const GatherList* list, size_t n) {
+		if (n > SIZE_MAX - slots) {
+			return ASTCENC_ERR_BAD_PARAM;
+		}
+		if (n != 0) {
+			e.first = slots;
+			table.push_back(e);
+			if (list != nullptr) {
+				lists.push_back(*list);
+			}
+			slots += n;
+		}
+		return ASTCENC_SUCCESS;
+	}
+};
+
 // Entry e of an image table: dim_z slices of dim_x * dim_y texels of `data_type` at `data`, its payload at `payload`, call blocks
 // [first, first + its blocks). Advances `first`. ASTCENC_ERR_BAD_PARAM when the image's payload does not fit a size_t, the image
 // has 2^32 blocks or more (the table walks index an image's blocks with 32 bits, as block lists do) or the call's total does
@@ -1462,13 +1573,13 @@ static void enqueue_decode(astcenc_context* ctx, const GatherImage* d_table, uns
 // context's table buffer, ctx->list).
 static astcenc_error launch_decode(astcenc_context* ctx, const GatherImage* table, unsigned int image_count, size_t blocks, int data_type,
                                    const astcenc_swizzle& swizzle, cudaStream_t stream) {
-	astcenc_error st = ensure_buffer(ctx->list, image_count * sizeof(GatherImage));
+	TableUpload up;
+	const size_t table_at = up.add(table, image_count);
+	astcenc_error st = up.send(ctx->list, stream);
 	if (st != ASTCENC_SUCCESS) {
 		return st;
 	}
-	// (from pageable memory: staged by the driver before the call returns)
-	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, table, image_count * sizeof(GatherImage), cudaMemcpyHostToDevice, stream), return ASTCENC_ERR_BAD_CONTEXT);
-	enqueue_decode(ctx, ctx->list.as<const GatherImage>(), image_count, blocks, data_type, swizzle, stream);
+	enqueue_decode(ctx, up.at<const GatherImage>(table_at), image_count, blocks, data_type, swizzle, stream);
 	CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 	return ASTCENC_SUCCESS;
 }
@@ -1588,24 +1699,18 @@ static bool check_block_metric(astcenc_b200_block_metric block_metric) {
 // block_metric when an entry asks for a map. The sums of entry j are left at ctx->metric_partials + (plan.ctas + j) * ASTC_METRIC_SUMS doubles.
 static astcenc_error launch_metrics(astcenc_context* ctx, const std::vector<MetricEntry>& table, const MetricPlan& plan, int hdr, int normal,
                                     int input_components, astcenc_b200_block_metric block_metric, int fstop_lo, int fstop_hi, cudaStream_t stream) {
-	const size_t table_bytes = table.size() * sizeof(MetricEntry);
-	const size_t map_bytes = plan.maps.size() * sizeof(MetricMap);
-	std::vector<uint8_t> up(table_bytes + map_bytes);
-	memcpy(up.data(), table.data(), table_bytes);
-	if (map_bytes != 0) {
-		memcpy(up.data() + table_bytes, plan.maps.data(), map_bytes);
-	}
-	astcenc_error st = ensure_buffer(ctx->list, up.size());
+	TableUpload up;
+	const size_t table_at = up.add(table);
+	const size_t maps_at = up.add(plan.maps);
+	astcenc_error st = up.send(ctx->list, stream);
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->metric_partials, plan.partial_doubles * sizeof(double));
 	if (st != ASTCENC_SUCCESS) {
 		return st;
 	}
-	// (from pageable memory: staged by the driver before the call returns)
-	CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, stream), return ASTCENC_ERR_BAD_CONTEXT);
 	MetricArgs a;
-	a.entries = ctx->list.as<const MetricEntry>();
+	a.entries = up.at<const MetricEntry>(table_at);
 	a.count = (unsigned int)table.size();
-	a.maps = reinterpret_cast<const MetricMap*>(ctx->list.ptr + table_bytes);
+	a.maps = up.at<const MetricMap>(maps_at);
 	a.map_count = (unsigned int)plan.maps.size();
 	a.map_blocks = plan.map_blocks;
 	a.bx = ctx->config.block_x;
@@ -1664,19 +1769,13 @@ astcenc_error astcenc_b200_compute_error_metrics(astcenc_context* ctx, int compu
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	std::vector<MetricEntry> table(1);
+	// (the images are uploaded whole, so each keeps its own pitch and stride)
+	std::vector<MetricEntry> table{metric_pair(ctx, nullptr, img1->data_type, nullptr, img2->data_type, dim_x, dim_y, dim_z, nullptr, nullptr)};
 	MetricEntry& e = table[0];
-	e.type1 = (int)img1->data_type;
-	e.type2 = (int)img2->data_type;
 	e.pitch1 = img1->dim_x;
 	e.pitch2 = img2->dim_x;
 	e.stride1 = (size_t)img1->dim_x * img1->dim_y;
 	e.stride2 = (size_t)img2->dim_x * img2->dim_y;
-	e.dim_x = dim_x;
-	e.dim_y = dim_y;
-	e.dim_z = dim_z;
-	e.metrics = nullptr;
-	e.block_error = nullptr;
 	MetricPlan plan;
 	if (!plan_metrics(table, ctx->config.block_x, ctx->config.block_y, ctx->config.block_z > 1 ? ctx->config.block_z : 1, plan)) {
 		return ASTCENC_ERR_BAD_PARAM;
@@ -1753,8 +1852,7 @@ astcenc_error astcenc_b200_compress_device(astcenc_context* ctx, const void* d_p
 	if (!guard.ok) {
 		return ASTCENC_ERR_BAD_CONTEXT;
 	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return launch_slab(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, 1, *swizzle), block_row0, block_rows, d_out, s);
+	return launch_slab(ctx, pass_image(ctx, d_pixels, (int)data_type, dim_x, dim_y, 1, *swizzle), block_row0, block_rows, d_out, call_stream(ctx, cuda_stream));
 }
 
 // One entry of a staging call: an image and its payload (plan_blocks sets `first` and `avg_offset`), its list (null: every
@@ -1777,18 +1875,15 @@ struct RefineSpec {
 	int components = 0;
 };
 
-// What launch_blocks compresses: a block-list table (astc_dev_gather.cuh). Entry j is table[j], lists[j] (no lists: every block
-// of each image), the block rows of its alpha-scale pre-pass (rows[j]) and, in a refine call, its pair (pairs[j]; no pairs: the
-// staged blocks are scattered). `words` go up behind the lists: a host list's count word and indices, at which its GatherList
-// (count and indices null here) is pointed. A packed call (astc_dev_pack.cuh) stages min(budget, blocks) slots, and its table's
-// firsts are rewritten on the device before the first gather.
-struct BlockCall {
-	std::vector<GatherImage> table;
-	std::vector<GatherList> lists;
+// What launch_blocks compresses: a block-list table whose slots are the call's staging blocks (a packed call: the sum of the
+// capacities). Entry j also has the block rows of its alpha-scale pre-pass (rows[j]) and, in a refine call, its pair (pairs[j];
+// no pairs: the staged blocks are scattered). `words` go up behind the lists: a host list's count word and indices, at which its
+// GatherList (count and indices null here) is pointed. A packed call (astc_dev_pack.cuh) stages min(budget, slots) slots, and
+// its table's firsts are rewritten on the device before the first gather.
+struct BlockCall : ListTable {
 	std::vector<std::pair<unsigned int, unsigned int>> rows;
 	std::vector<MetricEntry> pairs;
 	std::vector<uint32_t> words;
-	size_t blocks = 0;                 // staging blocks of the whole call (a packed call: the sum of the capacities)
 	int data_type = 0;
 	RefineSpec refine;                 // (refine calls)
 	bool packed = false;               // (packed calls) the budget and the device word that receives the overflow, or null
@@ -1802,24 +1897,20 @@ static astcenc_error plan_blocks(const std::vector<BlockEntry>& entries, astcenc
 	call.data_type = (int)data_type;
 	size_t avg_offset = 0;
 	for (const BlockEntry& en : entries) {
-		if (en.blocks == 0) {
+		const size_t kept = call.table.size();
+		const astcenc_error st = call.add(en.image, en.list, en.blocks);
+		if (st != ASTCENC_SUCCESS) {
+			return st;
+		}
+		if (call.table.size() == kept) {
 			continue;
 		}
-		if (en.blocks > SIZE_MAX - call.blocks) {
-			return ASTCENC_ERR_BAD_PARAM;
-		}
-		GatherImage e = en.image;
-		e.first = call.blocks;
+		GatherImage& e = call.table.back();
 		e.avg_offset = avg_offset;
-		call.table.push_back(e);
-		if (en.list != nullptr) {
-			call.lists.push_back(*en.list);
-		}
 		if (en.pair != nullptr) {
 			call.pairs.push_back(*en.pair);
 		}
 		call.rows.push_back({en.row0, en.row1 < e.blocks_y ? en.row1 : e.blocks_y});
-		call.blocks += en.blocks;
 		avg_offset += (size_t)e.dim_x * e.dim_y;
 	}
 	return ASTCENC_SUCCESS;
@@ -1835,72 +1926,65 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	const DevBsd& bsd = ctx->tables->bsd;
 	const bool volume = bsd.dim_z > 1;
 	const unsigned int radius = volume ? 0 : ctx->config.a_scale_radius;
-	const size_t n = call.packed && call.budget < call.blocks ? call.budget : call.blocks;
+	const size_t n = call.packed && call.budget < call.slots ? call.budget : call.slots;
 	const size_t chunk = n < ctx->knobs.batch_blocks ? n : ctx->knobs.batch_blocks;
 	const size_t avg_floats = call.table.back().avg_offset + (size_t)call.table.back().dim_x * call.table.back().dim_y;
 	const bool refine = !call.pairs.empty();
-	// in the table buffer: the table (a packed call: and its sentinel), its lists, a refine call's pairs and its two decode tables
-	// (a full chunk's decode row, the last chunk's), then the words
-	const size_t table_bytes = (call.table.size() + (call.packed ? 1 : 0)) * sizeof(GatherImage);
-	const size_t lists_bytes = call.lists.size() * sizeof(GatherList);
-	const size_t pairs_bytes = call.pairs.size() * sizeof(MetricEntry);
-	const size_t rows_bytes = refine && n != 0 ? 2 * sizeof(GatherImage) : 0;
-	const size_t words_at = table_bytes + lists_bytes + pairs_bytes + rows_bytes;
-	const size_t list_bytes = words_at + call.words.size() * sizeof(uint32_t);
 	// the refine buffer: the decode row of a chunk, then its values and decisions
 	const size_t row_bytes = (chunk * bsd.texel_count * texel_bytes(call.refine.decoded_type) + 255) & ~(size_t)255;
-	astcenc_error st = ensure_buffer(ctx->list, list_bytes);
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * texel_bytes(call.data_type));
+	astcenc_error st = ensure_buffer(ctx->list_image, chunk * bsd.texel_count * texel_bytes(call.data_type));
 	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->list_out, chunk * 16);
 	if (st == ASTCENC_SUCCESS && refine) st = ensure_buffer(ctx->refine, row_bytes + chunk * (sizeof(float) + 1));
 	if (st == ASTCENC_SUCCESS && radius != 0 && n != 0) {
 		st = ensure_buffer(ctx->list_alpha, avg_floats * sizeof(float));
 		if (st == ASTCENC_SUCCESS) st = ensure_scratch(ctx, 0, chunk * bsd.texel_count);
 	}
-	if (st == ASTCENC_SUCCESS) {
-		// the table, its lists, the pairs, the decode tables and the words in one copy, from pageable memory: staged by the driver
-		// before the call returns, so a host list may go when this function does
-		std::vector<GatherList> lists = call.lists;
-		for (GatherList& l : lists) {
-			if (l.count == nullptr) {
-				l.count = reinterpret_cast<const uint32_t*>(ctx->list.ptr + words_at);
-				l.indices = l.count + 1;
-			}
-		}
-		// a decode row of m blocks is an image of m x 1 blocks: the staged candidates (list_out) decoded into the refine buffer
-		std::vector<GatherImage> rows;
-		for (size_t m : {chunk, n - (n - 1) / (chunk != 0 ? chunk : 1) * chunk}) {
-			if (rows_bytes != 0) {
-				rows.push_back({ctx->refine.ptr, ctx->list_out.ptr, 0, 0, (unsigned int)(m * bsd.dim_x), bsd.dim_y, volume ? bsd.dim_z : 1u, (unsigned int)m, 1});
-			}
-		}
-		std::vector<GatherImage> table = call.table;
-		if (call.packed) {
-			table.push_back(GatherImage{});      // (the sentinel: astc_pack_lists_kernel writes the packed total there)
-		}
-		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(lists.data()), reinterpret_cast<const uint8_t*>(lists.data()) + lists_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.pairs.data()), reinterpret_cast<const uint8_t*>(call.pairs.data()) + pairs_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(rows.data()), reinterpret_cast<const uint8_t*>(rows.data()) + rows_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(call.words.data()), reinterpret_cast<const uint8_t*>(call.words.data()) + call.words.size() * sizeof(uint32_t));
-		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), list_bytes, cudaMemcpyHostToDevice, stream), st = ASTCENC_ERR_BAD_CONTEXT);
+	if (st != ASTCENC_SUCCESS) {
+		return st;
 	}
-	if (st == ASTCENC_SUCCESS && call.packed) {
-		astc_pack_lists_kernel<<<1, 32, 0, stream>>>(ctx->list.as<GatherImage>(), reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes),
-		                                             (unsigned int)call.table.size(), call.budget, call.overflow);
+	// In the table buffer: the table (a packed call: and its sentinel, where astc_pack_lists_kernel writes the packed total), its
+	// lists, a refine call's pairs and its two decode tables (a full chunk's decode row, the last chunk's), then the words. A
+	// decode row of m blocks is an image of m x 1 blocks: the staged candidates (list_out) decoded into the refine buffer.
+	const GatherImage sentinel{};
+	std::vector<GatherImage> rows;
+	if (refine && n != 0) {
+		for (size_t m : {chunk, n - (n - 1) / chunk * chunk}) {
+			rows.push_back({ctx->refine.ptr, ctx->list_out.ptr, 0, 0, (unsigned int)(m * bsd.dim_x), bsd.dim_y, volume ? bsd.dim_z : 1u, (unsigned int)m, 1});
+		}
+	}
+	TableUpload up;
+	const size_t table_at = up.add(call.table);
+	up.add(&sentinel, call.packed ? 1 : 0);
+	const size_t lists_at = up.add(call.lists);
+	const size_t pairs_at = up.add(call.pairs);
+	const size_t rows_at = up.add(rows);
+	const size_t words_at = up.add(call.words);
+	st = up.place(ctx->list);
+	for (size_t k = 0; k < call.lists.size() && st == ASTCENC_SUCCESS; k++) {
+		GatherList& l = up.host<GatherList>(lists_at)[k];
+		if (l.count == nullptr) {
+			l.count = up.at<const uint32_t>(words_at);
+			l.indices = l.count + 1;
+		}
+	}
+	if (st == ASTCENC_SUCCESS) st = up.send(ctx->list, stream);
+	if (st != ASTCENC_SUCCESS) {
+		return st;
+	}
+	if (call.packed) {
+		astc_pack_lists_kernel<<<1, 32, 0, stream>>>(up.at<GatherImage>(table_at), up.at<const GatherList>(lists_at), (unsigned int)call.table.size(), call.budget,
+		                                             call.overflow);
 		ctx->launches++;
 		CUDA_TRY(cudaGetLastError(), st = ASTCENC_ERR_BAD_CONTEXT);
 	}
-	// (refine calls) the decide and commit arguments and the decode tables
+	// (refine calls) the decide and commit arguments
 	RefineArgs r{};
-	const GatherImage* d_rows = nullptr;
-	if (refine && st == ASTCENC_SUCCESS) {
-		r.pairs = reinterpret_cast<const MetricEntry*>(ctx->list.ptr + table_bytes + lists_bytes);
+	if (refine) {
+		r.pairs = up.at<const MetricEntry>(pairs_at);
 		r.row = ctx->refine.ptr;
 		r.values = reinterpret_cast<float*>(ctx->refine.ptr + row_bytes);
 		r.keep = ctx->refine.ptr + row_bytes + chunk * sizeof(float);
 		r.components = call.refine.components;
-		d_rows = reinterpret_cast<const GatherImage*>(ctx->list.ptr + table_bytes + lists_bytes + pairs_bytes);
 	}
 	// The staging pass reads averages gathered from the sources', so it runs no pre-pass of its own: its box filter would reach
 	// across the seams between unrelated blocks. A source's averages cover its window's rows, at their image positions, in the
@@ -1919,9 +2003,9 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 	g.bx = bsd.dim_x;
 	g.by = bsd.dim_y;
 	g.bz = bsd.dim_z;
-	g.images = ctx->list.as<const GatherImage>();
+	g.images = up.at<const GatherImage>(table_at);
 	g.image_count = (unsigned int)call.table.size();
-	g.lists = call.lists.empty() ? nullptr : reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes);
+	g.lists = call.lists.empty() ? nullptr : up.at<const GatherList>(lists_at);
 	for (size_t first = 0; first < n && st == ASTCENC_SUCCESS; first += chunk) {
 		const unsigned int m = (unsigned int)(n - first < chunk ? n - first : chunk);
 		g.base = first;
@@ -1940,7 +2024,7 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 		staged.alpha_threshold = threshold;
 		st = launch_slab_locked(ctx, staged, 0, 1, ctx->list_out.ptr, stream, nullptr);
 		if (st == ASTCENC_SUCCESS && refine) {
-			enqueue_decode(ctx, d_rows + (m == chunk ? 0 : 1), 1, m, call.refine.decoded_type, call.refine.decode_swizzle, stream);
+			enqueue_decode(ctx, up.at<const GatherImage>(rows_at) + (m == chunk ? 0 : 1), 1, m, call.refine.decoded_type, call.refine.decode_swizzle, stream);
 			const unsigned int grid = (m + ASTC_REFINE_LIST_WARPS - 1) / ASTC_REFINE_LIST_WARPS;
 			if (call.packed) {
 				with_block_metric(call.refine.block_metric, [&](auto mt) {
@@ -1972,15 +2056,10 @@ static astcenc_error launch_blocks_locked(astcenc_context* ctx, const BlockCall&
 // A staging call on `cuda_stream` (null: the context's stream); a call of no staging blocks launches nothing (a packed call:
 // one whose capacities are all 0, whatever its budget).
 static astcenc_error launch_blocks(astcenc_context* ctx, const BlockCall& call, const astcenc_swizzle& swizzle, void* cuda_stream) {
-	if (call.blocks == 0) {
+	if (call.slots == 0) {
 		return ASTCENC_SUCCESS;
 	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t stream = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, stream, [&] { return launch_blocks_locked(ctx, call, swizzle, stream); });
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t stream) { return launch_blocks_locked(ctx, call, swizzle, stream); });
 }
 
 // A host list is a one-entry block-list table: its count word and indices go up with the table (BlockCall::words).
@@ -2105,7 +2184,7 @@ astcenc_error astcenc_b200_compress_images(astcenc_context* ctx, astcenc_image* 
 		in_bytes += ((size_t)images[i]->dim_x * images[i]->dim_y * images[i]->dim_z * texel_bytes(call.data_type) + 255) & ~(size_t)255;
 	}
 	astcenc_error st = ensure_buffer(ctx->image, in_bytes);
-	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->out, call.blocks * 16);
+	if (st == ASTCENC_SUCCESS) st = ensure_buffer(ctx->out, call.slots * 16);
 	if (st != ASTCENC_SUCCESS) {
 		return st;
 	}
@@ -2163,12 +2242,7 @@ astcenc_error astcenc_b200_decompress_device_images(astcenc_context* ctx, const 
 	if (status != ASTCENC_SUCCESS || image_count == 0) {
 		return status;
 	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, s, [&] { return launch_decode(ctx, table.data(), image_count, blocks, (int)data_type, *swizzle, s); });
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) { return launch_decode(ctx, table.data(), image_count, blocks, (int)data_type, *swizzle, s); });
 }
 
 // Metrics calls: every pair is checked before anything is enqueued; the table goes up in one copy and the call is two
@@ -2189,8 +2263,7 @@ astcenc_error astcenc_b200_compute_block_metric_device_images(astcenc_context* c
 	if (image_count != 0 && !images) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
-	auto aligned = [](const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
-	std::vector<MetricEntry> table(image_count);
+	std::vector<MetricEntry> table;
 	for (unsigned int i = 0; i < image_count; i++) {
 		const astcenc_b200_device_metrics_image& im = images[i];
 		if (!im.original || !im.decoded || !im.metrics || check_texel_count(im.dim_x, im.dim_y, im.dim_z) != ASTCENC_SUCCESS ||
@@ -2199,18 +2272,7 @@ astcenc_error astcenc_b200_compute_block_metric_device_images(astcenc_context* c
 		    !aligned(im.block_error, 4)) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
-		MetricEntry& e = table[i];
-		e.img1 = im.original;
-		e.img2 = im.decoded;
-		e.type1 = (int)im.original_type;
-		e.type2 = (int)im.decoded_type;
-		e.pitch1 = e.pitch2 = im.dim_x;
-		e.stride1 = e.stride2 = (size_t)im.dim_x * im.dim_y;
-		e.dim_x = im.dim_x;
-		e.dim_y = im.dim_y;
-		e.dim_z = im.dim_z;
-		e.metrics = im.metrics;
-		e.block_error = im.block_error;
+		table.push_back(metric_pair(ctx, im.original, im.original_type, im.decoded, im.decoded_type, im.dim_x, im.dim_y, im.dim_z, im.metrics, im.block_error));
 	}
 	MetricPlan plan;
 	if (!plan_metrics(table, ctx->config.block_x, ctx->config.block_y, ctx->config.block_z > 1 ? ctx->config.block_z : 1, plan)) {
@@ -2219,12 +2281,7 @@ astcenc_error astcenc_b200_compute_block_metric_device_images(astcenc_context* c
 	if (image_count == 0) {
 		return ASTCENC_SUCCESS;
 	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, s, [&] {
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) {
 		return launch_metrics(ctx, table, plan, compute_hdr_metrics, compute_normal_metrics, input_components, block_metric, fstop_lo, fstop_hi, s);
 	});
 }
@@ -2237,32 +2294,43 @@ astcenc_error astcenc_b200_compute_error_metrics_device_images(astcenc_context* 
 }
 
 // Device block lists: an image table whose entry j owns capacity[j] staging blocks, the slots of its device list (GatherList).
-// Checked whole before anything is enqueued, in the image-table order of astcenc_b200_compress_device_images; entries with a
-// capacity of 0 are checked and then left out of the call. The unpacked and packed calls share this plan.
+// The tail of the compress-list and refine-list plans, once each has run its own checks: the image table (check_image_table),
+// then the staging call of the lists, in a refine call with pairs[j] beside entry j (null: no pairs). Entries with a capacity of
+// 0 are checked and then left out of the call.
+static astcenc_error plan_list_call(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count, astcenc_type data_type,
+                                    const MetricEntry* pairs, BlockCall& call) {
+	std::vector<astcenc_b200_device_image> descs;
+	for (unsigned int i = 0; i < list_count; i++) {
+		descs.push_back({lists[i].data, lists[i].dim_x, lists[i].dim_y, lists[i].dim_z, lists[i].payload});
+	}
+	std::vector<BlockEntry> entries;
+	astcenc_error status = check_image_table(ctx, descs.data(), list_count, data_type, entries);
+	std::vector<GatherList> gather_lists(list_count);
+	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
+		gather_lists[i] = {lists[i].indices, lists[i].count, lists[i].capacity, (unsigned int)entries[i].blocks};
+		entries[i].list = &gather_lists[i];
+		entries[i].blocks = lists[i].capacity;
+		entries[i].pair = pairs != nullptr ? &pairs[i] : nullptr;
+	}
+	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	return status;
+}
+
+// Checked whole before anything is enqueued, in the image-table order of astcenc_b200_compress_device_images. The unpacked and
+// packed calls share this plan.
 static astcenc_error plan_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_list* lists, unsigned int list_count,
                                              astcenc_type data_type, const astcenc_swizzle* swizzle, BlockCall& call) {
 	astcenc_error status = check_compress_context(ctx);
 	if (status == ASTCENC_SUCCESS && !swizzle) status = ASTCENC_ERR_BAD_PARAM;
 	if (status == ASTCENC_SUCCESS) status = check_swizzle(*swizzle, ASTCENC_SWZ_1);
 	if (status == ASTCENC_SUCCESS && list_count != 0 && !lists) status = ASTCENC_ERR_BAD_PARAM;
-	auto aligned4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; };
-	std::vector<astcenc_b200_device_image> descs;
 	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_block_list& l = lists[i];
-		if (!l.data || !l.payload || (l.capacity != 0 && (!l.indices || !l.count)) || !aligned4(l.indices) || !aligned4(l.count)) {
+		if (!l.data || !l.payload || (l.capacity != 0 && (!l.indices || !l.count)) || !aligned(l.indices, 4) || !aligned(l.count, 4)) {
 			status = ASTCENC_ERR_BAD_PARAM;
 		}
-		descs.push_back({l.data, l.dim_x, l.dim_y, l.dim_z, l.payload});
 	}
-	std::vector<BlockEntry> entries;
-	if (status == ASTCENC_SUCCESS) status = check_image_table(ctx, descs.data(), list_count, data_type, entries);
-	std::vector<GatherList> gather_lists(list_count);
-	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
-		gather_lists[i] = {lists[i].indices, lists[i].count, lists[i].capacity, (unsigned int)entries[i].blocks};
-		entries[i].list = &gather_lists[i];
-		entries[i].blocks = lists[i].capacity;
-	}
-	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	if (status == ASTCENC_SUCCESS) status = plan_list_call(ctx, lists, list_count, data_type, nullptr, call);
 	return status;
 }
 
@@ -2275,7 +2343,7 @@ astcenc_error astcenc_b200_compress_device_block_lists(astcenc_context* ctx, con
 
 // Packed calls (astc_dev_pack.cuh): the plan of the unpacked call, then the overflow pointer's alignment.
 static astcenc_error pack_call(BlockCall& call, unsigned int budget, uint32_t* overflow) {
-	if ((reinterpret_cast<uintptr_t>(overflow) & 3) != 0) {
+	if (!aligned(overflow, 4)) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
 	call.packed = true;
@@ -2312,42 +2380,18 @@ static astcenc_error plan_refine_lists(astcenc_context* ctx, const astcenc_b200_
 	// access, so each must be aligned to its texel)
 	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
 	if (status == ASTCENC_SUCCESS) status = check_data_type(decoded_type);
-	auto aligned = [](const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
-	std::vector<astcenc_b200_device_image> descs;
+	std::vector<astcenc_b200_device_block_list> block_lists;
+	std::vector<MetricEntry> pairs;
 	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_refine_list& l = lists[i];
 		if (!l.data || !l.payload || (l.capacity != 0 && (!l.indices || !l.count || !l.block_error)) || !aligned(l.indices, 4) || !aligned(l.count, 4) ||
 		    !aligned(l.block_error, 4) || !aligned(l.data, texel_bytes(data_type)) || !aligned(l.decoded, texel_bytes(decoded_type))) {
 			status = ASTCENC_ERR_BAD_PARAM;
 		}
-		descs.push_back({l.data, l.dim_x, l.dim_y, l.dim_z, l.payload});
+		block_lists.push_back({l.data, l.dim_x, l.dim_y, l.dim_z, l.payload, l.indices, l.count, l.capacity});
+		pairs.push_back(metric_pair(ctx, l.data, data_type, l.decoded, decoded_type, l.dim_x, l.dim_y, l.dim_z, nullptr, l.block_error));
 	}
-	std::vector<BlockEntry> entries;
-	if (status == ASTCENC_SUCCESS) status = check_image_table(ctx, descs.data(), list_count, data_type, entries);
-	std::vector<GatherList> gather_lists(list_count);
-	std::vector<MetricEntry> pairs(list_count);
-	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
-		const astcenc_b200_device_refine_list& l = lists[i];
-		gather_lists[i] = {l.indices, l.count, l.capacity, (unsigned int)entries[i].blocks};
-		MetricEntry& e = pairs[i];
-		memset(&e, 0, sizeof(e));
-		e.img1 = l.data;
-		e.img2 = l.decoded;
-		e.type1 = (int)data_type;
-		e.type2 = (int)decoded_type;
-		e.pitch1 = e.pitch2 = l.dim_x;
-		e.stride1 = e.stride2 = (size_t)l.dim_x * l.dim_y;
-		e.dim_x = l.dim_x;
-		e.dim_y = l.dim_y;
-		e.dim_z = l.dim_z;
-		e.blocks_x = entries[i].image.blocks_x;
-		e.blocks_y = entries[i].image.blocks_y;
-		e.block_error = l.block_error;
-		entries[i].list = &gather_lists[i];
-		entries[i].blocks = l.capacity;
-		entries[i].pair = &pairs[i];
-	}
-	if (status == ASTCENC_SUCCESS) status = plan_blocks(entries, data_type, call);
+	if (status == ASTCENC_SUCCESS) status = plan_list_call(ctx, block_lists.data(), list_count, data_type, pairs.data(), call);
 	if (status != ASTCENC_SUCCESS) {
 		return status;
 	}
@@ -2385,59 +2429,41 @@ astcenc_error astcenc_b200_decompress_device_block_lists(astcenc_context* ctx, c
                                                          astcenc_type data_type, const astcenc_swizzle* swizzle, void* cuda_stream) {
 	astcenc_error status = swizzle ? check_swizzle(*swizzle, ASTCENC_SWZ_Z) : ASTCENC_ERR_BAD_PARAM;
 	if (status == ASTCENC_SUCCESS && list_count != 0 && !lists) status = ASTCENC_ERR_BAD_PARAM;
-	auto aligned4 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; };
 	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_decode_block_list& l = lists[i];
-		if (!l.payload || !l.data || (l.capacity != 0 && (!l.indices || !l.count)) || !aligned4(l.indices) || !aligned4(l.count)) {
+		if (!l.payload || !l.data || (l.capacity != 0 && (!l.indices || !l.count)) || !aligned(l.indices, 4) || !aligned(l.count, 4)) {
 			status = ASTCENC_ERR_BAD_PARAM;
 		} else {
 			status = check_texel_count(l.dim_x, l.dim_y, l.dim_z);
 		}
 	}
 	if (status == ASTCENC_SUCCESS) status = check_data_type(data_type);
-	std::vector<GatherImage> table;
-	std::vector<GatherList> gather_lists;
-	size_t slots = 0;
+	ListTable t;
 	for (unsigned int i = 0; i < list_count && status == ASTCENC_SUCCESS; i++) {
 		const astcenc_b200_device_decode_block_list& l = lists[i];
 		GatherImage e;
 		size_t blocks = 0;
 		// (the payload is read, never written)
 		status = table_entry(ctx, (int)data_type, l.dim_x, l.dim_y, l.dim_z, l.data, const_cast<uint8_t*>(l.payload), blocks, e);
-		if (status == ASTCENC_SUCCESS && l.capacity > SIZE_MAX - slots) {
-			status = ASTCENC_ERR_BAD_PARAM;
-		}
-		if (status == ASTCENC_SUCCESS && l.capacity != 0) {
-			e.first = slots;
-			table.push_back(e);
-			gather_lists.push_back({l.indices, l.count, l.capacity, (unsigned int)blocks});
-			slots += l.capacity;
-		}
+		const GatherList list{l.indices, l.count, l.capacity, (unsigned int)blocks};
+		if (status == ASTCENC_SUCCESS) status = t.add(e, &list, l.capacity);
 	}
-	if (status != ASTCENC_SUCCESS || slots == 0) {
+	if (status != ASTCENC_SUCCESS || t.slots == 0) {
 		return status;
 	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, s, [&]() -> astcenc_error {
-		const size_t table_bytes = table.size() * sizeof(GatherImage);
-		const size_t lists_bytes = gather_lists.size() * sizeof(GatherList);
-		astcenc_error r = ensure_buffer(ctx->list, table_bytes + lists_bytes);
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) -> astcenc_error {
+		TableUpload up;
+		const size_t table_at = up.add(t.table);
+		const size_t lists_at = up.add(t.lists);
+		astcenc_error r = up.send(ctx->list, s);
 		if (r != ASTCENC_SUCCESS) {
 			return r;
 		}
-		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(gather_lists.data()), reinterpret_cast<const uint8_t*>(gather_lists.data()) + lists_bytes);
-		// (from pageable memory: staged by the driver before the call returns)
-		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
 		const size_t cap = (size_t)ctx->sm_count * ASTC_DECODE_LIST_CTAS_PER_SM;
-		const unsigned int grid = (unsigned int)(slots < cap ? slots : cap);
+		const unsigned int grid = (unsigned int)(t.slots < cap ? t.slots : cap);
 		astc_decompress_block_lists_kernel<<<grid, 32, ASTC_SMEM_HDR + D_SLICE, s>>>(
-		    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, (int)data_type, 0, 0, 0, *swizzle), ctx->list.as<const GatherImage>(),
-		    reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes), (unsigned int)table.size(), slots);
+		    ctx->tables->bsd, ctx->dcfg, pass_image(ctx, nullptr, (int)data_type, 0, 0, 0, *swizzle), up.at<const GatherImage>(table_at),
+		    up.at<const GatherList>(lists_at), (unsigned int)t.table.size(), t.slots);
 		ctx->launches++;
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		return ASTCENC_SUCCESS;
@@ -2459,8 +2485,7 @@ astcenc_error astcenc_b200_compute_block_metric_device_block_lists(astcenc_conte
 	if (list_count != 0 && !lists) {
 		return ASTCENC_ERR_BAD_PARAM;
 	}
-	auto aligned = [](const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
-	std::vector<MetricEntry> table(list_count);
+	std::vector<MetricEntry> table;
 	std::vector<GatherList> gather_lists(list_count);
 	std::vector<unsigned int> capacities(list_count);
 	for (unsigned int i = 0; i < list_count; i++) {
@@ -2471,18 +2496,7 @@ astcenc_error astcenc_b200_compute_block_metric_device_block_lists(astcenc_conte
 		    !aligned(l.decoded, texel_bytes(l.decoded_type)) || !aligned(l.block_error, 4) || !aligned(l.indices, 4) || !aligned(l.count, 4)) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
-		MetricEntry& e = table[i];
-		memset(&e, 0, sizeof(e));
-		e.img1 = l.original;
-		e.img2 = l.decoded;
-		e.type1 = (int)l.original_type;
-		e.type2 = (int)l.decoded_type;
-		e.pitch1 = e.pitch2 = l.dim_x;
-		e.stride1 = e.stride2 = (size_t)l.dim_x * l.dim_y;
-		e.dim_x = l.dim_x;
-		e.dim_y = l.dim_y;
-		e.dim_z = l.dim_z;
-		e.block_error = l.block_error;
+		table.push_back(metric_pair(ctx, l.original, l.original_type, l.decoded, l.decoded_type, l.dim_x, l.dim_y, l.dim_z, nullptr, l.block_error));
 		capacities[i] = l.capacity;
 	}
 	const unsigned int bz = ctx->config.block_z > 1 ? ctx->config.block_z : 1;
@@ -2497,28 +2511,19 @@ astcenc_error astcenc_b200_compute_block_metric_device_block_lists(astcenc_conte
 		// (the planner has refused images of 2^32 blocks or more)
 		gather_lists[i] = {lists[i].indices, lists[i].count, lists[i].capacity, table[i].blocks_x * table[i].blocks_y * ((table[i].dim_z + bz - 1) / bz)};
 	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, s, [&]() -> astcenc_error {
-		const size_t table_bytes = table.size() * sizeof(MetricEntry);
-		const size_t maps_bytes = plan.maps.size() * sizeof(MetricMap);
-		const size_t lists_bytes = gather_lists.size() * sizeof(GatherList);
-		astcenc_error r = ensure_buffer(ctx->list, table_bytes + maps_bytes + lists_bytes);
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) -> astcenc_error {
+		TableUpload up;
+		const size_t table_at = up.add(table);
+		const size_t maps_at = up.add(plan.maps);
+		const size_t lists_at = up.add(gather_lists);
+		astcenc_error r = up.send(ctx->list, s);
 		if (r != ASTCENC_SUCCESS) {
 			return r;
 		}
-		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(plan.maps.data()), reinterpret_cast<const uint8_t*>(plan.maps.data()) + maps_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(gather_lists.data()), reinterpret_cast<const uint8_t*>(gather_lists.data()) + lists_bytes);
-		// (from pageable memory: staged by the driver before the call returns)
-		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
 		MetricListArgs a;
-		a.entries = ctx->list.as<const MetricEntry>();
-		a.maps = reinterpret_cast<const MetricMap*>(ctx->list.ptr + table_bytes);
-		a.lists = reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes + maps_bytes);
+		a.entries = up.at<const MetricEntry>(table_at);
+		a.maps = up.at<const MetricMap>(maps_at);
+		a.lists = up.at<const GatherList>(lists_at);
 		a.count = list_count;
 		a.slots = plan.slots;
 		a.bx = ctx->config.block_x;
@@ -2547,40 +2552,31 @@ astcenc_error astcenc_b200_compute_block_errors_device_block_lists(astcenc_conte
 
 // Selection calls (astc_dev_select.cuh): every entry is checked before anything is enqueued; in one scratch turn the table and
 // the pools go up, the pools' histograms are cleared and SELECT_KERNELS kernels run, whatever the number of pools and entries.
-static bool select_aligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
-
 static astcenc_error enqueue_select(astcenc_context* ctx, std::vector<SelectEntry>& table, std::vector<SelectPool>& pools, void* cuda_stream) {
 	if (table.empty()) {
 		return ASTCENC_SUCCESS;
 	}
 	const size_t tiles = plan_select(table, pools);
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, s, [&]() -> astcenc_error {
-		const size_t table_bytes = table.size() * sizeof(SelectEntry);
-		const size_t pool_bytes = pools.size() * sizeof(SelectPool);
-		const size_t hist_bytes = pools.size() * 1024 * sizeof(uint32_t);
-		astcenc_error r = ensure_buffer(ctx->select, table_bytes + pool_bytes + hist_bytes + tiles * 2 * sizeof(uint32_t));
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) -> astcenc_error {
+		// the table and the pools go up; the histograms and the tile counts follow them in the buffer
+		TableUpload up;
+		const size_t table_at = up.add(table);
+		const size_t pools_at = up.add(pools);
+		const size_t hist_at = up.reserve<uint32_t>(pools.size() * 1024);
+		const size_t tiles_at = up.reserve<uint32_t>(tiles * 2);
+		astcenc_error r = up.send(ctx->select, s);
 		if (r != ASTCENC_SUCCESS) {
 			return r;
 		}
-		// the table and the pools in one copy (from pageable memory: staged by the driver before the call returns)
-		std::vector<uint8_t> up(table_bytes + pool_bytes);
-		memcpy(up.data(), table.data(), table_bytes);
-		memcpy(up.data() + table_bytes, pools.data(), pool_bytes);
-		CUDA_TRY(cudaMemcpyAsync(ctx->select.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
-		CUDA_TRY(cudaMemsetAsync(ctx->select.ptr + table_bytes + pool_bytes, 0, hist_bytes, s), return ASTCENC_ERR_BAD_CONTEXT);
+		CUDA_TRY(cudaMemsetAsync(up.at<uint32_t>(hist_at), 0, pools.size() * 1024 * sizeof(uint32_t), s), return ASTCENC_ERR_BAD_CONTEXT);
 		SelectArgs a;
-		a.entries = ctx->select.as<const SelectEntry>();
-		a.pools = reinterpret_cast<const SelectPool*>(ctx->select.ptr + table_bytes);
+		a.entries = up.at<const SelectEntry>(table_at);
+		a.pools = up.at<const SelectPool>(pools_at);
 		a.count = (unsigned int)table.size();
 		a.pool_count = (unsigned int)pools.size();
 		a.tiles = tiles;
-		a.hist = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes + pool_bytes);
-		a.tile_counts = reinterpret_cast<uint32_t*>(ctx->select.ptr + table_bytes + pool_bytes + hist_bytes);
+		a.hist = up.at<uint32_t>(hist_at);
+		a.tile_counts = up.at<uint32_t>(tiles_at);
 		// grid-stride launches of SELECT_WARPS warps per CTA, at least one CTA, so that every call makes the same launches
 		const size_t cap = (size_t)ctx->sm_count * 16;
 		auto grid = [cap](size_t warps) {
@@ -2603,8 +2599,8 @@ static astcenc_error enqueue_select(astcenc_context* ctx, std::vector<SelectEntr
 // indices with a capacity or a pointer not aligned to 4 bytes.
 static bool select_entry(const float* map, unsigned int block_count, const float* weight, float threshold, unsigned int capacity, uint32_t* indices,
                          uint32_t* count, SelectEntry& e) {
-	if (!count || (block_count != 0 && !map) || (capacity != 0 && !indices) || !select_aligned(map) || !select_aligned(weight) ||
-	    !select_aligned(indices) || !select_aligned(count)) {
+	if (!count || (block_count != 0 && !map) || (capacity != 0 && !indices) || !aligned(map, 4) || !aligned(weight, 4) || !aligned(indices, 4) ||
+	    !aligned(count, 4)) {
 		return false;
 	}
 	e.map = map;
@@ -2675,8 +2671,7 @@ astcenc_error astcenc_b200_total_block_maps(astcenc_context* ctx, const astcenc_
 	std::vector<TotalEntry> table(entry_count);
 	for (unsigned int j = 0; j < entry_count; j++) {
 		const astcenc_b200_block_map_total& x = entries[j];
-		if ((x.block_count != 0 && !x.map) || x.limit != x.limit || !select_aligned(x.map) || !select_aligned(x.weight) ||
-		    (reinterpret_cast<uintptr_t>(x.total) & 7) != 0) {
+		if ((x.block_count != 0 && !x.map) || x.limit != x.limit || !aligned(x.map, 4) || !aligned(x.weight, 4) || !aligned(x.total, 8)) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
 		table[j] = {x.map, x.total, x.weight, x.limit, x.block_count, 0, 0};
@@ -2688,25 +2683,21 @@ astcenc_error astcenc_b200_total_block_maps(astcenc_context* ctx, const astcenc_
 	if (table.empty()) {
 		return ASTCENC_SUCCESS;
 	}
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	cudaStream_t s = cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream;
-	return scratch_turn(ctx, s, [&]() -> astcenc_error {
-		const size_t table_bytes = table.size() * sizeof(TotalEntry);      // (a multiple of 8: the partials follow)
-		astcenc_error r = ensure_buffer(ctx->select, table_bytes + ctas * sizeof(double));
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) -> astcenc_error {
+		// the table goes up; the partials follow it in the buffer
+		TableUpload up;
+		const size_t table_at = up.add(table);
+		const size_t partials_at = up.reserve<double>(ctas);
+		astcenc_error r = up.send(ctx->select, s);
 		if (r != ASTCENC_SUCCESS) {
 			return r;
 		}
-		// (from pageable memory: staged by the driver before the call returns)
-		CUDA_TRY(cudaMemcpyAsync(ctx->select.ptr, table.data(), table_bytes, cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
 		TotalArgs a;
-		a.entries = ctx->select.as<const TotalEntry>();
+		a.entries = up.at<const TotalEntry>(table_at);
 		a.count = (unsigned int)table.size();
 		a.rule = (int)rule;
 		a.ctas = ctas;
-		a.partials = reinterpret_cast<double*>(ctx->select.ptr + table_bytes);
+		a.partials = up.at<double>(partials_at);
 		const size_t grid = (ctas + TOTAL_WARPS - 1) / TOTAL_WARPS;      // (at least one CTA, so that every call makes the same launches)
 		astc_map_total_partial_kernel<<<(unsigned int)(grid == 0 ? 1 : grid), TOTAL_WARPS * 32, 0, s>>>(a);
 		astc_map_total_finish_kernel<<<(unsigned int)((table.size() + TOTAL_FINISH_THREADS - 1) / TOTAL_FINISH_THREADS), TOTAL_FINISH_THREADS, 0, s>>>(a);
@@ -2780,43 +2771,34 @@ astcenc_error astcenc_b200_last_timing(astcenc_context* ctx, float* kernel_ms, s
 // is enqueued, in the order include/astcenc.h gives; table_entry gives the block counts. The table (and a list call's lists)
 // go up in one copy and one launch does the call, in one scratch turn.
 static astcenc_error launch_block_info_table(astcenc_context* ctx, const std::vector<GatherImage>& table, const std::vector<GatherList>& lists, size_t total,
-                                             cudaStream_t s) {
-	DeviceGuard guard(ctx->device);
-	if (!guard.ok) {
-		return ASTCENC_ERR_BAD_CONTEXT;
-	}
-	return scratch_turn(ctx, s, [&]() -> astcenc_error {
-		const size_t table_bytes = table.size() * sizeof(GatherImage);
-		const size_t lists_bytes = lists.size() * sizeof(GatherList);
-		astcenc_error r = ensure_buffer(ctx->list, table_bytes + lists_bytes);
+                                             void* cuda_stream) {
+	return device_turn(ctx, cuda_stream, [&](cudaStream_t s) -> astcenc_error {
+		TableUpload up;
+		const size_t table_at = up.add(table);
+		const size_t lists_at = up.add(lists);
+		astcenc_error r = up.send(ctx->list, s);
 		if (r != ASTCENC_SUCCESS) {
 			return r;
 		}
-		std::vector<uint8_t> up(reinterpret_cast<const uint8_t*>(table.data()), reinterpret_cast<const uint8_t*>(table.data()) + table_bytes);
-		up.insert(up.end(), reinterpret_cast<const uint8_t*>(lists.data()), reinterpret_cast<const uint8_t*>(lists.data()) + lists_bytes);
-		// (from pageable memory: staged by the driver before the call returns)
-		CUDA_TRY(cudaMemcpyAsync(ctx->list.ptr, up.data(), up.size(), cudaMemcpyHostToDevice, s), return ASTCENC_ERR_BAD_CONTEXT);
 		const DevImage img{};
 		if (lists.empty()) {
 			const size_t ctas = (total + ASTC_SUMMARY_THREADS - 1) / ASTC_SUMMARY_THREADS;
 			const size_t cap = (size_t)ctx->sm_count * (2048 / ASTC_SUMMARY_THREADS);
 			astc_block_summaries_kernel<<<(unsigned int)(ctas < cap ? ctas : cap), ASTC_SUMMARY_THREADS, ASTC_SMEM_HDR, s>>>(
-			    ctx->tables->bsd, ctx->dcfg, img, ctx->list.as<const GatherImage>(), (unsigned int)table.size(), total);
+			    ctx->tables->bsd, ctx->dcfg, img, up.at<const GatherImage>(table_at), (unsigned int)table.size(), total);
 		} else {
 			const unsigned int warps = ASTC_INFO_LIST_THREADS / 32;
 			const size_t ctas = (total + warps - 1) / warps;
 			const size_t cap = (size_t)ctx->sm_count * 8;
 			astc_block_info_lists_kernel<<<(unsigned int)(ctas < cap ? ctas : cap), ASTC_INFO_LIST_THREADS, ASTC_SMEM_HDR + warps * D_SLICE, s>>>(
-			    ctx->tables->bsd, ctx->dcfg, img, ctx->list.as<const GatherImage>(), reinterpret_cast<const GatherList*>(ctx->list.ptr + table_bytes),
-			    (unsigned int)table.size(), total, block_info_head(ctx));
+			    ctx->tables->bsd, ctx->dcfg, img, up.at<const GatherImage>(table_at), up.at<const GatherList>(lists_at), (unsigned int)table.size(), total,
+			    block_info_head(ctx));
 		}
 		ctx->launches++;
 		CUDA_TRY(cudaGetLastError(), return ASTCENC_ERR_BAD_CONTEXT);
 		return ASTCENC_SUCCESS;
 	});
 }
-
-static bool aligned_to(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 astcenc_error astcenc_b200_get_block_summaries_device_images(astcenc_context* ctx, const astcenc_b200_device_block_summary_image* images,
                                                              unsigned int image_count, void* cuda_stream) {
@@ -2825,7 +2807,7 @@ astcenc_error astcenc_b200_get_block_summaries_device_images(astcenc_context* ct
 	}
 	for (unsigned int i = 0; i < image_count; i++) {
 		const astcenc_b200_device_block_summary_image& im = images[i];
-		if (!im.payload || !im.summaries || !aligned_to(im.summaries, 16) || check_texel_count(im.dim_x, im.dim_y, im.dim_z) != ASTCENC_SUCCESS) {
+		if (!im.payload || !im.summaries || !aligned(im.summaries, 16) || check_texel_count(im.dim_x, im.dim_y, im.dim_z) != ASTCENC_SUCCESS) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
 	}
@@ -2842,7 +2824,7 @@ astcenc_error astcenc_b200_get_block_summaries_device_images(astcenc_context* ct
 	if (blocks == 0) {
 		return ASTCENC_SUCCESS;
 	}
-	return launch_block_info_table(ctx, table, {}, blocks, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream);
+	return launch_block_info_table(ctx, table, {}, blocks, cuda_stream);
 }
 
 astcenc_error astcenc_b200_get_block_info_device_block_lists(astcenc_context* ctx, const astcenc_b200_device_block_info_list* lists, unsigned int list_count,
@@ -2852,35 +2834,26 @@ astcenc_error astcenc_b200_get_block_info_device_block_lists(astcenc_context* ct
 	}
 	for (unsigned int i = 0; i < list_count; i++) {
 		const astcenc_b200_device_block_info_list& l = lists[i];
-		if (!l.payload || (l.capacity != 0 && (!l.indices || !l.count || !l.infos)) || !aligned_to(l.indices, 4) || !aligned_to(l.count, 4) ||
-		    !aligned_to(l.infos, 4) || check_texel_count(l.dim_x, l.dim_y, l.dim_z) != ASTCENC_SUCCESS) {
+		if (!l.payload || (l.capacity != 0 && (!l.indices || !l.count || !l.infos)) || !aligned(l.indices, 4) || !aligned(l.count, 4) ||
+		    !aligned(l.infos, 4) || check_texel_count(l.dim_x, l.dim_y, l.dim_z) != ASTCENC_SUCCESS) {
 			return ASTCENC_ERR_BAD_PARAM;
 		}
 	}
-	std::vector<GatherImage> table;
-	std::vector<GatherList> gather_lists;
-	size_t slots = 0;
+	ListTable t;
 	for (unsigned int i = 0; i < list_count; i++) {
 		const astcenc_b200_device_block_info_list& l = lists[i];
 		GatherImage e;
 		size_t blocks = 0;
 		// (the payload is read, never written; data holds the structs)
 		astcenc_error status = table_entry(ctx, ASTCENC_TYPE_U8, l.dim_x, l.dim_y, l.dim_z, l.infos, const_cast<uint8_t*>(l.payload), blocks, e);
-		if (status == ASTCENC_SUCCESS && l.capacity > SIZE_MAX - slots) {
-			status = ASTCENC_ERR_BAD_PARAM;
-		}
+		const GatherList list{l.indices, l.count, l.capacity, (unsigned int)blocks};
+		if (status == ASTCENC_SUCCESS) status = t.add(e, &list, l.capacity);
 		if (status != ASTCENC_SUCCESS) {
 			return status;
 		}
-		if (l.capacity != 0) {
-			e.first = slots;
-			table.push_back(e);
-			gather_lists.push_back({l.indices, l.count, l.capacity, (unsigned int)blocks});
-			slots += l.capacity;
-		}
 	}
-	if (slots == 0) {
+	if (t.slots == 0) {
 		return ASTCENC_SUCCESS;
 	}
-	return launch_block_info_table(ctx, table, gather_lists, slots, cuda_stream ? static_cast<cudaStream_t>(cuda_stream) : ctx->stream);
+	return launch_block_info_table(ctx, t.table, t.lists, t.slots, cuda_stream);
 }
